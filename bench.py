@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- mapped query Gbp/s of the B200 mapping hot path (BASELINE.json metric).
+"""bench.py -- mapped query Gbp/s of the H100 mapping hot path (BASELINE.json metric).
 
 Workload (BASELINE.json configs[1]): 1 M synthetic ONT-like reads x 10 kb (per-read error ~ U[2 %,14 %],
 sub:ins:del 4:3:3) against a 3 Gbp uniform-random reference, MashMap defaults `-s 5000 --pi 85`
@@ -75,7 +75,13 @@ def parse_args():
                     "(oracle/_ref/libmm_ref.so: its own index build from FASTA, its own mapModule); 'port' = the oracle restatement on the "
                     "product's index content; 'auto' = real when the library is there")
     ap.add_argument("--as-rank", type=int, default=-1, help="debug: generate the reads rank R of a multi-GPU run would get (read seed 2 + R)")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="after the timed steps, write what the last step computed "
+                    "(segment results, L1 candidates, L2 loci of the resident path; mappings of the e2e path) as DIR/<name>.npy, "
+                    "float64, for a fixed seeded sample of the queries (see dump_outputs)")
+    a = ap.parse_args()
+    if a.steps < 1:
+        ap.error("--steps must be at least 1")
+    return a
 
 
 class ClockSampler:
@@ -158,7 +164,7 @@ def measured_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3)"
 
 
 def roofline_traffic():
@@ -173,7 +179,7 @@ def roofline_traffic():
 
 
 def issue_peak():
-    """measured INT32 issue rates (mashmap_b200/mm_issue_peak on this pool's B200), if committed"""
+    """measured INT32 issue rates (mashmap_b200/mm_issue_peak on an H100), if committed"""
     p = os.path.join(ROOT, "profiles", "issue_peak.json")
     if os.path.exists(p):
         try:
@@ -442,6 +448,7 @@ def gpu_arm(args):
         t_index = time.time()  # index_build_seconds is the product's side only
     want_port = want_cpu and not cpu_real
     ist = None
+    torch.cuda.empty_cache()  # the generators' cached blocks: the index builder sizes its grid to the free memory
     if rank == 0:  # rank 0 builds the index on its GPU; the other ranks receive the image
         ist = build_index_on_device(args, cfg, wl, ctx, keep_lookup=want_port)
     host_index_arrays = ctx.index_download() if (rank == 0 and want_port) else None
@@ -543,6 +550,8 @@ def gpu_arm(args):
 
     # ---- correctness of what was timed ----
     res = bm.results()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, seg_res, cands, loci, res, n_local, wl["first_counter"])
     acc = _accuracy(res, wl["truth"], wl["contig_len"], wl["first_counter"], wl["lo"]) if wl["truth"] is not None else None
     sharded_check = None
     if strong and world > 1 and rank == 0 and one_to_one:
@@ -664,6 +673,60 @@ def algorithmic_bytes_l1_l2(seg_res, cands, loci, idx_seq, idx_wpos, seg_len):
             "index_entries_scanned": n_scan, "loci": int(len(loci))}
 
 
+DUMP_SAMPLE_SEGMENTS = 1 << 17  # fragments whose records are written by --dump-outputs (all of them when the step has fewer)
+DUMP_SAMPLE_QUERIES = 1 << 16   # queries whose final mappings are written
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def _u64_columns(a):
+    """uint64 as two exact float64 columns (high and low 32 bits)"""
+    a = a.astype(np.uint64)
+    return [(a >> np.uint64(32)).astype(np.float64), (a & np.uint64(0xFFFFFFFF)).astype(np.float64)]
+
+
+def dump_outputs(out_dir, seg_res, cands, loci, mappings, n_queries, first_counter):
+    """What one step of each timed path hands its caller, for a fixed seeded sample of the step (the same sample for the
+    same arguments), as float64 arrays that compare exactly between two builds:
+      segments.npy   [fragment index, sketch_max_hash hi, lo, sketch_raw_count, sketch_size, n_points, minimum_hits,
+                      best_intersection, n_candidates]                                           (resident path, K1-K3)
+      candidates.npy [fragment index, seqId, rangeStartPos, rangeEndPos, intersectionSize, n_loci]   (K2)
+      loci.npy       [fragment index, candidate rank in its fragment, seqId, meanOptimalPos, optimalStart, optimalEnd,
+                      sharedSketchSize, strand]                                                   (K3)
+      mappings.npy   the e2e path's final mappings of the sampled queries (BatchMapper.results columns), sorted
+    Where a fragment's candidates and loci sit in the batch-wide arrays depends on the order the CTAs reserved them in, so
+    they are written fragment by fragment in the order the kernels produced them within a fragment."""
+    os.makedirs(out_dir, exist_ok=True)
+    rng = np.random.default_rng(12345)
+    n = len(seg_res)
+    pick = np.arange(n) if n <= DUMP_SAMPLE_SEGMENTS else np.sort(rng.choice(n, DUMP_SAMPLE_SEGMENTS, replace=False))
+    sr = seg_res[pick]
+    segs_out = np.column_stack([pick.astype(np.float64)] + _u64_columns(sr["sketch_max_hash"]) +
+                               [sr[f].astype(np.float64) for f in ("sketch_raw_count", "sketch_size", "n_points", "minimum_hits",
+                                                                   "best_intersection", "n_candidates")])
+    nc = sr["n_candidates"].astype(np.int64)
+    ci = np.repeat(sr["first_candidate"].astype(np.int64), nc) + (np.arange(int(nc.sum())) - np.repeat(np.cumsum(nc) - nc, nc))
+    c = cands[ci]
+    cand_seg = np.repeat(pick, nc).astype(np.float64)
+    cands_out = np.column_stack([cand_seg] + [c[f].astype(np.float64) for f in ("seqId", "rangeStartPos", "rangeEndPos", "intersectionSize", "n_loci")])
+    cand_rank = (np.arange(len(c)) - np.repeat(np.cumsum(nc) - nc, nc)).astype(np.float64)
+    nl = c["n_loci"].astype(np.int64)
+    li = np.repeat(c["first_locus"].astype(np.int64), nl) + (np.arange(int(nl.sum())) - np.repeat(np.cumsum(nl) - nl, nl))
+    lo = loci[li]
+    loci_out = np.column_stack([np.repeat(cand_seg, nl), np.repeat(cand_rank, nl)] +
+                               [lo[f].astype(np.float64) for f in ("seqId", "meanOptimalPos", "optimalStart", "optimalEnd", "sharedSketchSize", "strand")])
+    q = np.arange(n_queries) if n_queries <= DUMP_SAMPLE_QUERIES else np.sort(rng.choice(n_queries, DUMP_SAMPLE_QUERIES, replace=False))
+    m = mappings[np.isin(mappings[:, 0].astype(np.int64) - first_counter, q)] if len(mappings) else mappings
+    m = m[np.lexsort(tuple(m[:, c_] for c_ in range(m.shape[1] - 1, -1, -1)))] if len(m) else m
+    arrays = {"segments": segs_out, "candidates": cands_out.reshape(-1, 6), "loci": loci_out.reshape(-1, 8),
+              "mappings": m.astype(np.float64).reshape(-1, mappings.shape[1] if mappings.ndim == 2 else 10)}
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_LIMIT_BYTES:
+        raise SystemExit(f"--dump-outputs: {total} bytes exceed the {DUMP_LIMIT_BYTES}-byte limit")
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.ascontiguousarray(a))
+    log(f"outputs of the last step written to {out_dir}: " + ", ".join(f"{k} {v.shape}" for k, v in arrays.items()))
+
+
 def l1_l2_rooflines(ctx, seg_res, cands, loci, seg_len, k2_ms, k3_ms, peak):
     """roofline entries of K2 and K3 (VERDICT r1 weak 4): algorithmic bytes counted on the real configuration / stage time.
     Needs a host copy of the index records (6 GB at 3 Gbp, a few seconds, outside every timed region); any failure only
@@ -693,7 +756,7 @@ def _instruction_roofline(n_segs, seg, k1_ms, clocks, sm_count):
     hashes per position. What K1 loses against it is everything that is not hashing."""
     positions = n_segs * (seg - K + 1)
     achieved = positions / (k1_ms * 1e-3) / 1e9
-    mhz = (clocks or {}).get("sm_mhz") or 1965.0
+    mhz = (clocks or {}).get("sm_mhz") or 1980.0  # H100 SXM maximum SM clock
     ip = issue_peak() or {}
     per_clk = ip.get("hash19_per_clk_per_sm")
     if per_clk:

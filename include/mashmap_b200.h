@@ -1,5 +1,5 @@
 /*
- * mashmap_b200.h -- C ABI of the B200-native MashMap mapping hot path.
+ * mashmap_b200.h -- C ABI of the H100-native MashMap mapping hot path.
  *
  * The reference (marbl/MashMap v3.1.3) has no FFI/plugin boundary: its hot path is a set of
  * C++ member functions called once per query fragment from skch::Map::mapSingleQueryFrag
@@ -9,7 +9,7 @@
  * INTEGRATION.md shows the reference-side call sites (skch::Sketch / skch::Map) rewritten on top of it.
  *
  * All functions return MM_OK (0) or a negative MM_E* code; mm_last_error() gives the text.
- * There is NO CPU fallback: every compute entry point fails with MM_ENODEVICE when no sm_100
+ * There is NO CPU fallback: every compute entry point fails with MM_ENODEVICE when no sm_90
  * device is usable.
  */
 #ifndef MASHMAP_B200_H

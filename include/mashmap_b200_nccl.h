@@ -1,5 +1,5 @@
 /*
- * mashmap_b200_nccl.h -- multi-GPU entry points of the B200 mapping hot path (libmashmap_nccl.so; links NCCL).
+ * mashmap_b200_nccl.h -- multi-GPU entry points of the H100 mapping hot path (libmashmap_nccl.so; links NCCL).
  *
  * The reference (marbl/MashMap v3.1.3) is a single-process CPU program: there is no collective, no device and no
  * rank anywhere in it (SURVEY section 0, fact 5). What it has instead is ONE in-memory index (skch::Sketch, reference

@@ -6,7 +6,7 @@
  * hash uses, and prints warp instructions per clock per SM. bench.py reads the JSON line (profiles/issue_peak.json) for
  * the instruction roofline of K1.
  *
- * build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o mm_issue_peak mm_issue_peak.cu
+ * build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o mm_issue_peak mm_issue_peak.cu
  */
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -3,7 +3,7 @@
  *
  * Owns the device context: the index blob (one arena, see mm_internal.h), the per-batch buffers,
  * the stream and the stage timers, and drives K1 (mm_sketch.cu) -> K2 (mm_l1.cu) -> K3 (mm_l2.cu).
- * There is no CPU implementation behind any entry point: without a usable sm_100 device every call
+ * There is no CPU implementation behind any entry point: without a usable sm_90 device every call
  * fails with MM_ENODEVICE.
  */
 #include <algorithm>
@@ -608,7 +608,8 @@ int mm_ctx_create(int device, const mm_params *params, mm_ctx **out)
   if (device < 0 || device >= n_dev) return fail(nullptr, MM_ENODEVICE, "device %d out of range (%d devices)", device, n_dev);
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return fail(nullptr, MM_ENODEVICE, "cannot query device");
-  if (prop.major != 10) return fail(nullptr, MM_ENODEVICE, "device %d is sm_%d%d; this build is sm_100a only", device, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(nullptr, MM_ENODEVICE, "device %d is sm_%d%d; this build is sm_90a only", device, prop.major, prop.minor);
   if (int rc = mm_params_check(params)) return rc;
   mm_ctx *c = new mm_ctx();
   c->device = device;

@@ -520,10 +520,20 @@ int mm_build_index_device(const mm_params &p, const uint8_t *d_seq, const uint64
     if (const char *e = getenv("MM_INDEX_TPSM")) tpsm = std::max(128, atoi(e) / 128 * 128);
     uint32_t threads = (uint32_t)sm_count * (uint32_t)tpsm;
     if (threads > n_chunks) threads = (n_chunks + 127) / 128 * 128;
+    const uint32_t rec_cap = (uint32_t)(chunk_len / 4 + s + 64);
+    { /* one slab per machine (~0.4 MB at -s 5000): at 3 Gbp the slabs of a full grid and the chunks' record buffers
+       * together exceed an 80 GB device next to the caller's data, so the grid shrinks to the memory that is free
+       * (a smaller grid only scans more chunks per thread) */
+      size_t free_b = 0, total_b = 0;
+      CE(cudaMemGetInfo(&free_b, &total_b));
+      const uint64_t fixed = (uint64_t)n_chunks * rec_cap * sizeof(wm_record) + (uint64_t)n_chunks * wm_mem_cap(s) * sizeof(wb_open) + (1ULL << 30);
+      const uint64_t room = free_b > fixed ? (free_b - fixed) / 10 * 8 : 0;
+      const uint64_t fit = room / L.bytes / 128 * 128;
+      if (fit < threads) threads = (uint32_t)std::max<uint64_t>(fit, 128);
+    }
     const uint32_t grid = threads / 128;
     unsigned char *slabs = nullptr;
     CE(dv.alloc(slabs, (uint64_t)threads * L.bytes));
-    const uint32_t rec_cap = (uint32_t)(chunk_len / 4 + s + 64);
     wm_record *rec = nullptr;
     CE(dv.alloc(rec, (uint64_t)n_chunks * rec_cap));
     wb_chunk_out *d_outs = nullptr;

@@ -1,15 +1,15 @@
 """The product's option parser fills skch::Parameters exactly as the reference's parseandSave does
 (reference src/map/include/parseCmdArgs.hpp:257-659: defaults, automatic sketch size from the file size, --dense,
-filter modes, chaining / block-length defaults, skip-self when no query is given ...). CPU only."""
+filter modes, chaining / block-length defaults, skip-self when no query is given ...). CPU only. Where the reference is
+not built, against the parameters it produced, stored in tests/golden (golden_ref.py)."""
 import os
 
 import pytest
 
 import datasets
+import golden_ref
 import refh
 from mashmap_b200 import hostlib
-
-pytestmark = pytest.mark.skipif(not refh.available(), reason="oracle/_ref not built")
 
 OPTION_SETS = [
     [],
@@ -31,20 +31,31 @@ def d(workdir):
     return datasets.make_panel_set(workdir, tag="args", n_strains=2, chrom_len=40_000)
 
 
+def reference_parameters(args, d):
+    """skch::Parameters of the reference for a command line, field by field (computed, or stored)"""
+    key = golden_ref.key_of(args, d)
+    if not refh.available():
+        return golden_ref.get("parameters", key)
+    R = refh.RefSession(args)
+    try:
+        got = [getattr(R.p, name) for name, _ in refh.OrcParams._fields_]
+    finally:
+        R.close()
+    golden_ref.check_stored("parameters", key, got)
+    return got
+
+
 @pytest.mark.parametrize("opts", OPTION_SETS, ids=lambda o: " ".join(o) or "defaults")
 @pytest.mark.parametrize("with_query", [True, False])
 def test_parameters_equal_reference(d, opts, with_query):
     args = ["-r", d["ref"]] + (["-q", d["qry"]] if with_query else []) + ["-t", "2"] + opts
-    R = refh.RefSession(args)
-    try:
-        ours = hostlib.HostIndex.from_cli(args)
-        p = ours.params_into(refh.OrcParams())
-        for name, _ in refh.OrcParams._fields_:
-            a, b = getattr(R.p, name), getattr(p, name)
-            assert a == b, (name, a, b, args)
-        ours.close()
-    finally:
-        R.close()
+    want = reference_parameters(args, d)
+    ours = hostlib.HostIndex.from_cli(args)
+    p = ours.params_into(refh.OrcParams())
+    for (name, _), a in zip(refh.OrcParams._fields_, want):
+        b = getattr(p, name)
+        assert a == b, (name, a, b, args)
+    ours.close()
 
 
 @pytest.mark.parametrize("size", [2**31 - 1000, 2**31 + 1000, 3_100_000_000, 5_000_000_000, 2**32 + 4096])
@@ -57,9 +68,16 @@ def test_reference_size_wraps_like_the_reference(tmp_path, size):
         fh.write(b">c\nACGT\n")
         fh.truncate(size)
     args = ["-r", str(f), "-q", str(f), "-s", "5000", "--pi", "85"]
-    ref = refh.parse_only(args)
     ours = hostlib.HostIndex.params_from_cli(args)
     p = ours.params_into(refh.OrcParams())
     ours.close()
-    assert p.referenceSize == ref.referenceSize
-    assert p.sketchSize == ref.sketchSize
+    assert [p.referenceSize, p.sketchSize] == reference_size_and_sketch(args, size)
+
+
+def reference_size_and_sketch(args, size):
+    if not refh.available():
+        return golden_ref.get("reference_size", str(size))
+    ref = refh.parse_only(args)
+    got = [ref.referenceSize, ref.sketchSize]
+    golden_ref.check_stored("reference_size", str(size), got)
+    return got

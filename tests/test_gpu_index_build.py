@@ -2,20 +2,21 @@
 (oracle/_ref harness: Sketch::build / index / computeFreqHist / dropFreqSeedSet): minmerIndex after the frequent-seed drop,
 the lookup keys / interval points, the frequent-seed flags and the threshold. Records must be the reference's; the one
 permitted difference is the order of records with equal (seqId, wpos, wpos_end), which the reference leaves to std::sort's
-unspecified tie order (commonFunc.hpp:558) and the device builder keeps in emission order (DESIGN.md)."""
+unspecified tie order (commonFunc.hpp:558) and the device builder keeps in emission order (DESIGN.md). Where the reference
+is not built, the device index is compared with the reference's stored digests (golden_ref.py)."""
 import os
 
 import numpy as np
 import pytest
 
 import datasets
+import golden_ref
 import refh
 from conftest import have_gpu
 from mashmap_b200 import synth
 
 pytestmark = [pytest.mark.gpu,
-              pytest.mark.skipif(not have_gpu(), reason="no GPU"),
-              pytest.mark.skipif(not refh.available(), reason="oracle/_ref not built")]
+              pytest.mark.skipif(not have_gpu(), reason="no GPU")]
 
 
 def canon_minmers(mi):
@@ -52,7 +53,10 @@ def build_and_compare(d, args, chunk=None, monkeypatch=None, expect_fixed=None):
 
     if chunk is not None:
         monkeypatch.setenv("MM_INDEX_CHUNK", str(chunk))
+    if not refh.available():
+        return build_and_compare_stored(d, args, expect_fixed)
     R = refh.RefSession(args)
+    golden_ref.check_stored("sessions", golden_ref.key_of(args, d), golden_ref.session_digests(R))
     try:
         ctx = capi.Context(kmer_size=R.p.kmerSize, seg_length=R.p.segLength, sketch_size=R.p.sketchSize)
         seqs = np.concatenate(d["genome"]).astype(np.uint8)
@@ -92,6 +96,27 @@ def build_and_compare(d, args, chunk=None, monkeypatch=None, expect_fixed=None):
         return st
     finally:
         R.close()
+
+
+def build_and_compare_stored(d, args, expect_fixed):
+    """the device index against the digests of the reference's index for the same command line"""
+    from mashmap_b200 import capi
+
+    want = golden_ref.get("sessions", golden_ref.key_of(args, d))
+    k, seg, s, pi, _ = want["params"]
+    kmer_pct = float(args[args.index("--kmerThreshold") + 1]) if "--kmerThreshold" in args else 0.001
+    ctx = capi.Context(kmer_size=k, seg_length=seg, sketch_size=s)
+    seqs = np.concatenate(d["genome"]).astype(np.uint8)
+    offs = np.zeros(len(d["genome"]) + 1, dtype=np.uint64)
+    offs[1:] = np.cumsum([len(c) for c in d["genome"]])
+    st = ctx.index_build(seqs, offs, kmer_pct_threshold=kmer_pct, keep_lookup=True)
+    print("device index:", st)
+    mi, keys, ko, pts, fr = ctx.index_download()
+    assert golden_ref.index_digests(mi, keys, ko, pts, fr, st["freq_threshold"]) == want["index"]
+    if expect_fixed is not None:
+        assert (st["n_fixed_chunks"] > 0) == expect_fixed, st
+    ctx.close()
+    return st
 
 
 def test_index_random_genome(workdir, monkeypatch):
@@ -140,6 +165,9 @@ def test_index_degenerate_contigs(workdir, monkeypatch, w, s, k):
     for f in ("hash", "wpos", "wpos_end", "seqId", "strand"):
         assert np.array_equal(mi[f], want[f]), f
     # and against the reference itself wherever its order is defined: the records outside tie groups
+    if not refh.available():
+        ctx.close()
+        return
     exact = np.concatenate([refh.add_minmers(g, k, w, s, seq_id=i) for i, g in enumerate(genome)])
     def untied(a):
         key = np.stack([a["seqId"].astype(np.int64), a["wpos"].astype(np.int64), a["wpos_end"].astype(np.int64)], axis=1)

@@ -1,17 +1,42 @@
 """GPU parity, stage by stage, through the C ABI, against the UNMODIFIED reference (oracle/_ref harness):
 K1 sketch == CommonFunc::sketchSequence, K2 candidates == doL1Mapping, K3 loci == computeL2MappedRegions.
-Bit-exact (integer work)."""
+Bit-exact (integer work). Where the reference is not built, against its results stored in tests/golden (golden_ref.py)."""
 import numpy as np
 import pytest
 
 import datasets
+import golden_ref
 import refh
 from conftest import have_gpu
 from mashmap_b200 import synth
 
 pytestmark = [pytest.mark.gpu,
-              pytest.mark.skipif(not have_gpu(), reason="no GPU"),
-              pytest.mark.skipif(not refh.available(), reason="oracle/_ref not built")]
+              pytest.mark.skipif(not have_gpu(), reason="no GPU")]
+
+
+def open_session(args, d):
+    """the reference's Sketch + Map for a command line, or, without the reference, the product's host index checked
+    against the reference's stored digests"""
+    key = golden_ref.key_of(args, d)
+    if refh.available():
+        R = refh.RefSession(args)
+        golden_ref.check_stored("sessions", key, golden_ref.session_digests(R))
+    else:
+        R = golden_ref.ProductSession(args)
+        assert golden_ref.session_digests(R) == golden_ref.get("sessions", key)
+        R.contig_len = np.array([len(c) for c in d["genome"]], dtype=np.int32)
+        R.contig_names = list(d["names"])
+    R.key = key
+    return R
+
+
+def reference_sketch_digests(section, key, seqs, k, s, seq_ids):
+    """per sequence: the digest of the reference's sketchSequence (computed, or stored)"""
+    if refh.available():
+        got = [golden_ref.sketch_digest(refh.sketch_sequence(q, k, s, seq_id=i)) for q, i in zip(seqs, seq_ids)]
+        golden_ref.check_stored(section, key, got)
+        return got
+    return golden_ref.get(section, key)
 
 
 def build_segments(d, seg_length, k, name_ids=None):
@@ -38,13 +63,33 @@ def upload_reference_index(ctx, R):
     ctx.tables_upload(R.cutoffs(), R.min_hits_table())
 
 
+def device_fragment_digest(i, seg_res, cands, loci, dev_sketch, dev_count):
+    sr = seg_res[i]
+    c = cands[sr["first_candidate"] : sr["first_candidate"] + sr["n_candidates"]]
+    l2 = [loci[x["first_locus"] : x["first_locus"] + x["n_loci"]] for x in c]
+    return golden_ref.fragment_digest(dev_sketch[i][: dev_count[i]], int(sr["sketch_size"]), int(sr["n_points"]), c, l2)
+
+
 def compare_stages(ctx, R, d, ridx, start, length, seg_res, cands, loci, dev_sketch, dev_count, max_report=10, diag=None):
     bad = []
     n_cmp = 0
+    if not isinstance(R, refh.RefSession):  # the reference's stored per-fragment digests
+        want = golden_ref.get("fragments", R.key)
+        assert len(want) == len(ridx)
+        for i in range(len(ridx)):
+            if device_fragment_digest(i, seg_res, cands, loci, dev_sketch, dev_count) != want[i]:
+                bad.append((i, "fragment digest"))
+        n_cmp = len(cands)
+        for b in bad[:max_report]:
+            print("MISMATCH", b)
+        print(f"segments={len(ridx)} candidates={n_cmp} mismatches={len(bad)} (stored reference digests)")
+        return bad
+    ref_digests = []
     for i in range(len(ridx)):
         r = d["reads"][ridx[i]]
         seg = r[start[i] : start[i] + length[i]]
         o = R.map_fragment(d["rnames"][ridx[i]], seg, full_len=len(r), seq_counter=int(ridx[i]))
+        ref_digests.append(golden_ref.reference_fragment_digest(o))
         sr = seg_res[i]
         # sketch after frequent-seed removal
         rs = o["sketch"]
@@ -80,6 +125,7 @@ def compare_stages(ctx, R, d, ridx, start, length, seg_res, cands, loci, dev_ske
     for b in bad[:max_report]:
         print("MISMATCH", b)
     print(f"segments={len(ridx)} candidates_compared={n_cmp} mismatches={len(bad)}")
+    golden_ref.check_stored("fragments", R.key, ref_digests)
     return bad
 
 
@@ -105,28 +151,22 @@ def test_sketch_matches_reference(random_set, k, s, mode, monkeypatch):
     ctx = capi.Context(kmer_size=k, seg_length=5000, sketch_size=s)
     bases, segs, ridx, start, length = build_segments(d, 5000, k)
     out, cnt = ctx.sketch_segments(bases, segs)
+    want = reference_sketch_digests("sketch_random_set", f"k{k} s{s}", [d["reads"][ridx[i]][start[i] : start[i] + length[i]]
+                                    for i in range(len(segs))], k, s, [int(x) for x in ridx])
     bad = 0
     for i in range(len(segs)):
-        seg = d["reads"][ridx[i]][start[i] : start[i] + length[i]]
-        ref = refh.sketch_sequence(seg, k, s, seq_id=int(ridx[i]))
         dev = out[i][: cnt[i]]
-        ok = len(ref) == len(dev) and all(np.array_equal(ref[f], dev[f]) for f in ("hash", "wpos", "wpos_end", "seqId", "strand"))
+        ok = golden_ref.sketch_digest(dev) == want[i] and np.all(dev["seqId"] == ridx[i])
         if not ok:
             bad += 1
             if bad <= 5:
-                print("sketch mismatch seg", i, "len", length[i], "ref n", len(ref), "dev n", len(dev))
-                if len(ref) and len(dev):
-                    print(ref[:3], dev[:3])
+                print("sketch mismatch seg", i, "len", length[i], "dev n", len(dev))
     assert bad == 0
     ctx.close()
 
 
-def test_sketch_degenerate_inputs():
-    """all-N, low-complexity (fewer than s distinct k-mers), tandem repeats, tiny and ragged segments"""
-    from mashmap_b200 import capi
-
+def degenerate_sequences():
     rng = np.random.default_rng(5)
-    k, s, L = 19, 100, 5000
     seqs = [np.full(5000, ord("N"), np.uint8), np.full(5000, ord("A"), np.uint8),
             np.tile(np.frombuffer(b"ACGTTGCAAG", np.uint8), 500), np.tile(synth.random_sequence(300, rng), 17)[:5000],
             synth.random_sequence(19, rng), synth.random_sequence(18, rng), synth.random_sequence(57, rng),
@@ -136,6 +176,15 @@ def test_sketch_degenerate_inputs():
     seqs.append(mixed)
     pal = synth.random_sequence(2500, rng)
     seqs.append(np.concatenate([pal, synth.revcomp(pal)]))  # every k-mer occurs on both strands -> vote sums of 0
+    return seqs
+
+
+def test_sketch_degenerate_inputs():
+    """all-N, low-complexity (fewer than s distinct k-mers), tandem repeats, tiny and ragged segments"""
+    from mashmap_b200 import capi
+
+    k, s, L = 19, 100, 5000
+    seqs = degenerate_sequences()
     ctx = capi.Context(kmer_size=k, seg_length=L, sketch_size=s)
     segs = np.zeros(len(seqs), dtype=capi.segment_dtype)
     off = 0
@@ -143,12 +192,9 @@ def test_sketch_degenerate_inputs():
         segs[i]["offset"] = off; segs[i]["length"] = len(q); segs[i]["seq_counter"] = i; segs[i]["name_id"] = -1
         off += len(q)
     out, cnt = ctx.sketch_segments(np.concatenate(seqs), segs)
+    want = reference_sketch_digests("sketch_degenerate", f"k{k} s{s}", seqs, k, s, list(range(len(seqs))))
     for i, q in enumerate(seqs):
-        ref = refh.sketch_sequence(q, k, s, seq_id=i)
-        dev = out[i][: cnt[i]]
-        assert len(ref) == len(dev), (i, len(ref), len(dev))
-        for f in ("hash", "wpos", "wpos_end", "strand"):
-            assert np.array_equal(ref[f], dev[f]), (i, f)
+        assert golden_ref.sketch_digest(out[i], cnt[i]) == want[i], i
     # homopolymers, tandem repeats, all-N, fewer than s distinct k-mers: the fast kernel must have handed them over
     dg = ctx.diag()
     print("rare paths taken:", dg)
@@ -171,7 +217,7 @@ def run_stage_parity(d, args, seg_length, expect_diag=(), expect_freq_seeds=Fals
     expect_freq_seeds: the reference must have flagged frequent seeds and some query sketch must have lost hashes to them"""
     from mashmap_b200 import capi
 
-    R = refh.RefSession(args)
+    R = open_session(args, d)
     try:
         ctx = capi.Context(kmer_size=R.p.kmerSize, seg_length=R.p.segLength, sketch_size=R.p.sketchSize,
                            stage1_topani_filter=bool(R.p.stage1_topANI_filter), **ctx_kw)
@@ -191,7 +237,7 @@ def run_stage_parity(d, args, seg_length, expect_diag=(), expect_freq_seeds=Fals
             sr1 = seg_res[i]
             c1 = cands[sr1["first_candidate"] : sr1["first_candidate"] + sr1["n_candidates"]]
             print("   first (host-buffer) call gave", c1[["seqId", "rangeStartPos", "rangeEndPos", "intersectionSize"]].tolist())
-            if oracle_py.available():
+            if oracle_py.available() and isinstance(R, refh.RefSession):
                 O = oracle_py.Oracle(params=R.p)
                 idx = R.index()
                 keys, offs, pts, fr = R.lookup()
@@ -248,7 +294,7 @@ def test_packed_input_equals_text_input(random_set):
     from mashmap_b200 import capi
 
     d = random_set
-    R = refh.RefSession(["-r", d["ref"], "-q", d["qry"], "-s", "5000", "--pi", "85", "-t", "4"])
+    R = open_session(["-r", d["ref"], "-q", d["qry"], "-s", "5000", "--pi", "85", "-t", "4"], d)
     try:
         ctx = capi.Context(kmer_size=R.p.kmerSize, seg_length=R.p.segLength, sketch_size=R.p.sketchSize)
         upload_reference_index(ctx, R)
@@ -282,24 +328,24 @@ def test_packed_input_equals_text_input(random_set):
         R.close()
 
 
+def every_k_subset(d):
+    return dict(reads=d["reads"][:6] + d["reads"][-5:], rnames=d["rnames"][:6] + d["rnames"][-5:])
+
+
 @pytest.mark.parametrize("k", list(range(8, 33)))
 def test_sketch_every_kmer_size(random_set, k):
     """the reference accepts any -k (parseCmdArgs.hpp:435-443); every k-mer length from 8 to 32 is compiled in"""
     from mashmap_b200 import capi
 
-    d = random_set
     s = 60
     ctx = capi.Context(kmer_size=k, seg_length=3000, sketch_size=s)
-    sub = dict(reads=d["reads"][:6] + d["reads"][-5:], rnames=d["rnames"][:6] + d["rnames"][-5:])
+    sub = every_k_subset(random_set)
     bases, segs, ridx, start, length = build_segments(sub, 3000, k)
     out, cnt = ctx.sketch_segments(bases, segs)
+    want = reference_sketch_digests("sketch_every_k", f"k{k} s{s}", [sub["reads"][ridx[i]][start[i] : start[i] + length[i]]
+                                    for i in range(len(segs))], k, s, [int(x) for x in ridx])
     for i in range(len(segs)):
-        seg = sub["reads"][ridx[i]][start[i] : start[i] + length[i]]
-        ref = refh.sketch_sequence(seg, k, s, seq_id=int(ridx[i]))
-        dev = out[i][: cnt[i]]
-        assert len(ref) == len(dev), (k, i, len(ref), len(dev))
-        for f in ("hash", "wpos", "wpos_end", "strand"):
-            assert np.array_equal(ref[f], dev[f]), (k, i, f)
+        assert golden_ref.sketch_digest(out[i], cnt[i]) == want[i], (k, i)
     ctx.close()
 
 
