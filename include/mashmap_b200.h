@@ -98,10 +98,14 @@ typedef struct mm_params {
   int32_t _reserved[9];
 } mm_params;
 
-/* One query fragment = one call of mapSingleQueryFrag in the reference (computeMap.hpp:610-671). */
+/* One query fragment = one call of mapSingleQueryFrag in the reference (computeMap.hpp:587-671). A fragment is normally at
+ * most seg_length long; a longer one is a whole query mapped unsplit (--noSplit, :587-607) with windowLen = length -
+ * seg_length (:933, :1306), up to length - kmer_size + 1 < 2^30 k-mer positions (the reference computes
+ * (length - k + 1) * 2 in an int, :831). Results of such a fragment have the same layout (sketch_size slots, candidates,
+ * loci); MM_DIAG_LONG_FRAGMENTS counts them. */
 typedef struct mm_segment {
   uint64_t offset;      /* byte offset of the fragment in the batch's base buffer                  */
-  int32_t length;       /* Q.len, kmer_size <= length <= seg_length                                */
+  int32_t length;       /* Q.len, kmer_size <= length (<= seg_length unless the query is unsplit)  */
   int32_t seq_counter;  /* Q.seqCounter (query sequence number; lower_triangular, :893)            */
   int32_t name_id;      /* id of the reference contig NAME equal to Q.seqName, or -1 (skip_self)   */
   int32_t ref_group;    /* Q.refGroup (getRefGroup, computeMap.hpp:164-177), or -1                 */
@@ -131,6 +135,7 @@ uint64_t mm_kernel_launches(const mm_ctx *ctx);
 #define MM_DIAG_L2_GENERAL_CANDS 3 /* candidates redone by the general L2 kernel (more loci than the fixed slots / counter range) */
 #define MM_DIAG_L2_LOCI_REGROW 4   /* L2 re-runs because the locus buffer was too small                               */
 #define MM_DIAG_SKETCH_GENERAL_SEGMENTS 5 /* segments the fast sketch kernel handed to the general one (repeats, N-rich ...) */
+#define MM_DIAG_LONG_FRAGMENTS 6   /* fragments longer than seg_length (windowLen > 0) sketched / mapped               */
 int mm_ctx_diag(const mm_ctx *ctx, uint64_t out[8]);
 
 /* ---- reference index -> device (replaces the in-memory members of skch::Sketch) ---------------- */
@@ -198,7 +203,8 @@ int mm_ctx_share_index(mm_ctx *ctx, const mm_ctx *src);
 
 /* K1 only: CommonFunc::sketchSequence (commonFunc.hpp:182-288) for every segment.
  * out_sketch[seg*sketch_size + j] for j < out_count[seg], ascending by hash; seqId = seq_counter.
- * Host buffers in, host buffers out. */
+ * A segment may be longer than seg_length (see mm_segment): it is sketched in pieces and merged on the device, with the
+ * same result. Host buffers in, host buffers out. */
 int mm_sketch_segments(mm_ctx *ctx, const char *bases, uint64_t n_bases,
                        const mm_segment *segments, uint64_t n_segments,
                        mm_minmer *out_sketch, int32_t *out_count);

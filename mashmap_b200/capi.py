@@ -210,7 +210,8 @@ class Context:
         if rc != MM_OK:
             raise MashmapError(rc, self._L.mm_last_error(self._h).decode())
 
-    DIAG_NAMES = ("l1_cta_segments", "l1_pool_regrow", "cand_regrow", "l2_general_cands", "l2_loci_regrow", "sketch_general_segments")
+    DIAG_NAMES = ("l1_cta_segments", "l1_pool_regrow", "cand_regrow", "l2_general_cands", "l2_loci_regrow", "sketch_general_segments",
+                  "long_fragments")
 
     def diag(self):
         """how often the rare paths ran (mm_ctx_diag), by name"""

@@ -272,10 +272,6 @@ uint64_t getReferenceSize(const std::vector<std::string> &refSequences)
 static void checkPathLimits(const Parameters &p)
 {
   auto die = [](const std::string &m) { std::cerr << "[mashmap-b200] ERROR: " << m << std::endl; exit(1); };
-  if (!p.split)
-    std::cerr << "[mashmap-b200] NOTE: --noSplit: queries up to the segment length (" << p.segLength << " bp) are mapped as the reference maps "
-                 "them (one fragment, computeMap.hpp:587-607); a longer query stops the run (fragments longer than a segment, windowLen > 0, "
-                 "are not implemented on the device)" << std::endl;
   mm_params mp{};
   mp.kmer_size = p.kmerSize; mp.seg_length = p.segLength; mp.sketch_size = std::max(1, p.sketchSize);
   if (mm_params_check(&mp) != MM_OK) die(mm_last_error(nullptr));

@@ -153,8 +153,8 @@ void BatchMapper::phaseHook(void *user, int phase, int begin)
 
 BatchMapper::BatchMapper(const Parameters &p, const Sketch &refsketch) : param(p), refSketch(refsketch)
 {
-  // --noSplit (param.split == false): a query no longer than a segment is one fragment with or without the option
-  // (computeMap.hpp:587-607), so it is accepted; addRead stops the run at the first longer query.
+  // --noSplit (param.split == false): every query is one fragment of its full length (computeMap.hpp:587-607); one longer
+  // than a segment is mapped with windowLen = length - segLength (the device's long-fragment path).
   // Map::Map (computeMap.hpp:123-139): setProbs, setRefGroups; plus the per-sketch-size minimum-hit table
   sketchCutoffs = Stat::sketchCutoffs(param.sketchSize, param.kmerSize, param.ANIDiff, param.ANIDiffConf, param.stage1_topANI_filter);
   setRefGroups();
@@ -302,11 +302,10 @@ void BatchMapper::addRead(ReadBatch &b, const std::string &name, const char *seq
     s.offset = b.used + (uint64_t)start; s.length = flen; s.seq_counter = seqCounter; s.name_id = name_id; s.ref_group = rd.refGroup;
     b.segs.push_back(s);
   };
-  if (!param.split && len > param.segLength)
-    die("--noSplit: query '" + name + "' (" + std::to_string(len) + " bp) is longer than the segment length (" + std::to_string(param.segLength) +
-        " bp): the B200 path maps unsplit queries up to the segment length only (fragments longer than a segment -- windowLen > 0, "
-        "computeMap.hpp:933,1306 -- are not implemented on the device); raise -s or drop --noSplit");
-  if (len <= param.segLength) push(0, len);  // computeMap.hpp:587-607 (with or without --noSplit)
+  if (!param.split && (int64_t)len - param.kmerSize + 1 >= (1LL << 30))
+    die("--noSplit: query '" + name + "' (" + std::to_string(len) + " bp) has 2^30 or more k-mer positions: the reference computes "
+        "(length - k + 1) * 2 in an int (computeMap.hpp:831), so its result for this query is undefined");
+  if (!param.split || len <= param.segLength) push(0, len);  // computeMap.hpp:587-607: one fragment of the whole query
   else {
     const int n = len / param.segLength;  // :610-641
     for (int i = 0; i < n; i++) push(i * param.segLength, param.segLength);

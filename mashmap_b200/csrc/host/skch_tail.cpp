@@ -601,7 +601,7 @@ void MapTail::mapRead(const ReadRec &rd, IdentityCache &idc, MappingResultsVecto
   std::vector<mm_l1_candidate> &work = idc.work;
   unfiltered.clear(); l2Mappings.clear(); work.clear();
   bool split_mapping = true;
-  if (rd.len <= param.segLength) {  // :587-607 (with --noSplit no longer read gets here: BatchMapper::addRead stops the run)
+  if (!param.split || rd.len <= param.segLength) {  // :587-607: one fragment of the whole read
     fragmentMappings(segs[rd.first_seg], segRes[rd.first_seg], rd, idc, work, l2Mappings);
     unfiltered.insert(unfiltered.end(), l2Mappings.begin(), l2Mappings.end());
     split_mapping = false;

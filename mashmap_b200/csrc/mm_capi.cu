@@ -48,10 +48,23 @@ struct mm_ctx {
   cudaEvent_t ev_pack = nullptr;
   float pack_ms = 0;
   mm_segment *d_segs = nullptr; uint64_t segs_cap = 0; uint64_t n_segs = 0;
+  /* fragments longer than seg_length: K1 runs over d_work_segs = the caller's n_segs segments (a long one replaced by its
+   * first piece), then the n_work - n_segs pieces the long ones are cut into; d_long lists them (n_long) */
+  mm_segment *d_work_segs = nullptr; uint64_t work_segs_cap = 0;
+  uint64_t n_work = 0; uint32_t n_long = 0; uint64_t long_entries = 0;
   uint64_t *d_sk_hash = nullptr; uint64_t *d_sk_val = nullptr; int2 *d_sk_pos = nullptr; int8_t *d_sk_strand = nullptr; uint64_t sk_cap = 0;
   mm_segment_result *d_seg_res = nullptr;
   uint32_t *d_sk_reject = nullptr;
   int sk_mode = 0; /* 0 = fast sketch kernel + general kernel over its rejects; 1 = general kernel only (MM_SKETCH_TABLE=1) */
+  /* fragments longer than seg_length: vote sums of the pieces, the fragment list and the merge area (K1); the live-table
+   * offsets, the scan's work area and the live tables (K3) */
+  int32_t *d_sk_votes = nullptr; uint64_t votes_cap = 0;
+  mm_long_frag *d_long = nullptr; uint64_t long_cap = 0;
+  uint64_t *d_long_off = nullptr; uint64_t long_off_cap = 0;
+  unsigned char *d_long_tmp = nullptr; uint64_t long_tmp_cap = 0;
+  uint64_t *d_l2_long_off = nullptr; uint64_t l2_long_off_cap = 0;
+  unsigned char *d_long_scan_tmp = nullptr; uint64_t long_scan_tmp_cap = 0;
+  uint64_t *d_long_table = nullptr; uint64_t long_table_cap = 0;
   mm_l1_candidate *d_cands = nullptr; uint64_t cand_cap = 0;
   mm_l2_locus *d_loci = nullptr; uint64_t loci_cap = 0;
   uint32_t *d_counters = nullptr;
@@ -179,14 +192,16 @@ int check_ready(mm_ctx *c)
   return MM_OK;
 }
 
+/* A segment may be longer than seg_length (an unsplit query, windowLen > 0), up to the length at which the reference's
+ * (len - k + 1) * 2 (an int, computeMap.hpp:831) overflows. */
 int validate_segments(mm_ctx *c, const mm_segment *segs, uint64_t n_segs, uint64_t n_bases)
 {
   if (n_segs >= (1ULL << 31)) return fail(c, MM_EINVAL, "too many segments in one batch");
   for (uint64_t i = 0; i < n_segs; i++) {
     const mm_segment &s = segs[i];
-    if (s.length < 1 || s.length > c->params.seg_length)
-      return fail(c, MM_EINVAL, "segment %llu: length %d outside [1, seg_length=%d] (unsplit reads longer than "
-                  "seg_length are not supported)", (unsigned long long)i, s.length, c->params.seg_length);
+    if (s.length < 1 || (int64_t)s.length - c->params.kmer_size + 1 >= (1LL << 30))
+      return fail(c, MM_EINVAL, "segment %llu: length %d outside [1, 2^30 + kmer_size - 2] (the reference computes "
+                  "(length - k + 1) * 2 in an int)", (unsigned long long)i, s.length);
     if (s.offset + (uint64_t)s.length > n_bases) return fail(c, MM_EINVAL, "segment %llu exceeds the base buffer", (unsigned long long)i);
   }
   return MM_OK;
@@ -274,13 +289,50 @@ int copy_in(mm_ctx *c, uint8_t *dst, const void *src, uint64_t bytes)
   return MM_OK;
 }
 
-/* packed != 0: `bases` holds nibbles (mm_batch_upload_packed) */
+/* packed != 0: `bases` holds nibbles (mm_batch_upload_packed).
+ * A fragment longer than seg_length is sketched as pieces of at most seg_length bases that overlap by k-1 (piece j starts
+ * at base j * (seg_length - k + 1)); the sketch kernels see the caller's segments with the pieces appended and merged into
+ * the fragment's own slot afterwards (mm_launch_sketch_long_merge, mm_sketch.cu); that slot is sketched as a copy of the
+ * first piece meanwhile (the merge overwrites it). Everything after K1 sees the caller's segments. */
 int upload_batch(mm_ctx *c, const void *bases, uint64_t n_bases, const mm_segment *segs, uint64_t n_segs, int packed)
 {
   int rc = validate_segments(c, segs, n_segs, n_bases);
   if (rc) return rc;
   CU(c, cudaSetDevice(c->device));
-  if ((rc = prepare_batch_buffers(c, n_bases, n_segs))) return rc;
+  const uint64_t S = (uint64_t)c->params.sketch_size;
+  const int L = c->params.seg_length, step = L - c->params.kmer_size + 1;
+  std::vector<mm_segment> work;
+  std::vector<mm_long_frag> longs;
+  std::vector<uint64_t> entry_off(1, 0);
+  for (uint64_t i = 0; i < n_segs; i++) {
+    const mm_segment &s = segs[i];
+    if (s.length <= L) continue;
+    if (work.empty()) work.assign(segs, segs + n_segs);
+    const uint32_t n_pieces = (uint32_t)(((int64_t)s.length - c->params.kmer_size + step) / step);
+    longs.push_back(mm_long_frag{(uint32_t)i, (uint32_t)work.size(), n_pieces, 0});
+    for (uint32_t p = 0; p < n_pieces; p++) {
+      mm_segment q = s;
+      q.offset += (uint64_t)p * (uint64_t)step;
+      q.length = (int32_t)std::min<int64_t>(L, (int64_t)s.length - (int64_t)p * step);
+      work.push_back(q);
+    }
+    work[i].length = L;
+    entry_off.push_back(entry_off.back() + (uint64_t)n_pieces * S);
+  }
+  const uint64_t n_work = longs.empty() ? n_segs : work.size();
+  if (n_work >= (1ULL << 31) || entry_off.back() >= (1ULL << 32))
+    return fail(c, MM_EINVAL, "too many segments in one batch after cutting the long fragments into pieces");
+  if ((rc = prepare_batch_buffers(c, n_bases, n_work))) return rc;
+  if (!longs.empty()) {
+    if ((rc = grow(c, c->d_work_segs, c->work_segs_cap, n_work))) return rc;
+    CU(c, cudaMemcpyAsync(c->d_work_segs, work.data(), n_work * sizeof(mm_segment), cudaMemcpyHostToDevice, c->stream));
+    if ((rc = grow(c, c->d_sk_votes, c->votes_cap, c->sk_cap))) return rc;
+    if ((rc = grow(c, c->d_long, c->long_cap, longs.size()))) return rc;
+    if ((rc = grow(c, c->d_long_off, c->long_off_cap, entry_off.size()))) return rc;
+    if ((rc = grow(c, c->d_long_tmp, c->long_tmp_cap, mm_sketch_long_tmp_bytes(entry_off.back(), (uint32_t)longs.size())))) return rc;
+    CU(c, cudaMemcpyAsync(c->d_long, longs.data(), longs.size() * sizeof(mm_long_frag), cudaMemcpyHostToDevice, c->stream));
+    CU(c, cudaMemcpyAsync(c->d_long_off, entry_off.data(), entry_off.size() * 8, cudaMemcpyHostToDevice, c->stream));
+  }
   CU(c, cudaEventRecord(c->ev[6], c->stream));
   if (packed) {
     const uint64_t pbytes = (n_bases + 1) / 2;
@@ -294,8 +346,12 @@ int upload_batch(mm_ctx *c, const void *bases, uint64_t n_bases, const mm_segmen
   }
   CU(c, cudaMemcpyAsync(c->d_segs, segs, n_segs * sizeof(mm_segment), cudaMemcpyHostToDevice, c->stream));
   CU(c, cudaEventRecord(c->ev[7], c->stream));
+  if (!longs.empty()) CU(c, cudaStreamSynchronize(c->stream)); /* work / longs / entry_off are about to go */
   c->n_bases = n_bases;
   c->n_segs = n_segs;
+  c->n_work = n_work;
+  c->n_long = (uint32_t)longs.size();
+  c->long_entries = entry_off.back();
   c->batch_is_ascii = !packed;
   c->batch_mapped = false;
   return MM_OK;
@@ -307,6 +363,32 @@ int launch_pack_if_ascii(mm_ctx *c)
   if (!c->batch_is_ascii) { c->pack_ms = 0; return MM_OK; }
   CU(c, mm_launch_pack_bases(c->d_bases, c->d_packed, c->n_bases, c->stream, c->sm_count));
   c->launches++;
+  return MM_OK;
+}
+
+mm_dev_batch make_batch(mm_ctx *c);
+
+/* K1 over the resident batch: the sketch kernels over the caller's segments and the pieces of the long fragments, then
+ * the merge of the pieces */
+int launch_sketch_all(mm_ctx *c)
+{
+  mm_dev_batch b = make_batch(c);
+  if (c->n_long) b.segs = c->d_work_segs;
+  CU(c, mm_launch_sketch(c->params, b, c->stream, c->sm_count, c->sk_mode));
+  c->launches += c->sk_mode ? 1 : 2;
+  if (c->n_long) {
+    /* the pieces: general kernel (it writes the vote sums the merge needs), then the merge */
+    const uint64_t S = (uint64_t)c->params.sketch_size, n0 = c->n_segs;
+    mm_dev_batch bp = b;
+    bp.segs = c->d_work_segs + n0; bp.n_segs = (uint32_t)(c->n_work - n0);
+    bp.sk_hash = c->d_sk_hash + n0 * S; bp.sk_pos = c->d_sk_pos + n0 * S; bp.sk_strand = c->d_sk_strand + n0 * S;
+    bp.sk_votes = c->d_sk_votes + n0 * S; bp.seg_res = c->d_seg_res + n0;
+    CU(c, mm_launch_sketch(c->params, bp, c->stream, c->sm_count, 1));
+    b.sk_votes = c->d_sk_votes;
+    CU(c, mm_launch_sketch_long_merge(c->params, b, c->d_long, c->d_long_off, c->n_long, (uint32_t)n0, c->long_entries,
+                                      c->d_long_tmp, c->long_tmp_cap, c->stream));
+    c->launches += 3; /* pieces, prep, merge (the segmented sort is a library call, not counted) */
+  }
   return MM_OK;
 }
 
@@ -472,6 +554,49 @@ int run_l2_stream(mm_ctx *c, uint32_t *h_cnt)
   return fail(c, MM_ECUDA, "locus buffer kept overflowing");
 }
 
+/* K3 of the candidates of fragments longer than seg_length (k_l2_long, mm_l2.cu), after the loci of the others, which end
+ * at c->n_loci: live-table sizes -> offsets -> (host reads the total) -> the scans, appending at counters[6]. Records
+ * ev[4] again at its end. */
+int run_l2_long(mm_ctx *c, uint32_t *h_cnt)
+{
+  const uint64_t nc = c->n_cands;
+  if (c->n_long == 0 || nc == 0) return MM_OK;
+  int rc;
+  if ((rc = grow(c, c->d_l2_long_off, c->l2_long_off_cap, nc + 1))) return rc;
+  if ((rc = grow(c, c->d_long_scan_tmp, c->long_scan_tmp_cap, mm_l2_scan_tmp_bytes((uint32_t)nc) + 256))) return rc;
+  mm_dev_batch b = make_batch(c);
+  CU(c, mm_launch_l2_long_ranges(c->params, c->ix, b, (uint32_t)nc, c->d_l2_long_off, c->d_long_scan_tmp, c->long_scan_tmp_cap,
+                                 c->stream));
+  c->launches++;
+  uint64_t words = 0;
+  RD(c, c->d_l2_long_off + nc, (uint32_t *)&words, 2);
+  if (words == 0) return MM_OK;
+  if ((rc = grow(c, c->d_long_table, c->long_table_cap, words))) return rc;
+  for (int attempt = 0; attempt < 4; attempt++) {
+    b = make_batch(c);
+    ZERO_WORDS(c, c->d_counters + 1, 1);
+    k_set_u32<<<1, 1, 0, c->stream>>>(c->d_counters + 6, (uint32_t)c->n_loci);
+    CU(c, mm_launch_l2_long(c->params, c->ix, b, (uint32_t)nc, c->d_l2_long_off, c->d_long_table, c->stream, c->sm_count));
+    c->launches += 2;
+    CU(c, cudaEventRecord(c->ev[4], c->stream));
+    RD(c, c->d_counters, h_cnt, 16);
+    if (h_cnt[1] == 1 || h_cnt[6] > c->loci_cap) { /* a bigger locus buffer that keeps the loci already there, then again */
+      c->diag[MM_DIAG_L2_LOCI_REGROW]++;
+      const uint64_t cap = (uint64_t)h_cnt[6] + h_cnt[6] / 4 + 1024;
+      mm_l2_locus *p = nullptr;
+      CU(c, cudaMalloc((void **)&p, cap * sizeof(mm_l2_locus)));
+      if (c->n_loci) CU(c, cudaMemcpyAsync(p, c->d_loci, c->n_loci * sizeof(mm_l2_locus), cudaMemcpyDeviceToDevice, c->stream));
+      CU(c, cudaStreamSynchronize(c->stream));
+      cudaFree(c->d_loci);
+      c->d_loci = p; c->loci_cap = cap;
+      continue;
+    }
+    c->n_loci = h_cnt[6];
+    return MM_OK;
+  }
+  return fail(c, MM_ECUDA, "locus buffer kept overflowing");
+}
+
 /* K1 -> K2 -> K3 on the resident batch, growing output buffers and retrying on overflow */
 int run_pipeline(mm_ctx *c)
 {
@@ -506,12 +631,16 @@ int run_pipeline(mm_ctx *c)
     CU(c, cudaEventRecord(c->ev[0], c->stream));
     if ((rc = launch_pack_if_ascii(c))) return rc;
     CU(c, cudaEventRecord(c->ev_pack, c->stream));
-    CU(c, mm_launch_sketch(c->params, b, c->stream, c->sm_count, c->sk_mode));
+    if ((rc = launch_sketch_all(c))) return rc;
     CU(c, cudaEventRecord(c->ev[1], c->stream));
     int l1_launches = 0;
     CU(c, mm_launch_l1(c->params, c->ix, b, c->stream, c->sm_count, c->d_l1_slow, c->l1_warp, &l1_launches));
+    if (c->n_long) { /* windowLen > 0: k_l1_long (mm_l1.cu), after the general path (it reuses its scratch slices) */
+      CU(c, mm_launch_l1_long(c->params, c->ix, b, c->d_long, c->n_long, c->stream, c->sm_count));
+      l1_launches++;
+    }
     CU(c, cudaEventRecord(c->ev[2], c->stream));
-    c->launches += (c->sk_mode ? 1 : 2) + (uint64_t)l1_launches;
+    c->launches += (uint64_t)l1_launches;
     RD(c, c->d_counters, h_cnt, 16);
     const uint64_t need_cands = h_cnt[0];
     bool retry = false;
@@ -536,12 +665,13 @@ int run_pipeline(mm_ctx *c)
     /* K3 */
     if (c->l2_mode == 1) {
       int rc2 = run_l2_stream(c, h_cnt);
-      if (rc2 == MM_OK) {
+      if (rc2 == MM_OK && (rc2 = run_l2_long(c, h_cnt)) == MM_OK) {
         if (c->batch_is_ascii) cudaEventElapsedTime(&c->pack_ms, c->ev[0], c->ev_pack);
         cudaEventElapsedTime(&c->stage_ms[0], c->ev_pack, c->ev[1]);
         cudaEventElapsedTime(&c->stage_ms[1], c->ev[1], c->ev[2]);
         cudaEventElapsedTime(&c->stage_ms[2], c->ev[3], c->ev[4]);
         cudaEventElapsedTime(&c->stage_ms[5], c->ev[0], c->ev[4]);
+        c->diag[MM_DIAG_LONG_FRAGMENTS] += c->n_long;
         c->batch_mapped = true;
         return MM_OK;
       }
@@ -567,11 +697,13 @@ int run_pipeline(mm_ctx *c)
         continue;
       }
       c->n_loci = h_cnt[6];
+      if ((rc = run_l2_long(c, h_cnt))) return rc;
       if (c->batch_is_ascii) cudaEventElapsedTime(&c->pack_ms, c->ev[0], c->ev_pack);
       cudaEventElapsedTime(&c->stage_ms[0], c->ev_pack, c->ev[1]);
       cudaEventElapsedTime(&c->stage_ms[1], c->ev[1], c->ev[2]);
       cudaEventElapsedTime(&c->stage_ms[2], c->ev[3], c->ev[4]);
       cudaEventElapsedTime(&c->stage_ms[5], c->ev[0], c->ev[4]); /* first launch -> last kernel end, incl. host gaps */
+      c->diag[MM_DIAG_LONG_FRAGMENTS] += c->n_long;
       c->batch_mapped = true;
       return MM_OK;
     }
@@ -647,6 +779,8 @@ int mm_ctx_destroy(mm_ctx *c)
   mm_built_index_free(&c->built);
   cudaFree(c->d_bases); cudaFree(c->d_packed); cudaFree(c->d_sk_reject); cudaFree(c->d_segs); cudaFree(c->d_sk_hash); cudaFree(c->d_sk_val); cudaFree(c->d_sk_pos); cudaFree(c->d_sk_strand);
   cudaFree(c->d_seg_res); cudaFree(c->d_cands); cudaFree(c->d_loci); cudaFree(c->d_counters); cudaFree(c->d_scratch);
+  cudaFree(c->d_sk_votes); cudaFree(c->d_work_segs); cudaFree(c->d_long); cudaFree(c->d_long_off); cudaFree(c->d_long_tmp);
+  cudaFree(c->d_l2_long_off); cudaFree(c->d_long_scan_tmp); cudaFree(c->d_long_table);
   cudaFree(c->d_l1_slow); cudaFree(c->d_l2_order); cudaFree(c->d_l2_ranges); cudaFree(c->d_l2_rec_off); cudaFree(c->d_l2_recs); cudaFree(c->d_scan_tmp);
   for (auto &ev : c->ev) cudaEventDestroy(ev);
   if (c->h_pub) cudaFreeHost(c->h_pub);
@@ -928,22 +1062,21 @@ int mm_batch_fetch_sketch(mm_ctx *c, mm_minmer *out, int32_t *out_count)
 int mm_sketch_segments(mm_ctx *c, const char *bases, uint64_t n_bases, const mm_segment *segs, uint64_t n_segs,
                        mm_minmer *out, int32_t *out_count)
 {
-  if (!c || !out || !out_count) return fail(c, MM_EINVAL, "null argument");
+  if (!c || !out || !out_count || (!segs && n_segs)) return fail(c, MM_EINVAL, "null argument");
   int rc = upload_batch(c, bases, n_bases, segs, n_segs, 0);
   if (rc) return rc;
-  mm_dev_batch b = make_batch(c);
   if ((rc = launch_pack_if_ascii(c))) return rc;
   ZERO_WORDS(c, c->d_counters, 16);
   CU(c, cudaEventRecord(c->ev[0], c->stream));
-  CU(c, mm_launch_sketch(c->params, b, c->stream, c->sm_count, c->sk_mode));
+  if ((rc = launch_sketch_all(c))) return rc;
   CU(c, cudaEventRecord(c->ev[1], c->stream));
-  c->launches += c->sk_mode ? 1 : 2;
   CU(c, cudaStreamSynchronize(c->stream));
   cudaEventElapsedTime(&c->stage_ms[0], c->ev[0], c->ev[1]);
   {
     uint32_t h9 = 0;
     if (cudaMemcpy(&h9, c->d_counters + 9, 4, cudaMemcpyDeviceToHost) == cudaSuccess) c->diag[MM_DIAG_SKETCH_GENERAL_SEGMENTS] += h9;
   }
+  c->diag[MM_DIAG_LONG_FRAGMENTS] += c->n_long;
   c->batch_mapped = true; /* sketches only; fetch_sketch reads sketch_size == raw count */
   rc = mm_batch_fetch_sketch(c, out, out_count);
   c->batch_mapped = false;

@@ -81,6 +81,8 @@ struct mm_dev_batch {
   uint64_t *sk_val;   /* lookup-table value of every sketch hash (written by k_l1_probe): 0 = absent */
   int2 *sk_pos;               /* (first position, last position)                                */
   int8_t *sk_strand;
+  int32_t *sk_votes;          /* optional (nullptr = not written; general sketch kernel only): the vote SUM of every     */
+                              /* sketch slot, which the merge of a long fragment's pieces needs (sk_strand: its sign)   */
   mm_segment_result *seg_res;
   uint32_t *sk_reject;        /* work list of the general sketch kernel: segments the fast kernel handed over (count in counters[9]) */
   mm_l1_candidate *cands;
@@ -127,12 +129,35 @@ MM_HD uint32_t mm_tab_slot_of(uint64_t key, int log2)
 
 /* launchers implemented in the .cu files; all return cudaError_t from the launch */
 cudaError_t mm_launch_sketch(const mm_params &p, const mm_dev_batch &b, cudaStream_t st, int sm_count, int mode);
+/* K1 for fragments longer than seg_length (mm_sketch.cu): the fragment was cut into pieces of at most seg_length bases
+ * that overlap by kmer_size-1 (piece j starts at base j * (seg_length - kmer_size + 1)); the pieces were sketched by
+ * mm_launch_sketch in mode 1 (general kernel) as segments [piece0, piece0 + n_pieces) of the same batch, with
+ * b.sk_votes set. This merges the pieces of each long fragment into the fragment's own sketch slot. */
+struct mm_long_frag {
+  uint32_t seg;      /* the fragment's segment index: where its sketch goes          */
+  uint32_t piece0;   /* segment index of its first piece                              */
+  uint32_t n_pieces;
+  uint32_t _pad;
+};
+size_t mm_sketch_long_tmp_bytes(uint64_t n_entries, uint32_t n_frags);
+cudaError_t mm_launch_sketch_long_merge(const mm_params &p, const mm_dev_batch &b, const mm_long_frag *frags,
+                                        const uint64_t *entry_off, uint32_t n_frags, uint32_t piece_base, uint64_t n_entries,
+                                        void *tmp, size_t tmp_bytes, cudaStream_t st);
 /* K0: ASCII -> nibbles (makeUpperCaseAndValidDNA as a format change); both buffers padded to a multiple of 16 bases */
 cudaError_t mm_launch_pack_bases(const uint8_t *ascii, uint8_t *packed, uint64_t n_bases, cudaStream_t st, int sm_count);
 cudaError_t mm_launch_l1(const mm_params &p, const mm_dev_index &ix, const mm_dev_batch &b,
                          cudaStream_t st, int sm_count, uint32_t *slow_list, int use_warp_path, int *n_launched);
 cudaError_t mm_launch_l2(const mm_params &p, const mm_dev_index &ix, const mm_dev_batch &b,
                          uint32_t n_cands, cudaStream_t st, int sm_count);
+/* K2 / K3 of the fragments longer than seg_length (windowLen > 0): the kernels above skip them. K3: one warp per
+ * candidate of such a fragment, live hashes in a per-candidate open-addressing table of `table_slots[c]` slots at
+ * `table_off[c]` in `table` (u64 words; sized by mm_launch_l2_long_ranges) */
+cudaError_t mm_launch_l1_long(const mm_params &p, const mm_dev_index &ix, const mm_dev_batch &b, const mm_long_frag *longs,
+                              uint32_t n_long, cudaStream_t st, int sm_count);
+cudaError_t mm_launch_l2_long_ranges(const mm_params &p, const mm_dev_index &ix, const mm_dev_batch &b, uint32_t n_cands,
+                                     uint64_t *table_off, void *scan_tmp, size_t scan_tmp_bytes, cudaStream_t st);
+cudaError_t mm_launch_l2_long(const mm_params &p, const mm_dev_index &ix, const mm_dev_batch &b, uint32_t n_cands,
+                              const uint64_t *table_off, uint64_t *table, cudaStream_t st, int sm_count);
 /* new L2: ranges -> (host reads the total) -> prep -> lane-per-candidate scan -> general kernel for overflow */
 cudaError_t mm_launch_l2_ranges(const mm_params &p, const mm_dev_index &ix, const mm_dev_batch &b, uint32_t n_cands,
                                 void *scan_tmp, size_t scan_tmp_bytes, cudaStream_t st);

@@ -27,8 +27,12 @@
  *              that warp's shared memory (<= 512 points). Segments with more points are pushed on a list ...
  *   k_l1_cta   NT = 128: ... and done by one CTA each: 2048 points in shared memory, more in a per-CTA global
  *              scratch slice or a bump-allocated pool (the host grows the pool and re-runs if it is exhausted).
- * windowLen (computeMap.hpp:933) is 0 for every fragment of a split read and for reads no longer than
- * segLength, which is all the C ABI accepts.
+ * windowLen (computeMap.hpp:933) is 0 for every fragment of a split read and for reads no longer than segLength.
+ * A fragment longer than segLength (an unsplit query, --noSplit) has windowLen = len - segLength > 0: the two kernels above
+ * leave it alone and k_l1_long (one CTA per such fragment) runs the same steps 1-3 -- with every point's hit (= its
+ * query hash) sorted along -- and then the two sweeps of computeMap.hpp:946-1116 literally, with hash_to_freq as one
+ * counter per hit (every point's hash is a query-sketch hash). These fragments are few and have about as many points
+ * as a segment, so one thread runs the sweeps.
  */
 #include <algorithm>
 
@@ -87,9 +91,9 @@ __device__ __forceinline__ uint32_t group_exclusive_scan(uint32_t v, uint32_t *w
   return base + incl - v;
 }
 
-/* in-place bitonic sort of n (power of two) u64 keys by the group (shared or global memory) */
-template <int NT>
-__device__ void group_bitonic_sort(uint64_t *a, uint32_t n)
+/* in-place bitonic sort of n (power of two) u64 keys by the group (shared or global memory); PAIRS: v[] moves along */
+template <int NT, bool PAIRS = false>
+__device__ void group_bitonic_sort(uint64_t *a, uint32_t n, uint32_t *v = nullptr)
 {
   /* (a register-resident variant -- keys in lanes, exchanges by warp shuffle -- was measured slower than this one:
    * 64-bit shuffles cost two SHFL each and the selects outweigh the saved shared-memory traffic) */
@@ -100,7 +104,10 @@ __device__ void group_bitonic_sort(uint64_t *a, uint32_t n)
         const uint32_t p = i | j;
         const bool up = (i & k) == 0;
         const uint64_t x = a[i], y = a[p];
-        if ((x > y) == up) { a[i] = y; a[p] = x; }
+        if ((x > y) == up) {
+          a[i] = y; a[p] = x;
+          if (PAIRS) { const uint32_t t2 = v[i]; v[i] = v[p]; v[p] = t2; }
+        }
       }
       grp<NT>::sync();
     }
@@ -344,6 +351,96 @@ __device__ int l1_process_range(const mm_params &prm, const mm_dev_index &ix, co
   return best;
 }
 
+/* computeL1CandidateRegions (computeMap.hpp:915-1116) over the sorted points keys[0..n) of ONE reference group of a
+ * fragment with windowLen > 0, literally, by ONE thread. hid[i] = the hit (query hash) of point i; freq[0..n_hits) is
+ * hash_to_freq, cleared here and between the sweeps (:1003). Candidates go to o (join of :1102-1115 through
+ * l1_close_run). Returns bestIntersectionSize of sweep #1 (uncapped); mh_out = minimumHits after the HG raise, 0 on the
+ * early return (:987-990). */
+__device__ int l1_window_range(const mm_params &prm, const mm_dev_index &ix, const uint64_t *keys, const uint32_t *hid,
+                               uint32_t n, int qs, int window_len, int *freq, uint32_t n_hits, l1_out_list &o, int &mh_out)
+{
+  auto seq = [&](uint32_t i) { return mm_point_seq(keys[i]); };
+  auto pos = [&](uint32_t i) { return mm_point_pos(keys[i]); };
+  /* the trailing iterator (:946-976, :1033-1046): CLOSE points at or before lead.pos - windowLen on the lead's contig,
+   * or on an earlier contig; a hash stops counting when its last open window closes */
+  auto trail = [&](uint32_t &tr, uint32_t ld, int &overlap) {
+    while (tr < n && ((seq(tr) == seq(ld) && pos(tr) <= pos(ld) - window_len) || seq(tr) < seq(ld))) {
+      if (!mm_point_open(keys[tr]) && --freq[hid[tr]] == 0) overlap--;
+      tr++;
+    }
+  };
+  /* the leading iterator: every point of one position group (seqId not compared, :976, :1051); a hash starts counting
+   * with its first open window */
+  auto lead = [&](uint32_t &ld, int p, int &overlap) {
+    while (ld < n && pos(ld) == p) {
+      if (mm_point_open(keys[ld]) && freq[hid[ld]]++ == 0) overlap++;
+      ld++;
+    }
+  };
+  for (uint32_t j = 0; j < n_hits; j++) freq[j] = 0;
+  int overlap = 0, best = 0;
+  for (uint32_t tr = 0, ld = 0; ld < n;) { /* sweep #1 (:946-983) */
+    trail(tr, ld, overlap);
+    lead(ld, pos(ld), overlap);
+    best = max(best, overlap);
+  }
+  int mh = ix.min_hits[min(qs, ix.n_min_hits - 1)];
+  mh_out = 0;
+  if (prm.stage1_topani_filter) {
+    if (best < mh) return best; /* :987-990 */
+    const double denom = fmax(1.0, (double)prm.sketch_size / 1000.0);
+    const int ci = min((int)((double)min(best, qs) / denom), ix.n_cutoffs - 1);
+    mh = max(ix.cutoffs[ci], mh); /* :992-997 */
+  }
+  mh_out = mh;
+  for (uint32_t j = 0; j < n_hits; j++) freq[j] = 0; /* :1003 */
+  /* sweep #2 (:1009-1098): the test lags one position group behind; a run is cut where the contig changes */
+  l1_walk_state w;
+  w.in_run = false; w.have_out = false; w.prev_group = -2;
+  w.run_seq = w.run_start = w.run_end = w.run_isz = 0;
+  w.out_seq = w.out_start = w.out_end = w.out_isz = 0;
+  bool in_cand = false;
+  int c_seq = 0, c_start = 0, c_end = 0, c_isz = 0; /* l1_out */
+  int prev_seq = 0, prev_pos = 0, cur_seq = seq(0), cur_pos = pos(0);
+  auto push_local = [&]() { /* localOpts.push_back(l1_out), joined on the fly (:1102-1115) */
+    w.in_run = true;
+    w.run_seq = c_seq; w.run_start = c_start; w.run_end = c_end; w.run_isz = c_isz;
+    l1_close_run(w, prm.seg_length, o);
+    c_seq = c_start = c_end = c_isz = 0; /* l1_out = L1_candidateLocus_t() */
+  };
+  overlap = 0;
+  for (uint32_t tr = 0, ld = 0; ld < n;) {
+    const int prev_overlap = overlap;
+    trail(tr, ld, overlap);
+    if (pos(ld) != cur_pos) {
+      prev_seq = cur_seq; prev_pos = cur_pos;
+      cur_seq = seq(ld); cur_pos = pos(ld);
+    }
+    lead(ld, cur_pos, overlap);
+    if (prev_overlap >= mh) {
+      if (c_seq != prev_seq && in_cand) {
+        push_local();
+        in_cand = false;
+      }
+      if (!in_cand) {
+        c_start = c_end = prev_pos - window_len;
+        c_seq = prev_seq;
+        c_isz = prev_overlap;
+        in_cand = true;
+      } else { /* stage2_full_scan is always true (parseCmdArgs.hpp:590) */
+        c_isz = max(c_isz, prev_overlap);
+        c_end = prev_pos - window_len;
+      }
+    } else {
+      if (in_cand) push_local();
+      in_cand = false;
+    }
+  }
+  if (in_cand) push_local();
+  if (w.have_out) l1_emit(o, w.out_seq, w.out_start, w.out_end, w.out_isz);
+  return best;
+}
+
 /* probe the lookup table for one hash: 0 = absent, else offset<<25 | count<<1 | isFreqSeed */
 __device__ __forceinline__ uint64_t l1_probe(const mm_dev_index &ix, uint64_t h)
 {
@@ -373,8 +470,10 @@ __global__ void __launch_bounds__(256) k_l1_probe(const mm_dev_index ix, const m
 }
 
 /* One segment, processed by a group of NT threads (the table values of its hashes are in b.sk_val).
- * Returns false (NT == 32 only) if the segment has more points than the warp path holds: nothing was modified. */
-template <int NT, int LOCAL, int SMEM_POINTS>
+ * Returns false (NT == 32 only) if the segment has more points than the warp path holds: nothing was modified.
+ * WIN: the segment is a fragment longer than seg_length (windowLen > 0, k_l1_long); without WIN such a fragment is
+ * skipped (returns true, writes nothing). */
+template <int NT, int LOCAL, int SMEM_POINTS, bool WIN = false>
 __device__ bool l1_segment(const mm_params &prm, const mm_dev_index &ix, const mm_dev_batch &b, uint32_t seg, l1_hit *hits,
                            uint64_t *skeys, uint32_t *scopn, uint32_t *shead, uint32_t *sginfo,
                            l1_shared<NT, LOCAL> &sh, uint32_t scratch_slot)
@@ -382,6 +481,7 @@ __device__ bool l1_segment(const mm_params &prm, const mm_dev_index &ix, const m
   const int S = prm.sketch_size;
   const int tid = grp<NT>::tid();
   const mm_segment sg = b.segs[seg];
+  if (!WIN && sg.length > prm.seg_length) return true; /* k_l1_long's */
   const size_t sbase = (size_t)seg * (size_t)S;
   const int raw = b.seg_res[seg].sketch_raw_count;
   if (tid == 0) { sh.fail = 0; sh.cand_base = 0; sh.out_n = 0; }
@@ -501,21 +601,28 @@ __device__ bool l1_segment(const mm_params &prm, const mm_dev_index &ix, const m
 #pragma unroll
         for (int u = 0; u < 4; u++) {
           const uint32_t p = p0 + u * NT;
-          if (p < m) keys[p] = admit(v[u]);
+          if (p < m) {
+            keys[p] = admit(v[u]);
+            if (WIN) copn[p] = owner[p]; /* the point's hit: its query hash */
+          }
         }
       }
     } else {
       for (uint32_t hi = tid; hi < hit_total; hi += NT) {
         const l1_hit hh = hits[hi];
-        for (uint32_t q = 0; q < hh.cnt; q++) keys[hh.dst + q] = admit(ix.pts[hh.off + q]);
+        for (uint32_t q = 0; q < hh.cnt; q++) {
+          keys[hh.dst + q] = admit(ix.pts[hh.off + q]);
+          if (WIN) copn[hh.dst + q] = hi;
+        }
       }
     }
     uint32_t dropped;
     (void)group_exclusive_scan<NT>(dropped_local, sh.warp_sums, dropped);
     mp = m - dropped;
     grp<NT>::sync();
-    /* ---- 3. sort by (seqId,pos,side); dropped points (all ones) go last ---- */
-    group_bitonic_sort<NT>(keys, n_pow2);
+    /* ---- 3. sort by (seqId,pos,side); dropped points (all ones) go last; WIN: the hits (in copn) move along ---- */
+    if (WIN) group_bitonic_sort<NT, true>(keys, n_pow2, copn);
+    else group_bitonic_sort<NT>(keys, n_pow2);
   }
 
   /* ---- 4./5./6. per reference group: scans, best, threshold, walk ---- */
@@ -539,8 +646,15 @@ __device__ bool l1_segment(const mm_params &prm, const mm_dev_index &ix, const m
         end = sh.range_end;
         grp<NT>::sync();
       }
-      int mh = 0;
-      const int best = l1_process_range<NT, LOCAL>(prm, ix, keys + start, copn, head, ginfo, end - start, (int)kept_total, sh, out, mh);
+      int mh = 0, best = 0;
+      if (WIN) { /* only thread 0's best / mh are read (the segment result below) */
+        if (tid == 0)
+          best = l1_window_range(prm, ix, keys + start, copn + start, end - start, (int)kept_total, sg.length - prm.seg_length,
+                                 (int *)hits, hit_total, out, mh); /* the hit list is dead: its space holds hash_to_freq */
+        grp<NT>::sync();
+      } else {
+        best = l1_process_range<NT, LOCAL>(prm, ix, keys + start, copn, head, ginfo, end - start, (int)kept_total, sh, out, mh);
+      }
       if (pass == 0) {
         best_all = max(best_all, best);
         if (first_range) mh_first = mh;
@@ -649,6 +763,23 @@ k_l1_cta(const mm_params prm, const mm_dev_index ix, const mm_dev_batch b, const
   }
 }
 
+/* fragments longer than seg_length (windowLen > 0): one CTA per listed fragment, the general path's layout and scratch
+ * slices (it runs after k_l1_cta on the same stream) */
+__global__ void __launch_bounds__(128)
+k_l1_long(const mm_params prm, const mm_dev_index ix, const mm_dev_batch b, const mm_long_frag *__restrict__ longs, uint32_t n_long)
+{
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int S = prm.sketch_size;
+  l1_hit *hits = (l1_hit *)smem_raw;
+  uint64_t *skeys = (uint64_t *)(smem_raw + (((size_t)S * sizeof(l1_hit) + 15) & ~(size_t)15));
+  uint32_t *scopn = (uint32_t *)(skeys + L1_CTA_POINTS);
+  uint32_t *shead = scopn + L1_CTA_POINTS;
+  uint32_t *sginfo = shead + L1_CTA_POINTS;
+  __shared__ l1_shared<128, L1_LOCAL_CANDS_CTA> sh;
+  for (uint32_t w = blockIdx.x; w < n_long; w += gridDim.x)
+    l1_segment<128, L1_LOCAL_CANDS_CTA, L1_CTA_POINTS, true>(prm, ix, b, longs[w].seg, hits, skeys, scopn, shead, sginfo, sh, blockIdx.x);
+}
+
 size_t l1_cta_smem(const mm_params &p)
 {
   return (((size_t)p.sketch_size * sizeof(l1_hit) + 15) & ~(size_t)15) + (size_t)L1_CTA_POINTS * (8 + 4 + 4 + 4);
@@ -701,5 +832,19 @@ cudaError_t mm_launch_l1(const mm_params &p, const mm_dev_index &ix, const mm_de
   /* the general path reads its work count from counters[8] on the device: no host round trip in between */
   k_l1_cta<<<grid, 128, l1_cta_smem(p), st>>>(p, ix, b, slow_list);
   if (n_launched) *n_launched = 3;
+  return cudaGetLastError();
+}
+
+/* K2 of the fragments longer than seg_length (after mm_launch_l1, whose kernels skip them and whose probe covered them) */
+cudaError_t mm_launch_l1_long(const mm_params &p, const mm_dev_index &ix, const mm_dev_batch &b, const mm_long_frag *longs,
+                              uint32_t n_long, cudaStream_t st, int sm_count)
+{
+  if (n_long == 0) return cudaSuccess;
+  const uint32_t grid = mm_l1_grid_size(p, sm_count);
+  if (grid == 0) return cudaErrorInvalidValue;
+  const size_t smem = l1_cta_smem(p);
+  cudaError_t e = cudaFuncSetAttribute(k_l1_long, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return e;
+  k_l1_long<<<min(grid, n_long), 128, smem, st>>>(p, ix, b, longs, n_long);
   return cudaGetLastError();
 }

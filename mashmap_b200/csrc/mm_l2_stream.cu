@@ -72,8 +72,10 @@ __global__ void k_l2_ranges(const mm_params prm, const mm_dev_index ix, const mm
   /* evictions: wpos_end > rangeStart (anything smaller is never live) and <= rangeEnd (the last insert position) */
   r.d0 = lower_bound_i32(ix.idx2_wend, cs, ce, cd.rangeStartPos + 1);
   const uint64_t d1 = lower_bound_i32(ix.idx2_wend, r.d0, ce, cd.rangeEndPos + 1);
-  r.nI = (uint32_t)(it1 - r.it0);
-  r.nD = (uint32_t)(d1 - r.d0);
+  /* a fragment longer than seg_length (windowLen > 0) is scanned by k_l2_long (mm_l2.cu): no records here */
+  const bool windowed = b.segs[cd.segment].length > prm.seg_length;
+  r.nI = windowed ? 0u : (uint32_t)(it1 - r.it0);
+  r.nD = windowed ? 0u : (uint32_t)(d1 - r.d0);
   r.next_wpos = 0;
   if (r.nI > 0) r.next_wpos = (it1 < ce) ? ix.idx_wpos[it1] : ix.idx_wpos[it1 - 1]; /* std::next(windowIt,...) (:1387-1390) */
   r._pad = 0;

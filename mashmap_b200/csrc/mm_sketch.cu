@@ -32,6 +32,8 @@
  *   A thread whose stretch of the segment contains an N (nibble bit 3) takes the same loop with the run-length test
  *   of commonFunc.hpp:207-223 compiled in; all others skip it.
  */
+#include <cub/cub.cuh>
+
 #include "mm_internal.h"
 
 namespace {
@@ -421,7 +423,7 @@ __global__ void __launch_bounds__(SK_THREADS)
 k_sketch_table(const uint8_t *__restrict__ packed, const mm_segment *__restrict__ segs, uint32_t n_segs_all,
                const uint32_t *__restrict__ work_list, const uint32_t *__restrict__ work_count, int S,
                int seg_length, int C, int CAP, uint64_t *__restrict__ sk_hash, int2 *__restrict__ sk_pos,
-               int8_t *__restrict__ sk_strand, mm_segment_result *__restrict__ seg_res)
+               int8_t *__restrict__ sk_strand, int32_t *__restrict__ sk_votes, mm_segment_result *__restrict__ seg_res)
 {
   extern __shared__ __align__(16) unsigned char smem[];
   const uint32_t n_segs = work_list ? *work_count : n_segs_all;
@@ -598,6 +600,7 @@ k_sketch_table(const uint8_t *__restrict__ packed, const mm_segment *__restrict_
         sk_pos[obase + rank] = make_int2(first[slot], last[slot]);
         const int v = votes[slot];
         sk_strand[obase + rank] = (int8_t)(v > 0 ? 1 : (v == 0 ? 0 : -1)); /* commonFunc.hpp:282 */
+        if (sk_votes) sk_votes[obase + rank] = v;
       }
     }
     if (tid == 0) {
@@ -608,6 +611,7 @@ k_sketch_table(const uint8_t *__restrict__ packed, const mm_segment *__restrict_
           sk_pos[obase + dt] = make_int2(ctrl->max_first, ctrl->max_last);
           const int v = ctrl->max_votes;
           sk_strand[obase + dt] = (int8_t)(v > 0 ? 1 : (v == 0 ? 0 : -1));
+          if (sk_votes) sk_votes[obase + dt] = v;
         }
         count = dt + 1;
       }
@@ -967,7 +971,7 @@ cudaError_t launch_k(const mm_params &p, const mm_dev_batch &b, cudaStream_t st,
   if (mode == 1 || NC > 65535 || FL.total > 227u * 1024u) {
     const uint32_t grid = full > b.n_segs ? b.n_segs : full;
     k_sketch_table<K><<<grid, SK_THREADS, smem, st>>>(b.packed, b.segs, b.n_segs, nullptr, nullptr, p.sketch_size, p.seg_length, C,
-                                                      CAP, b.sk_hash, b.sk_pos, b.sk_strand, b.seg_res);
+                                                      CAP, b.sk_hash, b.sk_pos, b.sk_strand, b.sk_votes, b.seg_res);
     return cudaGetLastError();
   }
   e = cudaFuncSetAttribute(k_sketch<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FL.total);
@@ -986,11 +990,140 @@ cudaError_t launch_k(const mm_params &p, const mm_dev_batch &b, cudaStream_t st,
   uint32_t rgrid = (uint32_t)sm_count;
   if (rgrid > b.n_segs) rgrid = b.n_segs;
   k_sketch_table<K><<<rgrid, SK_THREADS, smem, st>>>(b.packed, b.segs, b.n_segs, b.sk_reject, b.counters + 9, p.sketch_size, p.seg_length,
-                                                     C, CAP, b.sk_hash, b.sk_pos, b.sk_strand, b.seg_res);
+                                                     C, CAP, b.sk_hash, b.sk_pos, b.sk_strand, b.sk_votes, b.seg_res);
   return cudaGetLastError();
 }
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * K1 for a fragment longer than seg_length (an unsplit query, --noSplit): it does not fit one CTA's shared memory, so
+ * it is cut into pieces of at most seg_length bases, consecutive pieces overlapping by k-1 bases -- every k-mer start
+ * position belongs to exactly one piece, and the N test and both hashes of a k-mer read only its own k bases -- the
+ * pieces are sketched as ordinary segments by the general kernel above (k_sketch_table, the only one that writes the
+ * vote SUMS; the fast kernel stays as it is for the ordinary segments), and merged here.
+ *
+ * Exactness: let h be one of the s smallest distinct hashes of the whole fragment. In every piece where h occurs, fewer
+ * than s distinct hashes of the piece are smaller than h (each is also a hash of the fragment), so h is among the
+ * piece's s smallest and the piece reports h with its first and last position and the vote sum of ALL its occurrences
+ * in that piece. Over the pieces these cover every occurrence of h: first = min, last = max (plus the piece offset),
+ * votes = sum. Every hash the pieces report is a hash of the fragment, so the s smallest distinct hashes of the union
+ * are exactly the fragment's s smallest; and where the fragment has fewer than s distinct hashes every piece reports
+ * all of its own, so the union is all of them. The union's other (larger) hashes may have partial statistics; they are
+ * never written.
+ *
+ * The merge: one sort of the pieces' slots by hash per fragment (library segmented radix sort, plumbing), then one warp
+ * per fragment walks the sorted slots 32 at a time: the first slot of every hash run is a head, a ballot ranks the heads,
+ * a head whose rank is < s adds up its run (at most one slot per piece) and writes the fragment's slot `rank`.
+ * ------------------------------------------------------------------------------------------------------------- */
+
+/* slot i of the pieces' area: key = its hash, or ~0 where the piece has fewer than s hashes (value i either way, so a
+ * padding slot is told apart from a real hash ~0 by its index) */
+__global__ void k_long_prep(const mm_segment_result *__restrict__ seg_res, uint64_t *__restrict__ sk_hash, uint32_t piece_base,
+                            int S, uint64_t n_entries, uint32_t *__restrict__ vals)
+{
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_entries) return;
+  const uint64_t slot = (uint64_t)piece_base * (uint64_t)S + i;
+  const uint32_t seg = piece_base + (uint32_t)(i / (uint64_t)S);
+  if ((int)(i % (uint64_t)S) >= seg_res[seg].sketch_size) sk_hash[slot] = SK_EMPTY;
+  vals[i] = (uint32_t)i;
+}
+
+__global__ void __launch_bounds__(128) k_long_merge(const mm_long_frag *__restrict__ frags, uint32_t n_frags,
+                                                    const uint64_t *__restrict__ entry_off, const uint64_t *__restrict__ keys,
+                                                    const uint32_t *__restrict__ vals, uint32_t piece_base, int S,
+                                                    int piece_step, const int32_t *__restrict__ pk_votes,
+                                                    uint64_t *__restrict__ sk_hash, int2 *sk_pos, int8_t *__restrict__ sk_strand,
+                                                    mm_segment_result *seg_res)
+{
+  const uint32_t f = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (f >= n_frags) return;
+  const mm_long_frag fr = frags[f];
+  const uint64_t b0 = entry_off[f], b1 = entry_off[f + 1];
+  const uint32_t q0 = fr.piece0 - piece_base; /* first piece of this fragment in the pieces' area */
+  const size_t obase = (size_t)fr.seg * (size_t)S;
+  int rank = 0;
+  for (uint64_t base = b0; base < b1 && rank < S; base += 32) {
+    const uint64_t i = base + (uint64_t)lane;
+    bool head = false;
+    uint64_t h = 0;
+    if (i < b1) {
+      h = keys[i];
+      head = i == b0 || keys[i - 1] != h;
+    }
+    int first = 0x7fffffff, last = -1, votes = 0;
+    bool real = false;
+    if (head) {
+      for (uint64_t t = i; t < b1 && keys[t] == h; t++) {
+        const uint32_t v = vals[t];
+        const uint32_t q = v / (uint32_t)S, j = v % (uint32_t)S;
+        if ((int)j >= seg_res[piece_base + q].sketch_size) continue; /* padding of a piece with fewer than s hashes */
+        const uint64_t slot = (uint64_t)piece_base * (uint64_t)S + v;
+        const int off = (int)(q - q0) * piece_step;
+        const int2 p = sk_pos[slot]; /* a piece's slot: never one the merge writes */
+        first = min(first, p.x + off);
+        last = max(last, p.y + off);
+        votes += pk_votes[slot];
+        real = true;
+      }
+    }
+    const uint32_t heads = __ballot_sync(0xffffffffu, real);
+    const int r = rank + __popc(heads & ((1u << lane) - 1u));
+    if (real && r < S) {
+      sk_hash[obase + r] = h;
+      sk_pos[obase + r] = make_int2(first, last);
+      sk_strand[obase + r] = (int8_t)(votes > 0 ? 1 : (votes == 0 ? 0 : -1)); /* commonFunc.hpp:282 */
+    }
+    rank += __popc(heads);
+  }
+  if (lane == 0) {
+    const int count = min(rank, S);
+    mm_segment_result res;
+    res.sketch_max_hash = 0;
+    res.sketch_raw_count = count;
+    res.sketch_size = count;
+    res.n_points = 0; res.minimum_hits = 0; res.best_intersection = 0;
+    res.first_candidate = 0; res.n_candidates = 0; res._pad = 0;
+    seg_res[fr.seg] = res;
+  }
+}
+
 } // namespace
+
+size_t mm_sketch_long_tmp_bytes(uint64_t n_entries, uint32_t n_frags)
+{
+  size_t sort_bytes = 0;
+  cub::DeviceSegmentedRadixSort::SortPairs(nullptr, sort_bytes, (const uint64_t *)nullptr, (uint64_t *)nullptr,
+                                           (const uint32_t *)nullptr, (uint32_t *)nullptr, (int64_t)n_entries, (int64_t)n_frags,
+                                           (const uint64_t *)nullptr, (const uint64_t *)nullptr);
+  /* keys out (u64) + values in / out (u32) + the sort's own area */
+  return n_entries * 16 + 256 * 3 + sort_bytes;
+}
+
+cudaError_t mm_launch_sketch_long_merge(const mm_params &p, const mm_dev_batch &b, const mm_long_frag *frags,
+                                        const uint64_t *entry_off, uint32_t n_frags, uint32_t piece_base, uint64_t n_entries,
+                                        void *tmp, size_t tmp_bytes, cudaStream_t st)
+{
+  if (n_frags == 0 || n_entries == 0) return cudaSuccess;
+  const int S = p.sketch_size;
+  unsigned char *t = (unsigned char *)tmp;
+  uint64_t *keys_out = (uint64_t *)t;
+  uint32_t *vals_in = (uint32_t *)(t + ((n_entries * 8 + 255) & ~255ULL));
+  uint32_t *vals_out = (uint32_t *)((unsigned char *)vals_in + ((n_entries * 4 + 255) & ~255ULL));
+  unsigned char *sort_tmp = (unsigned char *)vals_out + ((n_entries * 4 + 255) & ~255ULL);
+  size_t sort_bytes = tmp_bytes - (size_t)(sort_tmp - t);
+  uint64_t *keys_in = b.sk_hash + (uint64_t)piece_base * (uint64_t)S;
+  k_long_prep<<<(uint32_t)((n_entries + 255) / 256), 256, 0, st>>>(b.seg_res, b.sk_hash, piece_base, S, n_entries, vals_in);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  e = cub::DeviceSegmentedRadixSort::SortPairs(sort_tmp, sort_bytes, keys_in, keys_out, vals_in, vals_out, (int64_t)n_entries,
+                                               (int64_t)n_frags, entry_off, entry_off + 1, 0, 64, st);
+  if (e != cudaSuccess) return e;
+  k_long_merge<<<(n_frags + 3) / 4, 128, 0, st>>>(frags, n_frags, entry_off, keys_out, vals_out, piece_base, S,
+                                                  p.seg_length - p.kmer_size + 1, b.sk_votes, b.sk_hash, b.sk_pos, b.sk_strand,
+                                                  b.seg_res);
+  return cudaGetLastError();
+}
 
 #define MM_FOR_EACH_K(X) \
   X(8) X(9) X(10) X(11) X(12) X(13) X(14) X(15) X(16) X(17) X(18) X(19) X(20) X(21) X(22) X(23) X(24) X(25) X(26) X(27) \
