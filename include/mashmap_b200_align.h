@@ -1,0 +1,70 @@
+/*
+ * mashmap_b200_align.h -- C ABI of the device path of mashmap-b200-align (base-level alignment of mappings).
+ *
+ * The reference aligner (src/align, mashmap-align) calls edlibAlign(query, target, k, EDLIB_MODE_HW, EDLIB_TASK_PATH)
+ * once per mapping line on one CPU thread (computeAlignments.hpp:268-269). These entry points run that call for a whole
+ * batch of mappings on the device and give the same edit distance, start, end and edit-op path (DESIGN.md section 10).
+ * Same conventions as mashmap_b200.h: MM_OK or a negative MM_E* code, mm_align_last_error() for the text, no CPU
+ * fallback. Lives in libmashmap_b200.so.
+ */
+#ifndef MASHMAP_B200_ALIGN_H
+#define MASHMAP_B200_ALIGN_H
+
+#include <stdint.h>
+
+#include "mashmap_b200.h"
+
+#ifdef __cplusplus
+extern "C" {
+#endif
+
+/* One edlibAlign call: query = qbases[q_offset, q_offset + q_len) (already oriented: the reverse complement for a '-'
+ * mapping, computeAlignments.hpp:243-248), target = tbases[t_offset, t_offset + t_len) (:230-236), and
+ * k = editDistanceLimit (:256-261; k < 0: unbounded, edlib's doubling from 64, edlib.hxx:173-191). Bytes are compared for
+ * identity only (no additional equalities): N matches N, NUL matches NUL. q_len, t_len >= 1. 32 bytes. */
+typedef struct mm_align_job {
+  uint64_t q_offset;
+  uint64_t t_offset;
+  int32_t q_len;
+  int32_t t_len;
+  int32_t k;
+  int32_t _pad;
+} mm_align_job;
+
+/* EdlibAlignResult for one job (edlib.h:178-228): ed = editDistance (-1: none within k), start / end =
+ * startLocations[0] / endLocations[0] (target coordinates, end inclusive; end = -1 with start = 0 for the path that
+ * inserts the whole query), alignment_length and the path as edit ops (EDLIB_EDOP_*: 0 match, 1 insertion, 2 deletion,
+ * 3 mismatch) at ops[ops_offset, ops_offset + alignment_length). 24 bytes. */
+typedef struct mm_align_result {
+  int32_t ed;
+  int32_t start;
+  int32_t end;
+  int32_t alignment_length;
+  uint64_t ops_offset;
+} mm_align_result;
+
+typedef struct mm_align_ctx mm_align_ctx;
+
+/* Replaces nothing in the reference (it has no device). scratch_bytes bounds the device memory one batch's kernels
+ * use beyond the inputs and the op buffer (0: half the free memory, at most 8 GiB); work that does not fit runs in
+ * waves. */
+int mm_align_ctx_create(int device, uint64_t scratch_bytes, mm_align_ctx **out);
+int mm_align_ctx_destroy(mm_align_ctx *ctx);
+const char *mm_align_last_error(const mm_align_ctx *ctx); /* ctx may be NULL: error of the last failed create */
+
+/* edlibAlign(HW, PATH) (edlib.hxx:141-260) for every job: qbases / tbases in host memory (pinned or not, see
+ * mm_host_alloc). results[n_jobs]; ops[ops_cap]. On MM_ECAPACITY *n_ops holds the op count needed and nothing else is
+ * valid; the sum of q_len + t_len over the jobs is always enough. A batch may hold at most 16 distinct byte values. */
+int mm_align_batch(mm_align_ctx *ctx, const char *qbases, uint64_t n_qbases, const char *tbases, uint64_t n_tbases,
+                   const mm_align_job *jobs, uint64_t n_jobs, mm_align_result *results, uint8_t *ops,
+                   uint64_t ops_cap, uint64_t *n_ops);
+
+/* CUDA-event time in milliseconds of each stage of the last mm_align_batch:
+ * [0] H2D  [1] distance and end (HW pass)  [2] start (reverse SHW pass)  [3] Hirschberg levels  [4] leaf NW + traceback
+ * [5] D2H  [6] whole call on the host clock  [7] number of Hirschberg levels. */
+int mm_align_last_stage_ms(const mm_align_ctx *ctx, float ms[8]);
+
+#ifdef __cplusplus
+}
+#endif
+#endif /* MASHMAP_B200_ALIGN_H */

@@ -386,3 +386,75 @@ class Context:
         arr = (C.c_float * 8)()
         self._L.mm_last_stage_ms(self._h, C.byref(arr))
         return list(arr)
+
+
+# ---- include/mashmap_b200_align.h (base-level alignment of mappings, in the same library) ----------------------------
+
+align_job_dtype = np.dtype([("q_offset", "<u8"), ("t_offset", "<u8"), ("q_len", "<i4"), ("t_len", "<i4"), ("k", "<i4"),
+                            ("_pad", "<i4")])
+align_result_dtype = np.dtype([("ed", "<i4"), ("start", "<i4"), ("end", "<i4"), ("alignment_length", "<i4"),
+                               ("ops_offset", "<u8")])
+assert align_job_dtype.itemsize == 32 and align_result_dtype.itemsize == 24
+
+ALIGN_EXPORTED_SYMBOLS = ["mm_align_ctx_create", "mm_align_ctx_destroy", "mm_align_last_error", "mm_align_batch",
+                          "mm_align_last_stage_ms"]
+
+
+def _align_lib():
+    L = lib()
+    if not getattr(L, "_align_bound", False):
+        vp, u64 = C.c_void_p, C.c_uint64
+        L.mm_align_ctx_create.argtypes = [C.c_int, u64, C.POINTER(vp)]
+        L.mm_align_ctx_destroy.argtypes = [vp]
+        L.mm_align_last_error.argtypes = [vp]
+        L.mm_align_last_error.restype = C.c_char_p
+        L.mm_align_batch.argtypes = [vp, vp, u64, vp, u64, vp, u64, vp, vp, u64, C.POINTER(u64)]
+        L.mm_align_last_stage_ms.argtypes = [vp, C.POINTER(C.c_float * 8)]
+        L._align_bound = True
+    return L
+
+
+class AlignContext:
+    """mm_align_ctx: edlibAlign(HW, PATH) for batches of (query, target, k) on one device."""
+
+    def __init__(self, device=0, scratch_bytes=0):
+        L = _align_lib()
+        self._ctx = C.c_void_p()
+        rc = L.mm_align_ctx_create(int(device), int(scratch_bytes), C.byref(self._ctx))
+        if rc != MM_OK:
+            raise MashmapError(rc, L.mm_align_last_error(None).decode())
+
+    def align(self, qbases, tbases, jobs, ops_cap=None):
+        """jobs: align_job_dtype array. Returns (results, ops) with ops the concatenated edit ops (0 M, 1 I, 2 D, 3 X)."""
+        L = _align_lib()
+        q = np.ascontiguousarray(qbases, dtype=np.uint8)
+        t = np.ascontiguousarray(tbases, dtype=np.uint8)
+        jobs = np.ascontiguousarray(jobs, dtype=align_job_dtype)
+        res = np.zeros(len(jobs), dtype=align_result_dtype)
+        if ops_cap is None:
+            ops_cap = int(jobs["q_len"].astype(np.int64).sum() + jobs["t_len"].astype(np.int64).sum())
+        ops = np.zeros(max(int(ops_cap), 1), dtype=np.uint8)
+        n = C.c_uint64()
+        rc = L.mm_align_batch(self._ctx, _ptr(q), len(q), _ptr(t), len(t), _ptr(jobs), len(jobs), _ptr(res), _ptr(ops),
+                              int(ops_cap), C.byref(n))
+        if rc != MM_OK:
+            err = MashmapError(rc, L.mm_align_last_error(self._ctx).decode())
+            err.n_ops = n.value
+            raise err
+        return res, ops[: n.value]
+
+    def stage_ms(self):
+        a = (C.c_float * 8)()
+        _align_lib().mm_align_last_stage_ms(self._ctx, C.byref(a))
+        return list(a)
+
+    def close(self):
+        if self._ctx:
+            _align_lib().mm_align_ctx_destroy(self._ctx)
+            self._ctx = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
