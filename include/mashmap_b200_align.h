@@ -4,6 +4,7 @@
  * The reference aligner (src/align, mashmap-align) calls edlibAlign(query, target, k, EDLIB_MODE_HW, EDLIB_TASK_PATH)
  * once per mapping line on one CPU thread (computeAlignments.hpp:268-269). These entry points run that call for a whole
  * batch of mappings on the device and give the same edit distance, start, end and edit-op path (DESIGN.md section 10).
+ * They also run edlib's global mode (EDLIB_MODE_NW), which mashmap-b200 --align uses for the exact PAF region.
  * Same conventions as mashmap_b200.h: MM_OK or a negative MM_E* code, mm_align_last_error() for the text, no CPU
  * fallback. Lives in libmashmap_b200.so.
  */
@@ -18,17 +19,23 @@
 extern "C" {
 #endif
 
+/* Alignment modes of a job (edlib's EdlibAlignMode). */
+#define MM_ALIGN_HW 0 /* EDLIB_MODE_HW: the query anywhere in the target (mashmap-b200-align)                         */
+#define MM_ALIGN_NW 1 /* EDLIB_MODE_NW: query and target end to end (mashmap-b200 --align); start 0, end t_len - 1 */
+
 /* One edlibAlign call: query = qbases[q_offset, q_offset + q_len) (already oriented: the reverse complement for a '-'
  * mapping, computeAlignments.hpp:243-248), target = tbases[t_offset, t_offset + t_len) (:230-236), and
  * k = editDistanceLimit (:256-261; k < 0: unbounded, edlib's doubling from 64, edlib.hxx:173-191). Bytes are compared for
- * identity only (no additional equalities): N matches N, NUL matches NUL. q_len, t_len >= 1. 32 bytes. */
+ * identity only (no additional equalities): N matches N, NUL matches NUL. q_len, t_len >= 1. mode: MM_ALIGN_HW or
+ * MM_ALIGN_NW (anything else is MM_EINVAL); a batch may mix them, and a job's result does not depend on the others.
+ * 32 bytes. */
 typedef struct mm_align_job {
   uint64_t q_offset;
   uint64_t t_offset;
   int32_t q_len;
   int32_t t_len;
   int32_t k;
-  int32_t _pad;
+  int32_t mode;
 } mm_align_job;
 
 /* EdlibAlignResult for one job (edlib.h:178-228): ed = editDistance (-1: none within k), start / end =
@@ -52,7 +59,7 @@ int mm_align_ctx_create(int device, uint64_t scratch_bytes, mm_align_ctx **out);
 int mm_align_ctx_destroy(mm_align_ctx *ctx);
 const char *mm_align_last_error(const mm_align_ctx *ctx); /* ctx may be NULL: error of the last failed create */
 
-/* edlibAlign(HW, PATH) (edlib.hxx:141-260) for every job: qbases / tbases in host memory (pinned or not, see
+/* edlibAlign(job.mode, PATH) (edlib.hxx:141-260) for every job: qbases / tbases in host memory (pinned or not, see
  * mm_host_alloc). results[n_jobs]; ops[ops_cap]. On MM_ECAPACITY *n_ops holds the op count needed and nothing else is
  * valid; the sum of q_len + t_len over the jobs is always enough. A batch may hold at most 16 distinct byte values. */
 int mm_align_batch(mm_align_ctx *ctx, const char *qbases, uint64_t n_qbases, const char *tbases, uint64_t n_tbases,
@@ -60,7 +67,7 @@ int mm_align_batch(mm_align_ctx *ctx, const char *qbases, uint64_t n_qbases, con
                    uint64_t ops_cap, uint64_t *n_ops);
 
 /* CUDA-event time in milliseconds of each stage of the last mm_align_batch:
- * [0] H2D  [1] distance and end (HW pass)  [2] start (reverse SHW pass)  [3] Hirschberg levels  [4] leaf NW + traceback
+ * [0] H2D  [1] distance and end (HW and NW passes)  [2] start (reverse SHW pass)  [3] Hirschberg levels  [4] leaf NW + traceback
  * [5] D2H  [6] whole call on the host clock  [7] number of Hirschberg levels. */
 int mm_align_last_stage_ms(const mm_align_ctx *ctx, float ms[8]);
 

@@ -391,7 +391,8 @@ class Context:
 # ---- include/mashmap_b200_align.h (base-level alignment of mappings, in the same library) ----------------------------
 
 align_job_dtype = np.dtype([("q_offset", "<u8"), ("t_offset", "<u8"), ("q_len", "<i4"), ("t_len", "<i4"), ("k", "<i4"),
-                            ("_pad", "<i4")])
+                            ("mode", "<i4")])
+MM_ALIGN_HW, MM_ALIGN_NW = 0, 1  # align_job_dtype["mode"]: edlib's EDLIB_MODE_HW / EDLIB_MODE_NW
 align_result_dtype = np.dtype([("ed", "<i4"), ("start", "<i4"), ("end", "<i4"), ("alignment_length", "<i4"),
                                ("ops_offset", "<u8")])
 assert align_job_dtype.itemsize == 32 and align_result_dtype.itemsize == 24
@@ -415,7 +416,7 @@ def _align_lib():
 
 
 class AlignContext:
-    """mm_align_ctx: edlibAlign(HW, PATH) for batches of (query, target, k) on one device."""
+    """mm_align_ctx: edlibAlign(HW or NW, PATH) for batches of (query, target, k, mode) on one device."""
 
     def __init__(self, device=0, scratch_bytes=0):
         L = _align_lib()

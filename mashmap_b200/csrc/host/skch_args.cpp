@@ -33,6 +33,7 @@ const OptDef kOptions[] = {
     {"reportPercentage", nullptr, false},
     // B200-specific
     {"device", nullptr, true}, {"devices", nullptr, true}, {"hostIndex", nullptr, false}, {"batchBases", nullptr, true}, {"subBatchBases", nullptr, true},
+    {"align", nullptr, false}, {"alignMaxLen", nullptr, true},
 };
 
 [[noreturn]] void usage_error(const std::string &msg)
@@ -81,6 +82,9 @@ void printCmdOptions(const Parameters &p)
   std::cerr << "[mashmap-b200] Mapping output file = " << p.outFileName << std::endl;
   std::cerr << "[mashmap-b200] Filter mode = " << p.filterMode << " (1 = map, 2 = one-to-one, 3 = none)" << std::endl;
   std::cerr << "[mashmap-b200] Host threads = " << p.threads << ", CUDA device = " << p.device << std::endl;
+  if (p.align)
+    std::cerr << "[mashmap-b200] Alignment = NM:i and cg:Z from edlib NW over each mapping's region, regions up to "
+              << p.align_max_len << " bp" << std::endl;
 }
 
 void parseandSave(int argc, char **argv, Parameters &parameters)
@@ -108,8 +112,19 @@ void parseandSave(int argc, char **argv, Parameters &parameters)
 
   if (found("version")) { std::cerr << fixed::VERSION << std::endl; exit(0); }
   if (found("help")) {
-    std::cerr << "mashmap-b200 -r ref.fa -q seq.fq [OPTIONS]   (options as in MashMap v3.1.3, plus --device N | --devices 0-7, --batchBases N)" << std::endl;
+    std::cerr << "mashmap-b200 -r ref.fa -q seq.fq [OPTIONS]   (options as in MashMap v3.1.3, plus --device N | --devices 0-7, --batchBases N,\n"
+                 "    --align [--alignMaxLen N, default 100000]: append NM:i and cg:Z (edlib NW over each mapping's region, on the GPU))" << std::endl;
     exit(0);
+  }
+  parameters.align = found("align");
+  if (parameters.align && found("legacy"))
+    usage_error("ERROR, --align writes PAF tags and cannot be combined with --legacy (mashmap-b200-align aligns --legacy mapping files)");
+  if (found("alignMaxLen")) {
+    const std::string &v = opt["alignMaxLen"];
+    if (!parameters.align) usage_error("ERROR, --alignMaxLen is given without --align");
+    if (v.empty() || v.size() > 10 || v.find_first_not_of("0123456789") != std::string::npos || std::stoll(v) < 1)
+      usage_error("ERROR, --alignMaxLen needs a positive whole number of bases, not '" + v + "'");
+    parameters.align_max_len = std::stoll(v);
   }
   if (!found("ref") && !found("refList")) usage_error("ERROR, skch::parseandSave, Provide reference file(s)");
 

@@ -300,8 +300,18 @@ Sketch::Sketch(const Parameters &p, const std::vector<ContigInfo> &contigs, cons
     : metadata(contigs), param(p)
 {
   sequencesByFileInfo.push_back((int)contigs.size());
+  if (param.align)
+    for (size_t i = 0; i < seqs.size(); i++) keepForAlign(seqs[i], (size_t)metadata[i].len);
   buildFromMemory(seqs);
   finish();
+}
+
+void Sketch::keepForAlign(const char *seq, size_t len)
+{
+  const uint64_t at = refNibbles_.size();
+  refNibbleOffsets_.push_back(at);
+  refNibbles_.resize(at + (len + 1) / 2);
+  seqio::pack_bases(seq, len, refNibbles_.data() + at);
 }
 
 Sketch::Sketch(const Parameters &p, const std::vector<ContigInfo> &contigs, MI_Type &&minmers)
@@ -390,6 +400,7 @@ void Sketch::build()
                                           [&](const std::string &name, const std::string &seq) {
                                             offset_t len = seq.length();
                                             metadata.push_back(ContigInfo{name, len});
+                                            if (param.align) keepForAlign(seq.data(), seq.size());
                                             if (on_device) {  // every contig, also the short ones: seqId = position in metadata
                                               if (textBytes + seq.size() + 64 > textCap) {
                                                 textCap = std::max<uint64_t>(textCap * 2, textBytes + seq.size() + (64ULL << 20));

@@ -81,6 +81,11 @@ class Sketch {
   const std::vector<uint64_t> &deviceTextOffsets() const { return deviceTextOffsets_; }
   void deviceBuildDone(int freq_threshold) const;  // releases the text, records the threshold
 
+  /* --align: the bases of contig i (metadata[i]) as nibbles (seqio::pack_bases: ACGT, everything else N), base 0 in the
+   * low nibble of the first byte. Read with the contigs in every index mode and kept for the whole run (not kept by the
+   * constructor that takes a minmer list). */
+  const uint8_t *refNibbles(seqno_t i) const { return refNibbles_.data() + refNibbleOffsets_[(size_t)i]; }
+
   int getFreqThreshold() const { return freqThreshold; }   // winSketch.hpp:483-486
   bool isFreqSeed(hash_t h) const;                         // winSketch.hpp:506-509
   bool isMinmerIndexEnd(MI_Type::const_iterator it) const { return it == minmerIndex.end(); }
@@ -97,8 +102,11 @@ class Sketch {
   bool saving_ = false;
   mutable char *deviceText_ = nullptr;           // contigs back to back (text), until the device has built the index
   mutable std::vector<uint64_t> deviceTextOffsets_;
+  BigVec<uint8_t> refNibbles_;                   // --align only
+  std::vector<uint64_t> refNibbleOffsets_;       // byte offset of each contig in refNibbles_
 
   void build();
+  void keepForAlign(const char *seq, size_t len);  // appends a contig to refNibbles_
   void buildFromMemory(const std::vector<const char *> &seqs);
   void finish();
   void index();

@@ -259,6 +259,7 @@ BatchMapper::BatchMapper(const Parameters &p, const Sketch &refsketch) : param(p
       g->gate = new Gate();
       for (int l = 0; l < g->nLanes; l++) mm_ctx_set_phase_hook(g->lanes[l].ctx, &BatchMapper::phaseHook, g->gate);
     }
+    if (param.align) g->aligner = new MappingAligner(param, refSketch, g->device);
   }
 }
 
@@ -266,6 +267,7 @@ BatchMapper::~BatchMapper()
 {
   for (DeviceGroup *g : groups) {
     delete g->tailPool;
+    delete g->aligner;
     for (int l = 0; l < MAX_LANES; l++) { g->lanes[l].segRes.release(); g->lanes[l].cands.release(); g->lanes[l].loci.release(); }
     for (int l = g->nLanes - 1; l >= 1; l--) mm_ctx_destroy(g->lanes[l].ctx);
     if (g->owner && g->owner != ctx) mm_ctx_destroy(g->owner);
@@ -319,6 +321,42 @@ void BatchMapper::addRead(ReadBatch &b, const std::string &name, const char *seq
 void BatchMapper::finalizeOneToOne(MappingResultsVector_t &allReadMappings, const std::vector<ContigInfo> &qmetadata, std::string &paf) const
 {
   tail_->finalizeOneToOne(allReadMappings, qmetadata, paf);
+}
+
+void BatchMapper::alignOneToOne(const MappingResultsVector_t &maps, const std::function<const uint8_t *(seqno_t)> &query, std::string &paf)
+{
+  const size_t n = maps.size(), G = groups.size();
+  std::vector<MappingAligner::Item> items(n);
+  for (size_t i = 0; i < n; i++) items[i] = {&maps[i], query(maps[i].querySeqId)};
+  std::vector<std::vector<std::string>> tags(G);
+  auto run = [&](size_t g) {
+    const size_t lo = n * g / G, hi = n * (g + 1) / G;
+    groups[g]->aligner->align(items.data() + lo, hi - lo, tags[g]);
+  };
+  std::vector<std::thread> others;
+  for (size_t g = 1; g < G; g++) others.emplace_back(run, g);
+  run(0);
+  for (auto &t : others) t.join();
+  std::vector<std::string> all;
+  all.reserve(n);
+  for (auto &v : tags)
+    for (auto &t : v) all.push_back(std::move(t));
+  appendTags(paf, all.data());
+}
+
+void BatchMapper::reportAlignment() const
+{
+  uint64_t aligned = 0, tooLong = 0, unaligned = 0, bases = 0;
+  double seconds = 0;
+  for (const DeviceGroup *g : groups) {
+    aligned += g->aligner->aligned; tooLong += g->aligner->tooLong; unaligned += g->aligner->unaligned;
+    bases += g->aligner->bases; seconds += g->aligner->seconds;
+  }
+  std::cerr << "[mashmap-b200::align] " << aligned << " mappings aligned (edlib NW over " << bases << " query + target bases) in "
+            << seconds << " s, summed over " << groups.size() << " device(s); " << tooLong
+            << " mappings with a region longer than --alignMaxLen " << param.align_max_len << " printed without NM:i / cg:Z";
+  if (unaligned) std::cerr << "; " << unaligned << " without an alignment (empty regions)";
+  std::cerr << std::endl;
 }
 
 /* The three stages of one part (reads [r0, r1) of the batch) on one lane (= one device context with its own stream
@@ -406,6 +444,18 @@ void BatchMapper::laneFinish(DeviceGroup &g, Lane &ln, const ReadBatch &b, std::
   };
   g.tailPool->run(nthreads, worker);
   ln.secTail += since(t0);
+  if (text && g.aligner) {  // --align: the part's mappings in output order, then their tags onto the reads' lines
+    std::vector<MappingAligner::Item> items;
+    for (size_t r = r0; r < r1; r++)
+      for (const MappingResult &m : results[r]) items.push_back({&m, b.nibbles(b.segs[b.reads[r].first_seg].offset)});
+    std::vector<std::string> tags;
+    g.aligner->align(items.data(), items.size(), tags);
+    size_t k = 0;
+    for (size_t r = r0; r < r1; r++) {
+      appendTags((*text)[r], tags.data() + k);
+      k += results[r].size();
+    }
+  }
   static const bool trace = getenv("MM_TRACE") != nullptr;
   if (trace)
     fprintf(stderr, "[trace] lane %d reads %zu-%zu segs %zu: upload %.2f ms (h2d %.2f) compute %.2f ms (kernels %.2f [k1 %.2f k2 %.2f k3 %.2f: prep %.2f scan %.2f]) "
@@ -578,9 +628,25 @@ struct Map::Impl {
     if (workerActive) { worker.join(); workerActive = false; }
   }
 
+  // --align, -f one-to-one: the nibbles of every mapped query, kept for the run-wide alignment (query id -> offset)
+  BigVec<uint8_t> queryNibbles;
+  std::vector<uint64_t> queryNibbleAt;
+
+  void keepQueries(const ReadBatch &b)
+  {
+    for (const ReadRec &rd : b.reads) {
+      const uint64_t at = queryNibbles.size(), bytes = ((uint64_t)rd.len + 1) / 2;
+      queryNibbles.resize(at + bytes);
+      memcpy(queryNibbles.data() + at, b.nibbles(b.segs[rd.first_seg].offset), bytes);
+      if (queryNibbleAt.size() <= (size_t)rd.seqCounter) queryNibbleAt.resize((size_t)rd.seqCounter + 1);
+      queryNibbleAt[(size_t)rd.seqCounter] = at;
+    }
+  }
+
   void mapAndWrite(ReadBatch &b)
   {
     const bool report_now = param.filterMode != filter::ONETOONE;
+    if (!report_now && param.align) keepQueries(b);
     bm.mapBatch(b, results, report_now ? &text : nullptr, &qmetadata);
     for (size_t r = 0; r < results.size(); r++) {  // mapModuleHandleOutput (computeMap.hpp:724-747), in input order
       if (!results[r].empty()) totalReadsMapped++;
@@ -716,6 +782,8 @@ struct Map::Impl {
     if (param.filterMode == filter::ONETOONE) {  // :358-405
       std::string paf;
       bm.finalizeOneToOne(allReadMappings, qmetadata, paf);
+      if (param.align)
+        bm.alignOneToOne(allReadMappings, [&](seqno_t id) { return queryNibbles.data() + queryNibbleAt[(size_t)id]; }, paf);
       outstrm << paf;
       if (processMappingResults != nullptr)
         for (auto &e : allReadMappings) processMappingResults(e);
@@ -724,6 +792,7 @@ struct Map::Impl {
     std::cerr << "[mashmap-b200::skch::Map::mapQuery] count of mapped reads = " << totalReadsMapped
               << ", reads qualified for mapping = " << totalReadsPicked << ", total input reads = " << seqCounter
               << ", total input bp = " << self.totalQueryBases << std::endl;
+    if (param.align) bm.reportAlignment();
   }
 };
 

@@ -29,6 +29,7 @@
 #include <unordered_map>
 #include <vector>
 
+#include "skch_align.hpp"
 #include "skch_index.hpp"
 #include "skch_tail.hpp"
 #include "skch_types.hpp"
@@ -72,6 +73,11 @@ class BatchMapper {
    * ref start) and formatted. Works on whatever set the caller hands over -- the mappings of one process, or the
    * records gathered from all ranks (MappingResult is a POD, base_types.hpp:152-153). */
   void finalizeOneToOne(MappingResultsVector_t &allReadMappings, const std::vector<ContigInfo> &qmetadata, std::string &paf) const;
+  /* --align after finalizeOneToOne: appends NM:i / cg:Z to the lines of paf, which are maps in order; query(id) = the
+   * nibbles of query id. The mappings are split into one contiguous slice per device. (Outside one-to-one mode mapBatch
+   * aligns each part after its host tail.) */
+  void alignOneToOne(const MappingResultsVector_t &maps, const std::function<const uint8_t *(seqno_t)> &query, std::string &paf);
+  void reportAlignment() const;  // --align: totals of the run to stderr
 
   int getRefGroup(const std::string &seqName) const;  // computeMap.hpp:164-177
   const std::vector<int> &refGroups() const { return refIdGroup; }
@@ -139,6 +145,7 @@ class BatchMapper {
     int nLanes = 1;
     Gate *gate = nullptr;
     WorkerPool *tailPool = nullptr;  // persistent threads of the per-read host tail
+    MappingAligner *aligner = nullptr;  // --align; used by the thread that finishes this device's parts
     bool blockingWaits = false;  // host waits sleep on events instead of spinning (few CPUs per device)
     int tailThreads = 1;
   };

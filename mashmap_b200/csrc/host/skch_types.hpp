@@ -112,6 +112,10 @@ struct Parameters {
   std::vector<int> devices;       // --devices 0-7 / 0,2,5: several GPUs driven by this process (empty = {device})
   uint64_t batch_bases = 1ULL << 30;  // query bases per device batch
   uint64_t sub_batch_bases = 640ULL << 20;  // a batch is mapped as sub-batches of this size on two pipelined lanes
+  bool align = false;             // --align: NM:i / cg:Z tags from edlib NW over each printed mapping's region (on the device)
+  // --alignMaxLen: longer query or target regions are printed without the tags. One warp aligns one mapping without a band:
+  // 100 kb x 100 kb takes 1.9 s, 1 Mbp x 1 Mbp 341 s (H100 80GB HBM3, 400 W; scripts/map_align_perf.py)
+  int64_t align_max_len = 100000;
 };
 
 namespace fixed {  // map_parameters.hpp:86-102

@@ -1,6 +1,7 @@
 /*
  * mm_align.cu -- the device path of mashmap-b200-align: edlibAlign(query, target, k, EDLIB_MODE_HW, EDLIB_TASK_PATH)
- * (reference src/common/edlib.hxx:141-260, called from computeAlignments.hpp:268) for a batch of mappings.
+ * (reference src/common/edlib.hxx:141-260, called from computeAlignments.hpp:268) for a batch of mappings, and of
+ * mashmap-b200 --align: the same call in EDLIB_MODE_NW.
  *
  * edlib bands its Myers bit-vector computation (Ukkonen); every decision it takes depends only on exact scores <= k, and
  * banded scores never underestimate, so an unbanded computation takes the same decisions (DESIGN.md section 10; pinned by
@@ -13,10 +14,15 @@
  *      left, diagonal) when (2*8+4)*ceil(Q/64)*T + 8*T < 1 MiB, otherwise one Hirschberg split (target at T/2; first row
  *      whose forward + reverse scores sum to the score, then the -1 boundary, then the Q-1 boundary) and recursion.
  *
+ * Global mode (EDLIB_MODE_NW, edlib.hxx:193-248), for jobs with mode MM_ALIGN_NW:
+ *   1'. ed = the NW score at (Q-1, T-1) (-1 if k >= 0 and ed > k); start = 0, end = T-1, no SHW pass.
+ *   3'. path = rule 3 over the whole target with score ed.
+ *
  * Kernels, all one warp per problem with the 64-bit blocks of the query spread over the lanes (lane l owns a contiguous
  * run of blocks) and a wavefront along the target (lane l works on column s - l at step s; the horizontal carry moves
  * one lane down per step through a shuffle):
  *   k_align_hw      (a) rule 1              k_align_shw  (b) rule 2
+ *   k_align_nw      (a) rule 1'
  *   k_align_hirsch  (c) one Hirschberg level: forward and reverse NW boundary columns, then the split row
  *   k_align_leaf    (d) NW with every column's blocks stored, then the traceback to edit ops
  * The host walks the levels (the next level's list keeps sub-problems in alignment order) and schedules the leaves'
@@ -36,7 +42,7 @@
 namespace {
 
 constexpr unsigned FULL = 0xffffffffu;
-enum { M_HW = 0, M_SHW = 1, M_COL = 2, M_STORE = 3 };
+enum { M_HW = 0, M_SHW = 1, M_COL = 2, M_STORE = 3, M_NW = 4 };
 
 struct Prob {
   uint64_t q, t;     // forward substrings: d_q + q, d_t + t
@@ -69,8 +75,9 @@ __device__ void build_peq(uint64_t *peq, const uint8_t *q, int ql, bool rev, con
 
 /* One Myers sweep of a query (given by its Peq) over tl target columns. Block state: P / M vertical-delta words and the
  * score of the block's bottom row. M_HW / M_SHW track the last query row and return its minimum over the columns
- * (smallest column for HW, largest for SHW) in best / bestpos on every lane; M_STORE keeps every column's blocks at
- * [c * nb + b] for the traceback. The top boundary is 0 for HW (free start) and +1 per column otherwise. */
+ * (smallest column for HW, largest for SHW) in best / bestpos on every lane; M_NW tracks it the same way and returns its
+ * value at the last column; M_STORE keeps every column's blocks at [c * nb + b] for the traceback. The top boundary is 0
+ * for HW (free start) and +1 per column otherwise. */
 template <int MODE>
 __device__ void sweep(const uint64_t *peq, int ql, const uint8_t *t, int tl, bool trev, const uint8_t *code,
                       uint64_t *Ps, uint64_t *Ms, int *Ss, int lane, int &best, int &bestpos)
@@ -81,6 +88,7 @@ __device__ void sweep(const uint64_t *peq, int ql, const uint8_t *t, int tl, boo
   const int b0 = lane * bpl, b1 = min(nb, b0 + bpl);
   const int lastr = (ql - 1) & 63;
   const int top = MODE == M_HW ? 0 : 1;
+  constexpr bool track = MODE == M_HW || MODE == M_SHW || MODE == M_NW;
   if (MODE != M_STORE)
     for (int b = b0; b < b1; b++) { Ps[b] = ~0ull; Ms[b] = 0; Ss[b] = 64 * (b + 1); }
   int row = ql;  // last query row at column -1
@@ -111,7 +119,7 @@ __device__ void sweep(const uint64_t *peq, int ql, const uint8_t *t, int tl, boo
         uint64_t Ph = Mv | ~(Xh | Pv);
         uint64_t Mh = Pv & Xh;
         const int hout = (int)(Ph >> 63) - (int)(Mh >> 63);
-        if ((MODE == M_HW || MODE == M_SHW) && b == nb - 1)
+        if (track && b == nb - 1)
           row += (int)((Ph >> lastr) & 1) - (int)((Mh >> lastr) & 1);
         Ph <<= 1;
         Mh <<= 1;
@@ -129,8 +137,8 @@ __device__ void sweep(const uint64_t *peq, int ql, const uint8_t *t, int tl, boo
         h = hout;
       }
       carry = h;
-      if ((MODE == M_HW || MODE == M_SHW) && b1 == nb && b0 < b1) {
-        if (MODE == M_HW ? row < best : row <= best) { best = row; bestpos = c; }
+      if (track && b1 == nb && b0 < b1) {
+        if (MODE == M_NW ? c == tl - 1 : MODE == M_HW ? row < best : row <= best) { best = row; bestpos = c; }
       }
     }
   }
@@ -187,6 +195,24 @@ __global__ void k_align_hw(const Prob *probs, int n, const uint8_t *dq, const ui
   if (lane == 0) {
     out_ed[p.res] = best <= kk ? best : -1;
     out_end[p.res] = best <= kk ? pos : -1;
+  }
+}
+
+/* rule 1': edlib's NW distance accepts the exact score when it is <= k (myersCalcEditDistanceNW, edlib.hxx:695-902) */
+__global__ void k_align_nw(const Prob *probs, int n, const uint8_t *dq, const uint8_t *dt, const uint8_t *code, int nsym,
+                           uint8_t *scratch, int *out_ed, int *out_end)
+{
+  const int w = (int)((blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+  if (w >= n) return;
+  const Prob p = probs[w];
+  Scratch sc(scratch + p.scratch, p.ql, nsym, 1);
+  build_peq(sc.peq, dq + p.q, p.ql, false, code, nsym, lane);
+  int best, pos;
+  sweep<M_NW>(sc.peq, p.ql, dt + p.t, p.tl, false, code, sc.P, sc.M, sc.S, lane, best, pos);
+  const bool ok = p.k < 0 || best <= p.k;
+  if (lane == 0) {
+    out_ed[p.res] = ok ? best : -1;
+    out_end[p.res] = ok ? pos : -1;
   }
 }
 
@@ -447,6 +473,10 @@ int mm_align_batch(mm_align_ctx *c, const char *qbases, uint64_t n_q, const char
       c->err = "job " + std::to_string(j) + ": empty or out-of-range region";
       return MM_EINVAL;
     }
+    if (b.mode != MM_ALIGN_HW && b.mode != MM_ALIGN_NW) {
+      c->err = "job " + std::to_string(j) + ": mode " + std::to_string(b.mode) + " is neither MM_ALIGN_HW nor MM_ALIGN_NW";
+      return MM_EINVAL;
+    }
   }
   if (n_jobs == 0) return MM_OK;
   // symbols: every distinct byte of the batch gets a code (equality is byte identity)
@@ -474,28 +504,35 @@ int mm_align_batch(mm_align_ctx *c, const char *qbases, uint64_t n_q, const char
     const uint8_t *dq = c->q.as<uint8_t>(), *dt = c->t.as<uint8_t>(), *dc = c->code.as<uint8_t>();
     auto sweep_bytes = [nsym](const Prob &p) { return scratch_bytes(p.ql, nsym, 1, 0); };
 
-    // (a) distance and end
+    // (a) distance and end; HW and NW jobs in launches of their own
     std::vector<int> ed(n_jobs), end(n_jobs), start(n_jobs, 0);
     {
       StageTimer tm(c, 1);
-      std::vector<Prob> probs(n_jobs);
+      std::vector<Prob> hw, nw;
       for (uint64_t j = 0; j < n_jobs; j++)
-        probs[j] = Prob{jobs[j].q_offset, jobs[j].t_offset, jobs[j].q_len, jobs[j].t_len, jobs[j].k, (int)j, 0, 0};
+        (jobs[j].mode == MM_ALIGN_NW ? nw : hw)
+            .push_back(Prob{jobs[j].q_offset, jobs[j].t_offset, jobs[j].q_len, jobs[j].t_len, jobs[j].k, (int)j, 0, 0});
       ck(c, c->out_a.ensure(n_jobs * 4), "output allocation");
       ck(c, c->out_b.ensure(n_jobs * 4), "output allocation");
-      run_waves(c, probs, sweep_bytes, [&](const Prob *dp, int n, int grid, int blk) {
-        k_align_hw<<<grid, blk, 0, c->st>>>(dp, n, dq, dt, dc, nsym, c->scratch.as<uint8_t>(), c->out_a.as<int>(),
-                                            c->out_b.as<int>());
-      });
+      if (!hw.empty())
+        run_waves(c, hw, sweep_bytes, [&](const Prob *dp, int n, int grid, int blk) {
+          k_align_hw<<<grid, blk, 0, c->st>>>(dp, n, dq, dt, dc, nsym, c->scratch.as<uint8_t>(), c->out_a.as<int>(),
+                                              c->out_b.as<int>());
+        });
+      if (!nw.empty())
+        run_waves(c, nw, sweep_bytes, [&](const Prob *dp, int n, int grid, int blk) {
+          k_align_nw<<<grid, blk, 0, c->st>>>(dp, n, dq, dt, dc, nsym, c->scratch.as<uint8_t>(), c->out_a.as<int>(),
+                                              c->out_b.as<int>());
+        });
       ck(c, cudaMemcpyAsync(ed.data(), c->out_a.p, n_jobs * 4, cudaMemcpyDeviceToHost, c->st), "D2H");
       ck(c, cudaMemcpyAsync(end.data(), c->out_b.p, n_jobs * 4, cudaMemcpyDeviceToHost, c->st), "D2H");
     }
-    // (b) start; end = -1 (the whole query inserted before the target) has start 0
+    // (b) start of the HW jobs; end = -1 (the whole query inserted before the target) has start 0, as every NW job has
     {
       StageTimer tm(c, 2);
       std::vector<Prob> probs;
       for (uint64_t j = 0; j < n_jobs; j++)
-        if (ed[j] >= 0 && end[j] >= 0)
+        if (jobs[j].mode == MM_ALIGN_HW && ed[j] >= 0 && end[j] >= 0)
           probs.push_back(Prob{jobs[j].q_offset, jobs[j].t_offset, jobs[j].q_len, end[j] + 1, 0, (int)j, 0, 0});
       if (!probs.empty()) {
         run_waves(c, probs, sweep_bytes, [&](const Prob *dp, int n, int grid, int blk) {
