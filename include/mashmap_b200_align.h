@@ -23,6 +23,11 @@ extern "C" {
 #define MM_ALIGN_HW 0 /* EDLIB_MODE_HW: the query anywhere in the target (mashmap-b200-align)                         */
 #define MM_ALIGN_NW 1 /* EDLIB_MODE_NW: query and target end to end (mashmap-b200 --align); start 0, end t_len - 1 */
 
+/* Routing of NW sub-problems: the NW distance of an MM_ALIGN_NW job and every Hirschberg node (both modes) whose
+ * max(query length, target length) is at least this run banded, one CTA per sweep; shorter ones run unbanded, one warp
+ * per problem. Both give edlib's results (DESIGN.md section 10); the rule reads only the sub-problem's own size. */
+#define MM_ALIGN_BAND_MIN_LEN (32 * 1024)
+
 /* One edlibAlign call: query = qbases[q_offset, q_offset + q_len) (already oriented: the reverse complement for a '-'
  * mapping, computeAlignments.hpp:243-248), target = tbases[t_offset, t_offset + t_len) (:230-236), and
  * k = editDistanceLimit (:256-261; k < 0: unbounded, edlib's doubling from 64, edlib.hxx:173-191). Bytes are compared for

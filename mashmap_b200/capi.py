@@ -393,6 +393,7 @@ class Context:
 align_job_dtype = np.dtype([("q_offset", "<u8"), ("t_offset", "<u8"), ("q_len", "<i4"), ("t_len", "<i4"), ("k", "<i4"),
                             ("mode", "<i4")])
 MM_ALIGN_HW, MM_ALIGN_NW = 0, 1  # align_job_dtype["mode"]: edlib's EDLIB_MODE_HW / EDLIB_MODE_NW
+MM_ALIGN_BAND_MIN_LEN = 32 * 1024  # NW sub-problems with max(q_len, t_len) >= this run banded, one CTA per sweep
 align_result_dtype = np.dtype([("ed", "<i4"), ("start", "<i4"), ("end", "<i4"), ("alignment_length", "<i4"),
                                ("ops_offset", "<u8")])
 assert align_job_dtype.itemsize == 32 and align_result_dtype.itemsize == 24

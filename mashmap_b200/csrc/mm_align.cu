@@ -27,7 +27,13 @@
  *   k_align_leaf    (d) NW with every column's blocks stored, then the traceback to edit ops
  * The host walks the levels (the next level's list keeps sub-problems in alignment order) and schedules the leaves'
  * block storage in waves under the context's scratch budget.
+ *
+ * Long sub-problems (max(Q, T) >= MM_ALIGN_BAND_MIN_LEN; leaves never are) run banded, one CTA per sweep, sized to the
+ * band:
+ *   k_band_nw       (a) rule 1' for one pass of a k schedule the host drives
+ *   k_band_col      (c) one half-column of a Hirschberg node (two CTAs per node), then k_band_split for the split row
  */
+#include <cstdlib>
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -56,11 +62,13 @@ struct Prob {
 __host__ __device__ inline int nblocks(int ql) { return (ql + 63) >> 6; }
 __host__ __device__ inline uint64_t al16(uint64_t x) { return (x + 15) & ~(uint64_t)15; }
 
-/* Peq[s * nb + b]: bit i set when query row 64b + i holds symbol s; rows past the query (padding) match everything. */
-__device__ void build_peq(uint64_t *peq, const uint8_t *q, int ql, bool rev, const uint8_t *code, int nsym, int lane)
+/* Peq[s * nb + b]: bit i set when query row 64b + i holds symbol s; rows past the query (padding) match everything.
+ * The calling warp builds blocks b0, b0 + bstep, ... (the whole query by default). */
+__device__ void build_peq(uint64_t *peq, const uint8_t *q, int ql, bool rev, const uint8_t *code, int nsym, int lane,
+                          int b0 = 0, int bstep = 1)
 {
   const int nb = nblocks(ql);
-  for (int b = 0; b < nb; b++) {
+  for (int b = b0; b < nb; b += bstep) {
     const int r0 = b * 64 + lane, r1 = r0 + 32;
     const int c0 = r0 < ql ? code[rev ? q[ql - 1 - r0] : q[r0]] : -1;
     const int c1 = r1 < ql ? code[rev ? q[ql - 1 - r1] : q[r1]] : -1;
@@ -175,7 +183,7 @@ struct Scratch {  // carving of one problem's scratch
     S = (int *)(M + cols * nb);
   }
 };
-__host__ inline uint64_t scratch_bytes(int ql, int nsym, uint64_t cols, uint64_t extra)
+__host__ __device__ inline uint64_t scratch_bytes(int ql, int nsym, uint64_t cols, uint64_t extra)
 {
   const uint64_t nb = (uint64_t)nblocks(ql);
   return al16(nsym * nb * 8) + al16(cols * nb * 20) + al16(extra);
@@ -229,6 +237,24 @@ __global__ void k_align_shw(const Prob *probs, int n, const uint8_t *dq, const u
   if (lane == 0) out_start[p.res] = (p.tl - 1) - pos;
 }
 
+/* The Hirschberg split of a node from its boundary columns (left[i] = NW(query[0..i], target[0..lw)), right[i] =
+ * NW(query[i..Q), target[lw..T))): the first row in ascending order whose scores sum to the node's score, then the -1
+ * boundary, then the Q-1 boundary. {split row, upper-left score, lower-right score, 1}, or {0, 0, 0, 0} when no row
+ * sums to the score; the same on every lane. */
+__device__ int4 split_row(const int *left, const int *right, int Q, int lw, int rw, int best, int lane)
+{
+  int split = INT_MIN, ls = 0, rs = 0;
+  for (int base = 0; base < Q - 1 && split == INT_MIN; base += 32) {
+    const int i = base + lane;
+    const bool hit = i < Q - 1 && left[i] + right[i + 1] == best;
+    const unsigned m = __ballot_sync(FULL, hit);
+    if (m) { split = base + __ffs(m) - 1; ls = left[split]; rs = right[split + 1]; }
+  }
+  if (split == INT_MIN && lw + right[0] == best) { split = -1; ls = lw; rs = right[0]; }
+  if (split == INT_MIN && left[Q - 1] + rw == best) { split = Q - 1; ls = left[Q - 1]; rs = rw; }
+  return split == INT_MIN ? make_int4(0, 0, 0, 0) : make_int4(split, ls, rs, 1);
+}
+
 /* out[res] = {split row (-1 .. ql-1), upper-left score, lower-right score, 1} or {.., 0} when no row sums to the score */
 __global__ void k_align_hirsch(const Prob *probs, int n, const uint8_t *dq, const uint8_t *dt, const uint8_t *code,
                                int nsym, uint8_t *scratch, int4 *out)
@@ -251,16 +277,8 @@ __global__ void k_align_hirsch(const Prob *probs, int n, const uint8_t *dq, cons
   build_peq(sc.peq, dq + p.q, Q, true, code, nsym, lane);
   sweep<M_COL>(sc.peq, Q, dt + p.t + lw, rw, true, code, sc.P, sc.M, sc.S, lane, dummy0, dummy1);
   write_column(sc.P, sc.M, sc.S, Q, right, true, lane);  // right[i] = NW(query[i..Q), target[lw..T))
-  int split = INT_MIN, ls = 0, rs = 0;
-  for (int base = 0; base < Q - 1 && split == INT_MIN; base += 32) {
-    const int i = base + lane;
-    const bool hit = i < Q - 1 && left[i] + right[i + 1] == best;
-    const unsigned m = __ballot_sync(FULL, hit);
-    if (m) { split = base + __ffs(m) - 1; ls = left[split]; rs = right[split + 1]; }
-  }
-  if (split == INT_MIN && lw + right[0] == best) { split = -1; ls = lw; rs = right[0]; }
-  if (split == INT_MIN && left[Q - 1] + rw == best) { split = Q - 1; ls = left[Q - 1]; rs = rw; }
-  if (lane == 0) out[p.res] = split == INT_MIN ? make_int4(0, 0, 0, 0) : make_int4(split, ls, rs, 1);
+  const int4 r = split_row(left, right, Q, lw, rw, best, lane);
+  if (lane == 0) out[p.res] = r;
 }
 
 /* NW with every column stored, then the traceback (edlib's move preference) from (Q-1, T-1); ops come out in path order */
@@ -306,6 +324,233 @@ __global__ void k_align_leaf(const Prob *probs, int n, const uint8_t *dq, const 
   if (lane == 0) out_n[p.res] = cnt;
 }
 
+/* ---- long sub-problems (max(Q, T) >= MM_ALIGN_BAND_MIN_LEN): a static band, one CTA per sweep ----------------------
+ * Band rule (DESIGN.md section 10): with d = i - j and D = Q - T, a cell lies on a path of cost <= k only if
+ * |d| + |d - D| <= k, i.e. d in [min(0, D) - w, max(0, D) + w] with w = floor((k - |D|) / 2). Per column the rows of
+ * the band form one range whose first and last block are non-decreasing in j and advance by at most one block per
+ * column. Blocks outside the range are not computed; scores never underestimate (the first computed block takes the
+ * +1 top boundary, a block entering at the bottom starts from the block above plus 64), and a cell whose optimal path
+ * stays in the band is exact. The reversed sweep of a Hirschberg node uses the same rule in reversed coordinates. */
+constexpr int BAND_BPT = 8;            // blocks a thread keeps in registers over a column tile
+constexpr int BAND_INF = 0x3fffffff;   // score of a row outside the band; two of them still sum without overflow
+
+struct Band {
+  long long dmin, dmax;
+  int Q;
+  __host__ __device__ Band(int Q_, int T, int k) : Q(Q_)
+  {
+    const long long D = (long long)Q_ - T, ad = D < 0 ? -D : D;
+    const long long w = k > ad ? (k - ad) / 2 : 0;
+    dmin = (D < 0 ? D : 0) - w;
+    dmax = (D > 0 ? D : 0) + w;
+  }
+  __host__ __device__ int first(long long j) const { const long long lo = j + dmin; return lo <= 0 ? 0 : (int)(lo >> 6); }
+  __host__ __device__ int last(long long j) const { const long long hi = j + dmax; return (int)((hi < Q - 1 ? hi : Q - 1) >> 6); }
+};
+
+__device__ __forceinline__ int myers_block(uint64_t &Pv, uint64_t &Mv, int &sc, uint64_t Eq, int h)
+{
+  const uint64_t Xv = Eq | Mv;
+  if (h < 0) Eq |= 1ull;
+  const uint64_t Xh = (((Eq & Pv) + Pv) ^ Pv) | Eq;
+  uint64_t Ph = Mv | ~(Xh | Pv);
+  uint64_t Mh = Pv & Xh;
+  const int hout = (int)(Ph >> 63) - (int)(Mh >> 63);
+  Ph <<= 1;
+  Mh <<= 1;
+  if (h < 0) Mh |= 1ull;
+  else if (h > 0) Ph |= 1ull;
+  Pv = Mh | ~(Xv | Ph);
+  Mv = Ph & Xv;
+  sc += hout;
+  return hout;
+}
+
+/* score of row 64b + r from a block's P / M words and bottom-row score */
+__device__ __forceinline__ int block_row(uint64_t P, uint64_t M, int S, int r)
+{
+  const uint64_t above = r == 63 ? 0ull : (~0ull << (r + 1));
+  return S - __popcll(P & above) + __popcll(M & above);
+}
+
+/* Peq of the whole query, built by all warps of the CTA */
+__device__ void build_peq_cta(uint64_t *peq, const uint8_t *q, int ql, bool rev, const uint8_t *code, int nsym)
+{
+  build_peq(peq, q, ql, rev, code, nsym, threadIdx.x & 31, threadIdx.x >> 5, blockDim.x >> 5);
+  __syncthreads();
+}
+
+/* Banded sweep of a query (its Peq, nb blocks) over ncols target columns (read backwards when trev) by the whole CTA.
+ * Block state Ps / Ms / Ss is indexed by absolute block; on return it holds column ncols - 1 for the blocks
+ * [bd.first(ncols - 1), bd.last(ncols - 1)].
+ *
+ * Wavefront: thread t works on column j0 + s - t at step s and passes its horizontal carry (and the bottom score of its
+ * last block, for a block entering below it) to thread t + 1 through a shuffle, or shared memory between warps.
+ * Ownership is fixed per tile of C = 16 * NT columns: the tile's blocks are the union of its columns' ranges
+ * [first(j0), last(j1 - 1)], and thread t owns a fixed contiguous slice of them, kept in registers for the tile. Owning
+ * blocks by their position relative to the band instead would break the wavefront's order: when the first block
+ * advances, block b at column j - 1 would belong to a thread that reaches column j - 1 after the thread that owns b at
+ * column j needs it. The pipeline drains between tiles (NT - 1 idle steps per tile), and the block state goes through
+ * global memory only there. A CTA of one warp synchronises with shuffles only. */
+__device__ void band_sweep(const uint64_t *peq, int nb, const uint8_t *t, int ncols, bool trev, const uint8_t *code,
+                           uint64_t *Ps, uint64_t *Ms, int *Ss, const Band &bd, int *xfer)
+{
+  const int tid = threadIdx.x, NT = blockDim.x, lane = tid & 31, warp = tid >> 5;
+  const bool multi = NT > 32;
+  for (int b = bd.first(0) + tid; b <= bd.last(0); b += NT) { Ps[b] = ~0ull; Ms[b] = 0; Ss[b] = 64 * (b + 1); }
+  __syncthreads();
+  const int C = 16 * NT;
+  for (int j0 = 0; j0 < ncols; j0 += C) {
+    const int j1 = min(ncols, j0 + C);
+    if (j0 > 0 && tid == 0 && bd.last(j0) > bd.last(j0 - 1)) {  // a block entering at the tile's first column
+      const int b = bd.last(j0);
+      Ps[b] = ~0ull; Ms[b] = 0; Ss[b] = Ss[b - 1] + 64;
+    }
+    __syncthreads();
+    const int u0 = bd.first(j0), u1 = bd.last(j1 - 1);
+    const int per = (u1 - u0 + NT) / NT;
+    const int s0 = u0 + tid * per, s1 = min(u1 + 1, s0 + per);  // this thread's slice [s0, s1), possibly empty
+    uint64_t rP[BAND_BPT], rM[BAND_BPT];
+    int rS[BAND_BPT];
+    {
+      const int f = bd.first(j0), l = bd.last(j0);
+#pragma unroll
+      for (int i = 0; i < BAND_BPT; i++) {
+        const int b = s0 + i;
+        const bool on = b < s1 && b >= f && b <= l;
+        rP[i] = on ? Ps[b] : 0; rM[i] = on ? Ms[b] : 0; rS[i] = on ? Ss[b] : 0;
+      }
+    }
+    int carry = 0, carry_sc = 0, above = 0;
+    const int steps = (j1 - j0) + NT - 1;
+    for (int s = 0; s < steps; s++) {
+      int hin = __shfl_up_sync(FULL, carry, 1), ain = __shfl_up_sync(FULL, carry_sc, 1);
+      if (multi && lane == 0 && warp > 0) {
+        const int *x = xfer + (((s + 1) & 1) * 32 + warp - 1) * 2;  // written by the warp above at step s - 1
+        hin = x[0]; ain = x[1];
+      }
+      const int j = j0 + s - tid;
+      if (j >= j0 && j < j1) {
+        const int f = bd.first(j), l = bd.last(j), lp = j > j0 ? bd.last(j - 1) : l;
+        const int b0 = max(s0, f), b1 = min(s1 - 1, l);
+        if (b0 <= b1) {
+          const uint64_t *pq = peq + (size_t)code[trev ? t[ncols - 1 - j] : t[j]] * nb;
+          int h = b0 == f ? 1 : hin;
+          // bottom score at column j - 1 of the block above the next one; in a narrow band that block may already have
+          // left the band at column j (b < b0) and still holds column j - 1
+          int prev = above;
+#pragma unroll
+          for (int i = 0; i < BAND_BPT; i++) {
+            const int b = s0 + i;
+            if (b >= b0 && b <= b1) {
+              if (b > lp) { rP[i] = ~0ull; rM[i] = 0; rS[i] = prev + 64; }  // enters the band at the bottom
+              prev = rS[i];
+              h = myers_block(rP[i], rM[i], rS[i], pq[b], h);
+              carry_sc = rS[i];
+            } else if (b < b0 && b < s1) {
+              prev = rS[i];
+            }
+          }
+          if (b0 - 1 >= s0 + BAND_BPT) prev = Ss[b0 - 1];
+          for (int b = max(b0, s0 + BAND_BPT); b <= b1; b++) {  // a slice wider than the registers: the rest in memory
+            uint64_t Pv = Ps[b], Mv = Ms[b];
+            int sc = Ss[b];
+            if (b > lp) { Pv = ~0ull; Mv = 0; sc = prev + 64; }
+            prev = sc;
+            h = myers_block(Pv, Mv, sc, pq[b], h);
+            Ps[b] = Pv; Ms[b] = Mv; Ss[b] = sc;
+            carry_sc = sc;
+          }
+          carry = h;
+        }
+        above = ain;  // bottom score of block s0 - 1 at column j, for a block s0 entering at column j + 1
+      }
+      if (multi) {
+        if (lane == 31) {
+          int *x = xfer + ((s & 1) * 32 + warp) * 2;
+          x[0] = carry; x[1] = carry_sc;
+        }
+        __syncthreads();
+      } else {
+        __syncwarp();
+      }
+    }
+    {
+      const int f = bd.first(j1 - 1), l = bd.last(j1 - 1);
+#pragma unroll
+      for (int i = 0; i < BAND_BPT; i++) {
+        const int b = s0 + i;
+        if (b < s1 && b >= f && b <= l) { Ps[b] = rP[i]; Ms[b] = rM[i]; Ss[b] = rS[i]; }
+      }
+    }
+    __syncthreads();
+  }
+}
+
+/* Rule 1' for a long job, one CTA per problem: the banded NW score at (Q-1, T-1) with the band of bound p.k. It is
+ * exact when it is <= p.k and an upper bound of the distance otherwise; the host accepts or widens (out[res]). */
+__global__ void k_band_nw(const Prob *probs, const uint8_t *dq, const uint8_t *dt, const uint8_t *code, int nsym,
+                          uint8_t *scratch, int *out)
+{
+  __shared__ int xfer[2 * 32 * 2];
+  const Prob p = probs[blockIdx.x];
+  const int nb = nblocks(p.ql);
+  Scratch sc(scratch + p.scratch, p.ql, nsym, 1);
+  build_peq_cta(sc.peq, dq + p.q, p.ql, false, code, nsym);
+  const Band bd(p.ql, p.tl, p.k);
+  band_sweep(sc.peq, nb, dt + p.t, p.tl, false, code, sc.P, sc.M, sc.S, bd, xfer);
+  if (threadIdx.x == 0) out[p.res] = block_row(sc.P[nb - 1], sc.M[nb - 1], sc.S[nb - 1], (p.ql - 1) & 63);
+}
+
+/* scratch of a long Hirschberg node: two sweep areas (forward, reverse), then left[Q] and right[Q] */
+__host__ __device__ inline uint64_t band_node_bytes(int ql, int nsym)
+{
+  return 2 * scratch_bytes(ql, nsym, 1, 0) + 2 * al16((uint64_t)ql * 4);
+}
+
+/* One half of a long Hirschberg node per CTA (blockIdx.x = 2 * node + half): the forward column of the left half or
+ * the reverse column of the right half, banded with k = the node's score in the node's own (Q, T). Rows outside the
+ * last column's band are BAND_INF. k_band_split takes the split row from the two columns. */
+__global__ void k_band_col(const Prob *probs, const uint8_t *dq, const uint8_t *dt, const uint8_t *code, int nsym,
+                           uint8_t *scratch)
+{
+  __shared__ int xfer[2 * 32 * 2];
+  const Prob p = probs[blockIdx.x >> 1];
+  const bool rev = blockIdx.x & 1;
+  const int Q = p.ql, nb = nblocks(Q), lw = p.tl / 2, rw = p.tl - lw;
+  if (lw == 0) return;  // no split (k_band_split)
+  uint8_t *base = scratch + p.scratch;
+  const uint64_t half = scratch_bytes(Q, nsym, 1, 0);
+  Scratch sc(base + (rev ? half : 0), Q, nsym, 1);
+  int *col = (int *)(base + 2 * half + (rev ? al16((uint64_t)Q * 4) : 0));
+  build_peq_cta(sc.peq, dq + p.q, Q, rev, code, nsym);
+  const Band bd(Q, p.tl, p.k);
+  const int ncols = rev ? rw : lw;
+  band_sweep(sc.peq, nb, dt + p.t + (rev ? lw : 0), ncols, rev, code, sc.P, sc.M, sc.S, bd, xfer);
+  const int f = bd.first(ncols - 1), l = bd.last(ncols - 1);
+  for (int r = threadIdx.x; r < Q; r += blockDim.x) {
+    const int b = r >> 6;
+    col[rev ? Q - 1 - r : r] = b >= f && b <= l ? block_row(sc.P[b], sc.M[b], sc.S[b], r & 63) : BAND_INF;
+  }
+}
+
+/* the split of each long node from k_band_col's columns, one warp per node (the ballot scan of k_align_hirsch) */
+__global__ void k_band_split(const Prob *probs, int n, int nsym, uint8_t *scratch, int4 *out)
+{
+  const int w = (int)((blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+  if (w >= n) return;
+  const Prob p = probs[w];
+  const int Q = p.ql, lw = p.tl / 2, rw = p.tl - lw;
+  if (lw == 0) {  // as k_align_hirsch: a one-column target above the 1 MiB threshold has no alignment
+    if (lane == 0) out[p.res] = make_int4(0, 0, 0, 0);
+    return;
+  }
+  const int *left = (const int *)(scratch + p.scratch + 2 * scratch_bytes(Q, nsym, 1, 0));
+  const int *right = (const int *)((const uint8_t *)left + al16((uint64_t)Q * 4));
+  const int4 r = split_row(left, right, Q, lw, rw, p.k, lane);
+  if (lane == 0) out[p.res] = r;
+}
+
 struct DevBuf {
   void *p = nullptr;
   size_t cap = 0;
@@ -333,7 +578,7 @@ struct mm_align_ctx {
   cudaEvent_t e0 = nullptr, e1 = nullptr;
   std::string err;
   float ms[8] = {0};
-  DevBuf q, t, code, probs, scratch, out_a, out_b, ops, out_n;
+  DevBuf q, t, code, probs, scratch, out_a, out_b, out_c, ops, out_n;
 };
 
 namespace {
@@ -387,6 +632,36 @@ void run_waves(mm_align_ctx *c, std::vector<Prob> &probs, Bytes bytes, Launch la
     ck(c, cudaGetLastError(), "kernel launch");
     ck(c, cudaStreamSynchronize(c->st), "kernel");
     i = j;
+  }
+}
+
+/* the routing rule of the header: a sub-problem's own size decides, so a job's result never depends on its batch */
+inline bool is_long(int ql, int tl) { return std::max(ql, tl) >= MM_ALIGN_BAND_MIN_LEN; }
+
+/* threads of the CTA that sweeps a band of bound k: about six blocks per thread, a multiple of 32, 32 to 512. A narrow
+ * band (the first passes of the distance schedule) runs as one warp, so it does not pay a CTA barrier per column. */
+inline int band_threads(int ql, int tl, int k)
+{
+  const Band bd(ql, tl, k);
+  const long long rows = std::min<long long>(ql, bd.dmax - bd.dmin + 1);
+  const long long nt = ((rows / 64 + 2) / 6 + 31) / 32 * 32;
+  return (int)std::min<long long>(512, std::max<long long>(32, nt));
+}
+
+/* Runs banded problems in launches of one CTA size each (and in waves under the budget); launch(dp, n, threads). */
+template <class Launch, class Bytes>
+void run_band(mm_align_ctx *c, const std::vector<Prob> &probs, Bytes bytes, Launch launch)
+{
+  std::vector<int> nt(probs.size());
+  for (size_t i = 0; i < probs.size(); i++) nt[i] = band_threads(probs[i].ql, probs[i].tl, probs[i].k);
+  std::vector<int> sizes(nt);
+  std::sort(sizes.begin(), sizes.end());
+  sizes.erase(std::unique(sizes.begin(), sizes.end()), sizes.end());
+  for (const int threads : sizes) {
+    std::vector<Prob> group;
+    for (size_t i = 0; i < probs.size(); i++)
+      if (nt[i] == threads) group.push_back(probs[i]);
+    run_waves(c, group, bytes, [&](const Prob *dp, int n, int, int) { launch(dp, n, threads); });
   }
 }
 
@@ -504,14 +779,25 @@ int mm_align_batch(mm_align_ctx *c, const char *qbases, uint64_t n_q, const char
     const uint8_t *dq = c->q.as<uint8_t>(), *dt = c->t.as<uint8_t>(), *dc = c->code.as<uint8_t>();
     auto sweep_bytes = [nsym](const Prob &p) { return scratch_bytes(p.ql, nsym, 1, 0); };
 
-    // (a) distance and end; HW and NW jobs in launches of their own
+    // (a) distance and end; HW and NW jobs in launches of their own, long NW jobs banded
     std::vector<int> ed(n_jobs), end(n_jobs), start(n_jobs, 0);
+    std::vector<std::pair<int, int>> band_ed;  // (job, distance) of the long NW jobs
     {
       StageTimer tm(c, 1);
-      std::vector<Prob> hw, nw;
-      for (uint64_t j = 0; j < n_jobs; j++)
-        (jobs[j].mode == MM_ALIGN_NW ? nw : hw)
-            .push_back(Prob{jobs[j].q_offset, jobs[j].t_offset, jobs[j].q_len, jobs[j].t_len, jobs[j].k, (int)j, 0, 0});
+      std::vector<Prob> hw, nw, band;
+      for (uint64_t j = 0; j < n_jobs; j++) {
+        const mm_align_job &b = jobs[j];
+        Prob p{b.q_offset, b.t_offset, b.q_len, b.t_len, b.k, (int)j, 0, 0};
+        if (b.mode == MM_ALIGN_NW && is_long(b.q_len, b.t_len)) {
+          // k schedule: the first bound leaves 32 diagonals of slack on each side of the length difference
+          const long long D = std::abs((long long)b.q_len - b.t_len);
+          const long long kmax = b.k < 0 ? std::max(b.q_len, b.t_len) : b.k;
+          if (D > kmax) band_ed.push_back({(int)j, -1});  // ed >= |Q - T|
+          else { p.k = (int)std::min(kmax, std::max(64LL, D + 64)); band.push_back(p); }
+          continue;
+        }
+        (b.mode == MM_ALIGN_NW ? nw : hw).push_back(p);
+      }
       ck(c, c->out_a.ensure(n_jobs * 4), "output allocation");
       ck(c, c->out_b.ensure(n_jobs * 4), "output allocation");
       if (!hw.empty())
@@ -524,8 +810,33 @@ int mm_align_batch(mm_align_ctx *c, const char *qbases, uint64_t n_q, const char
           k_align_nw<<<grid, blk, 0, c->st>>>(dp, n, dq, dt, dc, nsym, c->scratch.as<uint8_t>(), c->out_a.as<int>(),
                                               c->out_b.as<int>());
         });
+      // Banded passes until each long job is decided. A pass's score is exact when it is <= the pass's bound and is the
+      // cost of a real path (so >= the distance) otherwise: the next bound is that score or 4x the bound, whichever is
+      // smaller, capped at the job's k (k < 0: at max(Q, T), where the band holds every row). A pass at the job's k
+      // that stays above it decides -1, as edlib does.
+      std::vector<int> v(n_jobs);
+      while (!band.empty()) {
+        ck(c, c->out_c.ensure(n_jobs * 4), "output allocation");
+        run_band(c, band, sweep_bytes, [&](const Prob *dp, int n, int threads) {
+          k_band_nw<<<n, threads, 0, c->st>>>(dp, dq, dt, dc, nsym, c->scratch.as<uint8_t>(), c->out_c.as<int>());
+        });
+        ck(c, cudaMemcpy(v.data(), c->out_c.p, n_jobs * 4, cudaMemcpyDeviceToHost), "D2H");
+        std::vector<Prob> next;
+        for (Prob p : band) {
+          const mm_align_job &b = jobs[p.res];
+          const long long kmax = b.k < 0 ? std::max(b.q_len, b.t_len) : b.k, s = v[p.res];
+          if (s <= p.k) band_ed.push_back({p.res, (int)s});
+          else if (p.k >= kmax) band_ed.push_back({p.res, -1});
+          else { p.k = (int)std::min({kmax, s, 4LL * p.k}); next.push_back(p); }
+        }
+        band.swap(next);
+      }
       ck(c, cudaMemcpyAsync(ed.data(), c->out_a.p, n_jobs * 4, cudaMemcpyDeviceToHost, c->st), "D2H");
       ck(c, cudaMemcpyAsync(end.data(), c->out_b.p, n_jobs * 4, cudaMemcpyDeviceToHost, c->st), "D2H");
+    }
+    for (const auto &x : band_ed) {
+      ed[x.first] = x.second;
+      end[x.first] = x.second >= 0 ? jobs[x.first].t_len - 1 : -1;
     }
     // (b) start of the HW jobs; end = -1 (the whole query inserted before the target) has start 0, as every NW job has
     {
@@ -563,11 +874,21 @@ int mm_align_batch(mm_align_ctx *c, const char *qbases, uint64_t n_q, const char
         if (probs.empty()) break;
         levels++;
         ck(c, c->out_a.ensure(probs.size() * sizeof(int4)), "output allocation");
-        run_waves(c, probs, [nsym](const Prob &p) { return scratch_bytes(p.ql, nsym, 1, (uint64_t)p.ql * 8 + 16); },
-                  [&](const Prob *dp, int n, int grid, int blk) {
-                    k_align_hirsch<<<grid, blk, 0, c->st>>>(dp, n, dq, dt, dc, nsym, c->scratch.as<uint8_t>(),
-                                                            c->out_a.as<int4>());
-                  });
+        std::vector<Prob> shortp, longp;  // copies: probs keeps the node order for the merge below
+        for (const Prob &p : probs) (is_long(p.ql, p.tl) ? longp : shortp).push_back(p);
+        if (!shortp.empty())
+          run_waves(c, shortp, [nsym](const Prob &p) { return scratch_bytes(p.ql, nsym, 1, (uint64_t)p.ql * 8 + 16); },
+                    [&](const Prob *dp, int n, int grid, int blk) {
+                      k_align_hirsch<<<grid, blk, 0, c->st>>>(dp, n, dq, dt, dc, nsym, c->scratch.as<uint8_t>(),
+                                                              c->out_a.as<int4>());
+                    });
+        if (!longp.empty())  // both halves of a node as two CTAs, then the split
+          run_band(c, longp, [nsym](const Prob &p) { return band_node_bytes(p.ql, nsym); },
+                   [&](const Prob *dp, int n, int threads) {
+                     k_band_col<<<2 * n, threads, 0, c->st>>>(dp, dq, dt, dc, nsym, c->scratch.as<uint8_t>());
+                     k_band_split<<<(n + 3) / 4, 128, 0, c->st>>>(dp, n, nsym, c->scratch.as<uint8_t>(),
+                                                                  c->out_a.as<int4>());
+                   });
         std::vector<int4> sp(probs.size());
         ck(c, cudaMemcpy(sp.data(), c->out_a.p, sp.size() * sizeof(int4), cudaMemcpyDeviceToHost), "D2H");
         std::vector<Node> next;
