@@ -369,12 +369,14 @@ int launch_pack_if_ascii(mm_ctx *c)
 mm_dev_batch make_batch(mm_ctx *c);
 
 /* K1 over the resident batch: the sketch kernels over the caller's segments and the pieces of the long fragments, then
- * the merge of the pieces */
-int launch_sketch_all(mm_ctx *c)
+ * the merge of the pieces. probe: the kernels also look every hash of the caller's segments up in the index's table
+ * (sk_val, read by K2); the pieces' own hashes never are */
+int launch_sketch_all(mm_ctx *c, bool probe)
 {
   mm_dev_batch b = make_batch(c);
   if (c->n_long) b.segs = c->d_work_segs;
-  CU(c, mm_launch_sketch(c->params, b, c->stream, c->sm_count, c->sk_mode));
+  if (!probe) b.sk_val = nullptr;
+  CU(c, mm_launch_sketch(c->params, c->ix, b, c->stream, c->sm_count, c->sk_mode));
   c->launches += c->sk_mode ? 1 : 2;
   if (c->n_long) {
     /* the pieces: general kernel (it writes the vote sums the merge needs), then the merge */
@@ -382,10 +384,10 @@ int launch_sketch_all(mm_ctx *c)
     mm_dev_batch bp = b;
     bp.segs = c->d_work_segs + n0; bp.n_segs = (uint32_t)(c->n_work - n0);
     bp.sk_hash = c->d_sk_hash + n0 * S; bp.sk_pos = c->d_sk_pos + n0 * S; bp.sk_strand = c->d_sk_strand + n0 * S;
-    bp.sk_votes = c->d_sk_votes + n0 * S; bp.seg_res = c->d_seg_res + n0;
-    CU(c, mm_launch_sketch(c->params, bp, c->stream, c->sm_count, 1));
+    bp.sk_votes = c->d_sk_votes + n0 * S; bp.seg_res = c->d_seg_res + n0; bp.sk_val = nullptr;
+    CU(c, mm_launch_sketch(c->params, c->ix, bp, c->stream, c->sm_count, 1));
     b.sk_votes = c->d_sk_votes;
-    CU(c, mm_launch_sketch_long_merge(c->params, b, c->d_long, c->d_long_off, c->n_long, (uint32_t)n0, c->long_entries,
+    CU(c, mm_launch_sketch_long_merge(c->params, c->ix, b, c->d_long, c->d_long_off, c->n_long, (uint32_t)n0, c->long_entries,
                                       c->d_long_tmp, c->long_tmp_cap, c->stream));
     c->launches += 3; /* pieces, prep, merge (the segmented sort is a library call, not counted) */
   }
@@ -631,7 +633,7 @@ int run_pipeline(mm_ctx *c)
     CU(c, cudaEventRecord(c->ev[0], c->stream));
     if ((rc = launch_pack_if_ascii(c))) return rc;
     CU(c, cudaEventRecord(c->ev_pack, c->stream));
-    if ((rc = launch_sketch_all(c))) return rc;
+    if ((rc = launch_sketch_all(c, true))) return rc;
     CU(c, cudaEventRecord(c->ev[1], c->stream));
     int l1_launches = 0;
     CU(c, mm_launch_l1(c->params, c->ix, b, c->stream, c->sm_count, c->d_l1_slow, c->l1_warp, &l1_launches));
@@ -1068,7 +1070,7 @@ int mm_sketch_segments(mm_ctx *c, const char *bases, uint64_t n_bases, const mm_
   if ((rc = launch_pack_if_ascii(c))) return rc;
   ZERO_WORDS(c, c->d_counters, 16);
   CU(c, cudaEventRecord(c->ev[0], c->stream));
-  if ((rc = launch_sketch_all(c))) return rc;
+  if ((rc = launch_sketch_all(c, false))) return rc; /* sketches only: no index needed */
   CU(c, cudaEventRecord(c->ev[1], c->stream));
   CU(c, cudaStreamSynchronize(c->stream));
   cudaEventElapsedTime(&c->stage_ms[0], c->ev[0], c->ev[1]);

@@ -78,7 +78,8 @@ struct mm_dev_batch {
   uint32_t n_segs;
   /* query sketches, slot seg*S + j (ascending hash); compacted in place by the L1 kernel      */
   uint64_t *sk_hash;
-  uint64_t *sk_val;   /* lookup-table value of every sketch hash (written by k_l1_probe): 0 = absent */
+  uint64_t *sk_val;   /* lookup-table value of every sketch hash (written by the sketch kernels, mm_tab_lookup): */
+                      /* 0 = absent; nullptr = no index, the sketch kernels skip the probe                      */
   int2 *sk_pos;               /* (first position, last position)                                */
   int8_t *sk_strand;
   int32_t *sk_votes;          /* optional (nullptr = not written; general sketch kernel only): the vote SUM of every     */
@@ -127,8 +128,31 @@ MM_HD uint32_t mm_tab_slot_of(uint64_t key, int log2)
   return (uint32_t)(x >> (64 - log2));
 }
 
+#ifdef __CUDACC__
+/* the rest of a lookup whose first slot (key, val at `slot`) is already loaded: follow the linear-probe chain. Returns 0
+ * when h is absent, else offset<<25 | count<<1 | isFreqSeed */
+__device__ __forceinline__ uint64_t mm_tab_resolve(const mm_tab_slot *tab, int log2, uint64_t h, uint32_t slot, uint64_t key,
+                                                   uint64_t val)
+{
+  const uint32_t tmask = (1u << log2) - 1u;
+  while (val != MM_TAB_EMPTY_VAL && key != h) {
+    slot = (slot + 1) & tmask;
+    key = tab[slot].key;
+    val = tab[slot].val;
+  }
+  return val;
+}
+__device__ __forceinline__ uint64_t mm_tab_lookup(const mm_tab_slot *tab, int log2, uint64_t h)
+{
+  const uint32_t slot = mm_tab_slot_of(h, log2);
+  return mm_tab_resolve(tab, log2, h, slot, tab[slot].key, tab[slot].val);
+}
+#endif
+
 /* launchers implemented in the .cu files; all return cudaError_t from the launch */
-cudaError_t mm_launch_sketch(const mm_params &p, const mm_dev_batch &b, cudaStream_t st, int sm_count, int mode);
+/* K1; where b.sk_val is set, every sketch hash written is also looked up in ix's table (K2's first step) */
+cudaError_t mm_launch_sketch(const mm_params &p, const mm_dev_index &ix, const mm_dev_batch &b, cudaStream_t st, int sm_count,
+                             int mode);
 /* K1 for fragments longer than seg_length (mm_sketch.cu): the fragment was cut into pieces of at most seg_length bases
  * that overlap by kmer_size-1 (piece j starts at base j * (seg_length - kmer_size + 1)); the pieces were sketched by
  * mm_launch_sketch in mode 1 (general kernel) as segments [piece0, piece0 + n_pieces) of the same batch, with
@@ -140,7 +164,7 @@ struct mm_long_frag {
   uint32_t _pad;
 };
 size_t mm_sketch_long_tmp_bytes(uint64_t n_entries, uint32_t n_frags);
-cudaError_t mm_launch_sketch_long_merge(const mm_params &p, const mm_dev_batch &b, const mm_long_frag *frags,
+cudaError_t mm_launch_sketch_long_merge(const mm_params &p, const mm_dev_index &ix, const mm_dev_batch &b, const mm_long_frag *frags,
                                         const uint64_t *entry_off, uint32_t n_frags, uint32_t piece_base, uint64_t n_entries,
                                         void *tmp, size_t tmp_bytes, cudaStream_t st);
 /* K0: ASCII -> nibbles (makeUpperCaseAndValidDNA as a format change); both buffers padded to a multiple of 16 bases */

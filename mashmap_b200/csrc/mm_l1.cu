@@ -441,35 +441,7 @@ __device__ int l1_window_range(const mm_params &prm, const mm_dev_index &ix, con
   return best;
 }
 
-/* probe the lookup table for one hash: 0 = absent, else offset<<25 | count<<1 | isFreqSeed */
-__device__ __forceinline__ uint64_t l1_probe(const mm_dev_index &ix, uint64_t h)
-{
-  uint32_t slot = mm_tab_slot_of(h, ix.tab_log2);
-  const uint32_t tmask = (1u << ix.tab_log2) - 1u;
-  while (true) {
-    /* (128 B of DRAM traffic per probe, ncu; neither cudaLimitMaxL2FetchGranularity = 32 nor ld.global.L2::64B / ::128B changes
-     * the kernel's time) */
-    const mm_tab_slot t = ix.tab[slot];
-    if (t.val == MM_TAB_EMPTY_VAL) return 0;
-    if (t.key == h) return t.val;
-    slot = (slot + 1) & tmask;
-  }
-}
-
-/* K2a: one thread per sketch entry -- the random table probes of the whole batch with full memory-level parallelism
- * (the per-segment kernels below are latency-bound when they probe themselves: 7 dependent DRAM round trips per lane). */
-__global__ void __launch_bounds__(256) k_l1_probe(const mm_dev_index ix, const mm_dev_batch b, int S)
-{
-  const uint64_t total = (uint64_t)b.n_segs * (uint64_t)S;
-  for (uint64_t e = (uint64_t)blockIdx.x * 256ULL + threadIdx.x; e < total; e += (uint64_t)gridDim.x * 256ULL) {
-    const uint32_t seg = (uint32_t)(e / (uint32_t)S);
-    const int j = (int)(e - (uint64_t)seg * (uint32_t)S);
-    if (j >= b.seg_res[seg].sketch_raw_count) continue;
-    b.sk_val[e] = l1_probe(ix, b.sk_hash[e]);
-  }
-}
-
-/* One segment, processed by a group of NT threads (the table values of its hashes are in b.sk_val).
+/* One segment, processed by a group of NT threads (the table values of its hashes are in b.sk_val, written by K1).
  * Returns false (NT == 32 only) if the segment has more points than the warp path holds: nothing was modified.
  * WIN: the segment is a fragment longer than seg_length (windowLen > 0, k_l1_long); without WIN such a fragment is
  * skipped (returns true, writes nothing). */
@@ -806,17 +778,10 @@ cudaError_t mm_launch_l1(const mm_params &p, const mm_dev_index &ix, const mm_de
   if (b.n_segs == 0) return cudaSuccess;
   uint32_t grid = mm_l1_grid_size(p, sm_count);
   if (grid == 0) return cudaErrorInvalidValue;
-  {
-    const uint64_t total = (uint64_t)b.n_segs * (uint64_t)p.sketch_size;
-    const uint64_t blocks = (total + 255) / 256;
-    k_l1_probe<<<(uint32_t)std::min<uint64_t>(blocks, 1u << 30), 256, 0, st>>>(ix, b, p.sketch_size);
-    cudaError_t e0 = cudaGetLastError();
-    if (e0 != cudaSuccess) return e0;
-  }
   const size_t wsmem = l1_warp_smem(p.sketch_size) * L1_WARPS_PER_CTA;
   if (!use_warp_path || !slow_list || wsmem > 227 * 1024) {
     k_l1_cta<<<min(grid, b.n_segs), 128, l1_cta_smem(p), st>>>(p, ix, b, nullptr);
-    if (n_launched) *n_launched = 2;
+    if (n_launched) *n_launched = 1;
     return cudaGetLastError();
   }
   cudaError_t e = cudaFuncSetAttribute(k_l1_warp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsmem);
@@ -831,11 +796,12 @@ cudaError_t mm_launch_l1(const mm_params &p, const mm_dev_index &ix, const mm_de
   if (e != cudaSuccess) return e;
   /* the general path reads its work count from counters[8] on the device: no host round trip in between */
   k_l1_cta<<<grid, 128, l1_cta_smem(p), st>>>(p, ix, b, slow_list);
-  if (n_launched) *n_launched = 3;
+  if (n_launched) *n_launched = 2;
   return cudaGetLastError();
 }
 
-/* K2 of the fragments longer than seg_length (after mm_launch_l1, whose kernels skip them and whose probe covered them) */
+/* K2 of the fragments longer than seg_length (after mm_launch_l1, whose kernels skip them; the merge of their pieces in
+ * K1 looked their hashes up) */
 cudaError_t mm_launch_l1_long(const mm_params &p, const mm_dev_index &ix, const mm_dev_batch &b, const mm_long_frag *longs,
                               uint32_t n_long, cudaStream_t st, int sm_count)
 {

@@ -28,7 +28,8 @@
  *     distinct hashes survived although larger ones exist, or the table overflowed, T is raised / lowered / bisected and
  *     the pass is redone (rare; always terminates because distinct-count(T) grows by at most one per unit of T). The
  *     <= C survivors are ordered with a 256-bucket counting sort on the leading bits plus in-bucket ranking, and the
- *     first s are written out.
+ *     first s are written out. Where the batch has an index (sk_val set), every hash written is also looked up in the
+ *     index's table (K2's first step, whose DRAM latency here overlaps the other CTAs' hashing).
  *   A thread whose stretch of the segment contains an N (nibble bit 3) takes the same loop with the run-length test
  *   of commonFunc.hpp:207-223 compiled in; all others skip it.
  */
@@ -415,6 +416,34 @@ __device__ __forceinline__ bool sk_any_n(const uint32_t *nib, uint32_t b0, uint3
   return (acc & 0x88888888u) != 0;
 }
 
+/* sk_val[r] = the lookup-table value of hs[r] for r < count (K2's probe, done here so that its DRAM latency overlaps the
+ * other CTAs' hashing). The first slot of every hash is loaded before any is resolved: one round trip per segment for
+ * count <= SK_PROBE_BATCH * SK_THREADS. Linear-probe continuations are followed one by one (rare). */
+constexpr int SK_PROBE_BATCH = 2;
+__device__ __forceinline__ void sk_probe(const mm_tab_slot *__restrict__ tab, int tab_log2, const uint64_t *hs,
+                                         uint64_t *__restrict__ sk_val, int count, int tid)
+{
+  for (int r0 = 0; r0 < count; r0 += SK_PROBE_BATCH * SK_THREADS) {
+    uint64_t h[SK_PROBE_BATCH], key[SK_PROBE_BATCH], val[SK_PROBE_BATCH];
+    uint32_t slot[SK_PROBE_BATCH];
+#pragma unroll
+    for (int u = 0; u < SK_PROBE_BATCH; u++) {
+      const int r = r0 + u * SK_THREADS + tid;
+      if (r < count) {
+        h[u] = hs[r];
+        slot[u] = mm_tab_slot_of(h[u], tab_log2);
+        key[u] = tab[slot[u]].key;
+        val[u] = tab[slot[u]].val;
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < SK_PROBE_BATCH; u++) {
+      const int r = r0 + u * SK_THREADS + tid;
+      if (r < count) sk_val[r] = mm_tab_resolve(tab, tab_log2, h[u], slot[u], key[u], val[u]);
+    }
+  }
+}
+
 /* The general kernel: handles every input (any number of repeated k-mers, fewer than s distinct k-mers, thresholds that
  * have to be re-estimated). work_list == nullptr: all n_segs segments; else the segments listed there, *work_count of them
  * (the fast kernel's rejects; the count is read on the device, no host round trip). */
@@ -423,7 +452,8 @@ __global__ void __launch_bounds__(SK_THREADS)
 k_sketch_table(const uint8_t *__restrict__ packed, const mm_segment *__restrict__ segs, uint32_t n_segs_all,
                const uint32_t *__restrict__ work_list, const uint32_t *__restrict__ work_count, int S,
                int seg_length, int C, int CAP, uint64_t *__restrict__ sk_hash, int2 *__restrict__ sk_pos,
-               int8_t *__restrict__ sk_strand, int32_t *__restrict__ sk_votes, mm_segment_result *__restrict__ seg_res)
+               int8_t *__restrict__ sk_strand, int32_t *__restrict__ sk_votes, mm_segment_result *__restrict__ seg_res,
+               const mm_tab_slot *__restrict__ tab, int tab_log2, uint64_t *__restrict__ sk_val)
 {
   extern __shared__ __align__(16) unsigned char smem[];
   const uint32_t n_segs = work_list ? *work_count : n_segs_all;
@@ -624,6 +654,11 @@ k_sketch_table(const uint8_t *__restrict__ packed, const mm_segment *__restrict_
       res.first_candidate = 0; res.n_candidates = 0; res._pad = 0;
       seg_res[seg] = res;
     }
+    if (sk_val) { /* the hashes just written, read back by the whole CTA */
+      const int count = min(dt + ctrl->has_max, S);
+      __syncthreads();
+      sk_probe(tab, tab_log2, sk_hash + obase, sk_val + obase, count, tid);
+    }
     __syncthreads(); /* all reads of the staging buffer and of the table are done */
   }
 }
@@ -635,9 +670,11 @@ k_sketch_table(const uint8_t *__restrict__ packed, const mm_segment *__restrict_
  *   compaction: every thread filters its own candidates exactly (valid k-mer, canonical hash <= T) and writes them to a
  *     dense array at an offset from a CTA-wide prefix sum;
  *   256-bucket counting sort on the leading bits of the hash (bucket sizes ~1.3);
- *   inside its bucket every candidate finds out whether it is the first occurrence of its hash and, if so, gathers
- *     first position / last position / vote sum of the occurrences and its rank among the bucket's distinct hashes;
- *   a prefix sum over the buckets' distinct counts turns that into the global rank; ranks < s are written out.
+ *   every thread takes whole buckets: it sorts the bucket by hash (insertion sort of its order[] entries) and counts the
+ *     distinct hashes;
+ *   a prefix sum over the buckets' distinct counts gives each bucket's first rank; the bucket's owner walks the sorted
+ *     bucket again, merges each run of equal hashes into first position / last position / vote sum, writes ranks < s and
+ *     looks each written hash up in the index's lookup table (K2's probe).
  * Anything unusual -- more candidates than the dense array holds, a bucket with more than SKF_BUCKET_MAX entries (heavily
  * repeated k-mers), fewer than s distinct hashes below T -- sends the segment to the general kernel through a device
  * work list. On random or genomic sequence that is a fraction of a per cent of the segments.
@@ -646,8 +683,8 @@ constexpr int SKF_SPILL = 64;       /* CTA-wide list for candidates that did not
 constexpr int SKF_BUCKET_MAX = 24;
 
 struct skf_layout {
-  uint32_t stage_bytes, off_bar, off_ctrl, off_list_h, off_list_p, off_spill_h, off_spill_p, off_cand_h, off_cand_m, off_order,
-      off_bcnt, off_bstart, off_bfill, off_dcnt, off_dstart, off_flag, total;
+  uint32_t stage_bytes, off_bar, off_ctrl, off_list_h, off_spill_h, off_spill_p, off_cand_h, off_cand_m, off_order,
+      off_list_p, off_bcnt, total;
 };
 struct skf_ctrl {
   int n_spill, n_cand, reject, warp_tot[SK_THREADS / 32];
@@ -663,19 +700,14 @@ __host__ __device__ inline skf_layout skf_make_layout(int seg_length, int NC, in
   L.off_spill_p = o; o += 4u * SKF_SPILL;
   L.off_cand_h = o; o += 8u * NC;   /* canonical hash */
   L.off_cand_m = o; o += 4u * NC;   /* position << 1 | (forward hash was the smaller one) */
-  /* the per-thread lists are dead after the compaction: order[], the bucket counters and the first-occurrence flags
-   * live in the same bytes */
+  /* the per-thread lists are dead after the compaction: order[] and five bucket counter arrays (bcnt, bstart, bfill, dcnt,
+   * dstart: SK_BUCKETS u32 each, addressed by constant offsets from bcnt) live in the same bytes */
   const uint32_t lists = (16u + 4u) * SK_THREADS * (uint32_t)CAP;
-  const uint32_t sorting = ((2u * NC + 15) & ~15u) + 5u * 4u * SK_BUCKETS + (((uint32_t)NC + 15) & ~15u);
+  const uint32_t sorting = ((2u * NC + 15) & ~15u) + 5u * 4u * SK_BUCKETS;
   L.off_list_h = o;
   L.off_list_p = o + 16u * SK_THREADS * (uint32_t)CAP;
   L.off_order = o;
   L.off_bcnt = o + ((2u * NC + 15) & ~15u);
-  L.off_bstart = L.off_bcnt + 4u * SK_BUCKETS;
-  L.off_bfill = L.off_bstart + 4u * SK_BUCKETS;
-  L.off_dcnt = L.off_bfill + 4u * SK_BUCKETS;
-  L.off_dstart = L.off_dcnt + 4u * SK_BUCKETS;
-  L.off_flag = L.off_dstart + 4u * SK_BUCKETS;
   o += lists > sorting ? lists : sorting;
   L.total = (o + 15) & ~15u;
   return L;
@@ -705,7 +737,8 @@ template <int K>
 __global__ void __launch_bounds__(SK_THREADS, MM_SK_MINB)
 k_sketch(const uint8_t *__restrict__ packed, const mm_segment *__restrict__ segs, uint32_t n_segs, int S, int seg_length,
          int NC, int CAP, uint64_t *__restrict__ sk_hash, int2 *__restrict__ sk_pos, int8_t *__restrict__ sk_strand,
-         mm_segment_result *__restrict__ seg_res, uint32_t *__restrict__ reject_list, uint32_t *__restrict__ reject_count)
+         mm_segment_result *__restrict__ seg_res, uint32_t *__restrict__ reject_list, uint32_t *__restrict__ reject_count,
+         const mm_tab_slot *__restrict__ tab, int tab_log2, uint64_t *__restrict__ sk_val)
 {
   extern __shared__ __align__(16) unsigned char smem[];
   const skf_layout L = skf_make_layout(seg_length, NC, CAP);
@@ -718,11 +751,8 @@ k_sketch(const uint8_t *__restrict__ packed, const mm_segment *__restrict__ segs
   uint32_t *cand_m = (uint32_t *)(smem + L.off_cand_m);
   uint16_t *order = (uint16_t *)(smem + L.off_order);
   uint32_t *bcnt = (uint32_t *)(smem + L.off_bcnt);
-  uint32_t *bstart = (uint32_t *)(smem + L.off_bstart);
-  uint32_t *bfill = (uint32_t *)(smem + L.off_bfill);
-  uint32_t *dcnt = (uint32_t *)(smem + L.off_dcnt);
-  uint32_t *dstart = (uint32_t *)(smem + L.off_dstart);
-  uint8_t *flag = (uint8_t *)(smem + L.off_flag);
+  uint32_t *bstart = bcnt + SK_BUCKETS, *bfill = bcnt + 2 * SK_BUCKETS, *dcnt = bcnt + 3 * SK_BUCKETS,
+           *dstart = bcnt + 4 * SK_BUCKETS;
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   uint4 *list_h = (uint4 *)(smem + L.off_list_h) + tid;
   uint32_t *list_p = (uint32_t *)(smem + L.off_list_p) + tid;
@@ -823,7 +853,7 @@ k_sketch(const uint8_t *__restrict__ packed, const mm_segment *__restrict__ segs
         }
       }
     }
-    __syncthreads(); /* lists consumed: their bytes become order[] / counters / flags */
+    __syncthreads(); /* lists consumed: their bytes become order[] / counters */
     bool reject = spill_over || total + n_spill > NC;
     int nc = total;
     if (!reject) {
@@ -841,7 +871,7 @@ k_sketch(const uint8_t *__restrict__ packed, const mm_segment *__restrict__ segs
           ctrl->n_cand = at;
         }
       }
-      for (int i = tid; i < SK_BUCKETS; i += SK_THREADS) { bcnt[i] = 0; bfill[i] = 0; dcnt[i] = 0; }
+      for (int i = tid; i < SK_BUCKETS; i += SK_THREADS) { bcnt[i] = 0; bfill[i] = 0; }
       __syncthreads();
       if (n_spill) nc = ctrl->n_cand;
       const int sh = max(0, (64 - __clzll((long long)T)) - 8);
@@ -854,56 +884,79 @@ k_sketch(const uint8_t *__restrict__ packed, const mm_segment *__restrict__ segs
         order[bstart[b] + atomicAdd(&bfill[b], 1u)] = (uint16_t)i;
       }
       __syncthreads();
-      /* first occurrence of its hash? (among equal hashes: the smallest position) */
+      /* one thread per bucket: order it by hash, count its distinct hashes */
       bool big_bucket = false;
-      for (int i = tid; i < nc; i += SK_THREADS) {
-        const uint64_t h = cand_h[i];
-        const uint32_t b = (uint32_t)(h >> sh);
-        const uint32_t bs = bstart[b], bn = bcnt[b];
-        if (bn > (uint32_t)SKF_BUCKET_MAX) { big_bucket = true; continue; }
-        const uint32_t pos = cand_m[i] >> 1;
-        bool is_first = true;
-        for (uint32_t q = bs; q < bs + bn; q++) {
-          const uint32_t j = order[q];
-          if (cand_h[j] == h && (cand_m[j] >> 1) < pos) is_first = false;
+      for (int b = tid; b < SK_BUCKETS; b += SK_THREADS) {
+        const uint32_t bs = bstart[b], be = bs + bcnt[b];
+        uint32_t nd = be - bs;
+        if (nd > (uint32_t)SKF_BUCKET_MAX) {
+          big_bucket = true;
+        } else if (nd > 1) {
+          for (uint32_t q = bs + 1; q < be; q++) {
+            const uint16_t j = order[q];
+            const uint64_t h = cand_h[j];
+            uint32_t p = q;
+            for (; p > bs && cand_h[order[p - 1]] > h; p--) order[p] = order[p - 1];
+            order[p] = j;
+          }
+          uint64_t prev = cand_h[order[bs]];
+          nd = 1;
+          for (uint32_t q = bs + 1; q < be; q++) {
+            const uint64_t h = cand_h[order[q]];
+            nd += h != prev ? 1u : 0u;
+            prev = h;
+          }
         }
-        flag[i] = is_first ? 1 : 0;
-        if (is_first) atomicAdd(&dcnt[b], 1u);
+        dcnt[b] = nd;
       }
       if (big_bucket) ctrl->reject = 1;
       __syncthreads();
       skf_bucket_prefix(dcnt, dstart, tid);
       __syncthreads();
-      int distinct = (int)(dstart[SK_BUCKETS - 1] + dcnt[SK_BUCKETS - 1]);
+      const int distinct = (int)(dstart[SK_BUCKETS - 1] + dcnt[SK_BUCKETS - 1]);
       reject = ctrl->reject != 0 || (distinct < S && T != SK_EMPTY);
       if (!reject) {
         const size_t obase = (size_t)seg * (size_t)S;
-        for (int i = tid; i < nc; i += SK_THREADS) {
-          if (!flag[i]) continue;
-          const uint64_t h = cand_h[i];
-          const uint32_t b = (uint32_t)(h >> sh);
-          const uint32_t bs = bstart[b], bn = bcnt[b];
-          uint32_t rank = dstart[b];
-          int first = 0x7fffffff, last = -1, votes = 0;
-          for (uint32_t q = bs; q < bs + bn; q++) {
-            const uint32_t j = order[q];
-            const uint64_t hj = cand_h[j];
-            if (hj == h) {
+        /* each bucket's owner merges the runs of equal hashes (first / last position, vote sum), writes ranks < s and
+         * looks each written hash up in the table: the loads of its first two ranks are issued in the walk and resolved
+         * after it, any further one at once (a separate probe phase behind one more barrier makes ptxas spill the hashing
+         * loop's state) */
+        int pr0 = -1, pr1 = -1;
+        uint32_t ps0 = 0, ps1 = 0;
+        uint64_t ph0 = 0, ph1 = 0, pk0 = 0, pk1 = 0, pv0 = 0, pv1 = 0;
+        for (int b = tid; b < SK_BUCKETS; b += SK_THREADS) {
+          const uint32_t bs = bstart[b], be = bs + bcnt[b];
+          int rank = (int)dstart[b];
+          uint32_t q = bs;
+          while (q < be && rank < S) {
+            const uint64_t h = cand_h[order[q]];
+            int first = 0x7fffffff, last = -1, votes = 0;
+            for (; q < be; q++) {
+              const uint16_t j = order[q];
+              if (cand_h[j] != h) break;
               const uint32_t m = cand_m[j];
               const int pj = (int)(m >> 1);
               first = min(first, pj); last = max(last, pj); votes += (m & 1u) ? 1 : -1;
-            } else if (hj < h && flag[j]) {
-              rank++;
             }
-          }
-          if ((int)rank < S) {
             sk_hash[obase + rank] = h;
             sk_pos[obase + rank] = make_int2(first, last);
             sk_strand[obase + rank] = (int8_t)(votes > 0 ? 1 : (votes == 0 ? 0 : -1)); /* commonFunc.hpp:282 */
+            if (sk_val) {
+              if (pr0 < 0) {
+                pr0 = rank; ph0 = h; ps0 = mm_tab_slot_of(h, tab_log2); pk0 = tab[ps0].key; pv0 = tab[ps0].val;
+              } else if (pr1 < 0) {
+                pr1 = rank; ph1 = h; ps1 = mm_tab_slot_of(h, tab_log2); pk1 = tab[ps1].key; pv1 = tab[ps1].val;
+              } else {
+                sk_val[obase + rank] = mm_tab_lookup(tab, tab_log2, h);
+              }
+            }
+            rank++;
           }
         }
+        if (pr0 >= 0) sk_val[obase + pr0] = mm_tab_resolve(tab, tab_log2, ph0, ps0, pk0, pv0);
+        if (pr1 >= 0) sk_val[obase + pr1] = mm_tab_resolve(tab, tab_log2, ph1, ps1, pk1, pv1);
+        const int count = min(distinct, S);
         if (tid == 0) {
-          const int count = min(distinct, S);
           mm_segment_result res;
           res.sketch_max_hash = 0; /* filled by the L1 kernel from sk_hash[count-1] */
           res.sketch_raw_count = count;
@@ -954,8 +1007,8 @@ int skf_cand_cap(int seg_length, int sketch_size, int kmer_size)
 }
 
 template <int K>
-cudaError_t launch_k(const mm_params &p, const mm_dev_batch &b, cudaStream_t st, int sm_count, int C, int CAP, size_t smem,
-                     int mode)
+cudaError_t launch_k(const mm_params &p, const mm_dev_index &ix, const mm_dev_batch &b, cudaStream_t st, int sm_count, int C,
+                     int CAP, size_t smem, int mode)
 {
   /* general kernel: over everything (mode 1, MM_SKETCH_TABLE=1) or over the fast kernel's rejects (mode 0) */
   cudaError_t e = cudaFuncSetAttribute(k_sketch_table<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -971,7 +1024,8 @@ cudaError_t launch_k(const mm_params &p, const mm_dev_batch &b, cudaStream_t st,
   if (mode == 1 || NC > 65535 || FL.total > 227u * 1024u) {
     const uint32_t grid = full > b.n_segs ? b.n_segs : full;
     k_sketch_table<K><<<grid, SK_THREADS, smem, st>>>(b.packed, b.segs, b.n_segs, nullptr, nullptr, p.sketch_size, p.seg_length, C,
-                                                      CAP, b.sk_hash, b.sk_pos, b.sk_strand, b.sk_votes, b.seg_res);
+                                                      CAP, b.sk_hash, b.sk_pos, b.sk_strand, b.sk_votes, b.seg_res, ix.tab,
+                                                      ix.tab_log2, b.sk_val);
     return cudaGetLastError();
   }
   e = cudaFuncSetAttribute(k_sketch<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FL.total);
@@ -983,14 +1037,16 @@ cudaError_t launch_k(const mm_params &p, const mm_dev_batch &b, cudaStream_t st,
   uint32_t fgrid = (uint32_t)sm_count * (uint32_t)focc; /* persistent: a whole number of CTAs per SM */
   if (fgrid > b.n_segs) fgrid = b.n_segs;
   k_sketch<K><<<fgrid, SK_THREADS, FL.total, st>>>(b.packed, b.segs, b.n_segs, p.sketch_size, p.seg_length, NC, CAP, b.sk_hash, b.sk_pos,
-                                                   b.sk_strand, b.seg_res, b.sk_reject, b.counters + 9);
+                                                   b.sk_strand, b.seg_res, b.sk_reject, b.counters + 9, ix.tab, ix.tab_log2,
+                                                   b.sk_val);
   e = cudaGetLastError();
   if (e != cudaSuccess) return e;
   /* the rejects: the count is read on the device; a grid of one CTA per SM is enough for a fraction of a per cent */
   uint32_t rgrid = (uint32_t)sm_count;
   if (rgrid > b.n_segs) rgrid = b.n_segs;
   k_sketch_table<K><<<rgrid, SK_THREADS, smem, st>>>(b.packed, b.segs, b.n_segs, b.sk_reject, b.counters + 9, p.sketch_size, p.seg_length,
-                                                     C, CAP, b.sk_hash, b.sk_pos, b.sk_strand, b.sk_votes, b.seg_res);
+                                                     C, CAP, b.sk_hash, b.sk_pos, b.sk_strand, b.sk_votes, b.seg_res, ix.tab,
+                                                     ix.tab_log2, b.sk_val);
   return cudaGetLastError();
 }
 
@@ -1033,7 +1089,8 @@ __global__ void __launch_bounds__(128) k_long_merge(const mm_long_frag *__restri
                                                     const uint32_t *__restrict__ vals, uint32_t piece_base, int S,
                                                     int piece_step, const int32_t *__restrict__ pk_votes,
                                                     uint64_t *__restrict__ sk_hash, int2 *sk_pos, int8_t *__restrict__ sk_strand,
-                                                    mm_segment_result *seg_res)
+                                                    mm_segment_result *seg_res, const mm_tab_slot *__restrict__ tab, int tab_log2,
+                                                    uint64_t *__restrict__ sk_val)
 {
   const uint32_t f = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
@@ -1073,6 +1130,7 @@ __global__ void __launch_bounds__(128) k_long_merge(const mm_long_frag *__restri
       sk_hash[obase + r] = h;
       sk_pos[obase + r] = make_int2(first, last);
       sk_strand[obase + r] = (int8_t)(votes > 0 ? 1 : (votes == 0 ? 0 : -1)); /* commonFunc.hpp:282 */
+      if (sk_val) sk_val[obase + r] = mm_tab_lookup(tab, tab_log2, h);
     }
     rank += __popc(heads);
   }
@@ -1100,7 +1158,7 @@ size_t mm_sketch_long_tmp_bytes(uint64_t n_entries, uint32_t n_frags)
   return n_entries * 16 + 256 * 3 + sort_bytes;
 }
 
-cudaError_t mm_launch_sketch_long_merge(const mm_params &p, const mm_dev_batch &b, const mm_long_frag *frags,
+cudaError_t mm_launch_sketch_long_merge(const mm_params &p, const mm_dev_index &ix, const mm_dev_batch &b, const mm_long_frag *frags,
                                         const uint64_t *entry_off, uint32_t n_frags, uint32_t piece_base, uint64_t n_entries,
                                         void *tmp, size_t tmp_bytes, cudaStream_t st)
 {
@@ -1121,7 +1179,7 @@ cudaError_t mm_launch_sketch_long_merge(const mm_params &p, const mm_dev_batch &
   if (e != cudaSuccess) return e;
   k_long_merge<<<(n_frags + 3) / 4, 128, 0, st>>>(frags, n_frags, entry_off, keys_out, vals_out, piece_base, S,
                                                   p.seg_length - p.kmer_size + 1, b.sk_votes, b.sk_hash, b.sk_pos, b.sk_strand,
-                                                  b.seg_res);
+                                                  b.seg_res, ix.tab, ix.tab_log2, b.sk_val);
   return cudaGetLastError();
 }
 
@@ -1169,13 +1227,14 @@ cudaError_t mm_launch_pack_bases(const uint8_t *ascii, uint8_t *packed, uint64_t
 
 /* mode 0: fast kernel + general kernel over its rejects (2 launches); mode 1: general kernel over everything (1 launch).
  * b.counters[9] must be 0 and b.sk_reject must hold n_segs entries. */
-cudaError_t mm_launch_sketch(const mm_params &p, const mm_dev_batch &b, cudaStream_t st, int sm_count, int mode)
+cudaError_t mm_launch_sketch(const mm_params &p, const mm_dev_index &ix, const mm_dev_batch &b, cudaStream_t st, int sm_count,
+                             int mode)
 {
   int C = 0, CAP = 0;
   const size_t smem = mm_sketch_smem_bytes(p.seg_length, p.sketch_size, p.kmer_size, &C, &CAP);
   if (smem == 0) return cudaErrorInvalidValue;
   switch (p.kmer_size) {
-#define X(KK) case KK: return launch_k<KK>(p, b, st, sm_count, C, CAP, smem, mode);
+#define X(KK) case KK: return launch_k<KK>(p, ix, b, st, sm_count, C, CAP, smem, mode);
     MM_FOR_EACH_K(X)
 #undef X
     default: return cudaErrorInvalidValue;
