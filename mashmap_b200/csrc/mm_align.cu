@@ -44,6 +44,7 @@
 #include <vector>
 
 #include "../../include/mashmap_b200_align.h"
+#include "mm_devbuf.h"
 
 namespace {
 
@@ -551,22 +552,6 @@ __global__ void k_band_split(const Prob *probs, int n, int nsym, uint8_t *scratc
   if (lane == 0) out[p.res] = r;
 }
 
-struct DevBuf {
-  void *p = nullptr;
-  size_t cap = 0;
-  cudaError_t ensure(size_t n)
-  {
-    if (n <= cap) return cudaSuccess;
-    if (p) cudaFree(p);
-    p = nullptr; cap = 0;
-    cudaError_t e = cudaMalloc(&p, std::max<size_t>(n, 256));
-    if (e == cudaSuccess) cap = std::max<size_t>(n, 256);
-    return e;
-  }
-  template <class T> T *as() const { return (T *)p; }
-  ~DevBuf() { if (p) cudaFree(p); }
-};
-
 thread_local std::string g_create_error;
 
 }  // namespace
@@ -578,7 +563,9 @@ struct mm_align_ctx {
   cudaEvent_t e0 = nullptr, e1 = nullptr;
   std::string err;
   float ms[8] = {0};
-  DevBuf q, t, code, probs, scratch, out_a, out_b, out_c, ops, out_n;
+  mm_devbuf<uint8_t> q, t, code, scratch, ops;
+  mm_devbuf<Prob> probs;
+  mm_devbuf<unsigned char> out_a, out_b, out_c, out_n; /* int or int4 results, by stage */
 };
 
 namespace {
@@ -624,11 +611,11 @@ void run_waves(mm_align_ctx *c, std::vector<Prob> &probs, Bytes bytes, Launch la
       used += b;
       j++;
     }
-    ck(c, c->scratch.ensure(used), "scratch allocation");
-    ck(c, c->probs.ensure((j - i) * sizeof(Prob)), "problem table allocation");
-    ck(c, cudaMemcpyAsync(c->probs.p, probs.data() + i, (j - i) * sizeof(Prob), cudaMemcpyHostToDevice, c->st), "H2D");
+    ck(c, c->scratch.reserve(used), "scratch allocation");
+    ck(c, c->probs.reserve(j - i), "problem table allocation");
+    ck(c, cudaMemcpyAsync(c->probs.get(), probs.data() + i, (j - i) * sizeof(Prob), cudaMemcpyHostToDevice, c->st), "H2D");
     const int n = (int)(j - i);
-    launch(c->probs.as<Prob>(), n, (n + 3) / 4, 128);
+    launch(c->probs.get(), n, (n + 3) / 4, 128);
     ck(c, cudaGetLastError(), "kernel launch");
     ck(c, cudaStreamSynchronize(c->st), "kernel");
     i = j;
@@ -769,14 +756,14 @@ int mm_align_batch(mm_align_ctx *c, const char *qbases, uint64_t n_q, const char
     ck(c, cudaSetDevice(c->device), "cudaSetDevice");
     {
       StageTimer tm(c, 0);
-      ck(c, c->q.ensure(n_q), "query allocation");
-      ck(c, c->t.ensure(n_t), "target allocation");
-      ck(c, c->code.ensure(256), "table allocation");
-      ck(c, cudaMemcpyAsync(c->q.p, qbases, n_q, cudaMemcpyHostToDevice, c->st), "H2D");
-      ck(c, cudaMemcpyAsync(c->t.p, tbases, n_t, cudaMemcpyHostToDevice, c->st), "H2D");
-      ck(c, cudaMemcpyAsync(c->code.p, code, 256, cudaMemcpyHostToDevice, c->st), "H2D");
+      ck(c, c->q.reserve(n_q), "query allocation");
+      ck(c, c->t.reserve(n_t), "target allocation");
+      ck(c, c->code.reserve(256), "table allocation");
+      ck(c, cudaMemcpyAsync(c->q.get(), qbases, n_q, cudaMemcpyHostToDevice, c->st), "H2D");
+      ck(c, cudaMemcpyAsync(c->t.get(), tbases, n_t, cudaMemcpyHostToDevice, c->st), "H2D");
+      ck(c, cudaMemcpyAsync(c->code.get(), code, 256, cudaMemcpyHostToDevice, c->st), "H2D");
     }
-    const uint8_t *dq = c->q.as<uint8_t>(), *dt = c->t.as<uint8_t>(), *dc = c->code.as<uint8_t>();
+    const uint8_t *dq = c->q.get(), *dt = c->t.get(), *dc = c->code.get();
     auto sweep_bytes = [nsym](const Prob &p) { return scratch_bytes(p.ql, nsym, 1, 0); };
 
     // (a) distance and end; HW and NW jobs in launches of their own, long NW jobs banded
@@ -798,17 +785,17 @@ int mm_align_batch(mm_align_ctx *c, const char *qbases, uint64_t n_q, const char
         }
         (b.mode == MM_ALIGN_NW ? nw : hw).push_back(p);
       }
-      ck(c, c->out_a.ensure(n_jobs * 4), "output allocation");
-      ck(c, c->out_b.ensure(n_jobs * 4), "output allocation");
+      ck(c, c->out_a.reserve(n_jobs * 4), "output allocation");
+      ck(c, c->out_b.reserve(n_jobs * 4), "output allocation");
       if (!hw.empty())
         run_waves(c, hw, sweep_bytes, [&](const Prob *dp, int n, int grid, int blk) {
-          k_align_hw<<<grid, blk, 0, c->st>>>(dp, n, dq, dt, dc, nsym, c->scratch.as<uint8_t>(), c->out_a.as<int>(),
-                                              c->out_b.as<int>());
+          k_align_hw<<<grid, blk, 0, c->st>>>(dp, n, dq, dt, dc, nsym, c->scratch.get(), (int *)c->out_a.get(),
+                                              (int *)c->out_b.get());
         });
       if (!nw.empty())
         run_waves(c, nw, sweep_bytes, [&](const Prob *dp, int n, int grid, int blk) {
-          k_align_nw<<<grid, blk, 0, c->st>>>(dp, n, dq, dt, dc, nsym, c->scratch.as<uint8_t>(), c->out_a.as<int>(),
-                                              c->out_b.as<int>());
+          k_align_nw<<<grid, blk, 0, c->st>>>(dp, n, dq, dt, dc, nsym, c->scratch.get(), (int *)c->out_a.get(),
+                                              (int *)c->out_b.get());
         });
       // Banded passes until each long job is decided. A pass's score is exact when it is <= the pass's bound and is the
       // cost of a real path (so >= the distance) otherwise: the next bound is that score or 4x the bound, whichever is
@@ -816,11 +803,11 @@ int mm_align_batch(mm_align_ctx *c, const char *qbases, uint64_t n_q, const char
       // that stays above it decides -1, as edlib does.
       std::vector<int> v(n_jobs);
       while (!band.empty()) {
-        ck(c, c->out_c.ensure(n_jobs * 4), "output allocation");
+        ck(c, c->out_c.reserve(n_jobs * 4), "output allocation");
         run_band(c, band, sweep_bytes, [&](const Prob *dp, int n, int threads) {
-          k_band_nw<<<n, threads, 0, c->st>>>(dp, dq, dt, dc, nsym, c->scratch.as<uint8_t>(), c->out_c.as<int>());
+          k_band_nw<<<n, threads, 0, c->st>>>(dp, dq, dt, dc, nsym, c->scratch.get(), (int *)c->out_c.get());
         });
-        ck(c, cudaMemcpy(v.data(), c->out_c.p, n_jobs * 4, cudaMemcpyDeviceToHost), "D2H");
+        ck(c, cudaMemcpy(v.data(), c->out_c.get(), n_jobs * 4, cudaMemcpyDeviceToHost), "D2H");
         std::vector<Prob> next;
         for (Prob p : band) {
           const mm_align_job &b = jobs[p.res];
@@ -831,8 +818,8 @@ int mm_align_batch(mm_align_ctx *c, const char *qbases, uint64_t n_q, const char
         }
         band.swap(next);
       }
-      ck(c, cudaMemcpyAsync(ed.data(), c->out_a.p, n_jobs * 4, cudaMemcpyDeviceToHost, c->st), "D2H");
-      ck(c, cudaMemcpyAsync(end.data(), c->out_b.p, n_jobs * 4, cudaMemcpyDeviceToHost, c->st), "D2H");
+      ck(c, cudaMemcpyAsync(ed.data(), c->out_a.get(), n_jobs * 4, cudaMemcpyDeviceToHost, c->st), "D2H");
+      ck(c, cudaMemcpyAsync(end.data(), c->out_b.get(), n_jobs * 4, cudaMemcpyDeviceToHost, c->st), "D2H");
     }
     for (const auto &x : band_ed) {
       ed[x.first] = x.second;
@@ -847,10 +834,10 @@ int mm_align_batch(mm_align_ctx *c, const char *qbases, uint64_t n_q, const char
           probs.push_back(Prob{jobs[j].q_offset, jobs[j].t_offset, jobs[j].q_len, end[j] + 1, 0, (int)j, 0, 0});
       if (!probs.empty()) {
         run_waves(c, probs, sweep_bytes, [&](const Prob *dp, int n, int grid, int blk) {
-          k_align_shw<<<grid, blk, 0, c->st>>>(dp, n, dq, dt, dc, nsym, c->scratch.as<uint8_t>(), c->out_a.as<int>());
+          k_align_shw<<<grid, blk, 0, c->st>>>(dp, n, dq, dt, dc, nsym, c->scratch.get(), (int *)c->out_a.get());
         });
         std::vector<int> s(n_jobs);
-        ck(c, cudaMemcpyAsync(s.data(), c->out_a.p, n_jobs * 4, cudaMemcpyDeviceToHost, c->st), "D2H");
+        ck(c, cudaMemcpyAsync(s.data(), c->out_a.get(), n_jobs * 4, cudaMemcpyDeviceToHost, c->st), "D2H");
         ck(c, cudaStreamSynchronize(c->st), "D2H");
         for (const Prob &p : probs) start[p.res] = s[p.res];
       }
@@ -873,24 +860,24 @@ int mm_align_batch(mm_align_ctx *c, const char *qbases, uint64_t n_q, const char
                                  i});
         if (probs.empty()) break;
         levels++;
-        ck(c, c->out_a.ensure(probs.size() * sizeof(int4)), "output allocation");
+        ck(c, c->out_a.reserve(probs.size() * sizeof(int4)), "output allocation");
         std::vector<Prob> shortp, longp;  // copies: probs keeps the node order for the merge below
         for (const Prob &p : probs) (is_long(p.ql, p.tl) ? longp : shortp).push_back(p);
         if (!shortp.empty())
           run_waves(c, shortp, [nsym](const Prob &p) { return scratch_bytes(p.ql, nsym, 1, (uint64_t)p.ql * 8 + 16); },
                     [&](const Prob *dp, int n, int grid, int blk) {
-                      k_align_hirsch<<<grid, blk, 0, c->st>>>(dp, n, dq, dt, dc, nsym, c->scratch.as<uint8_t>(),
-                                                              c->out_a.as<int4>());
+                      k_align_hirsch<<<grid, blk, 0, c->st>>>(dp, n, dq, dt, dc, nsym, c->scratch.get(),
+                                                              (int4 *)c->out_a.get());
                     });
         if (!longp.empty())  // both halves of a node as two CTAs, then the split
           run_band(c, longp, [nsym](const Prob &p) { return band_node_bytes(p.ql, nsym); },
                    [&](const Prob *dp, int n, int threads) {
-                     k_band_col<<<2 * n, threads, 0, c->st>>>(dp, dq, dt, dc, nsym, c->scratch.as<uint8_t>());
-                     k_band_split<<<(n + 3) / 4, 128, 0, c->st>>>(dp, n, nsym, c->scratch.as<uint8_t>(),
-                                                                  c->out_a.as<int4>());
+                     k_band_col<<<2 * n, threads, 0, c->st>>>(dp, dq, dt, dc, nsym, c->scratch.get());
+                     k_band_split<<<(n + 3) / 4, 128, 0, c->st>>>(dp, n, nsym, c->scratch.get(),
+                                                                  (int4 *)c->out_a.get());
                    });
         std::vector<int4> sp(probs.size());
-        ck(c, cudaMemcpy(sp.data(), c->out_a.p, sp.size() * sizeof(int4), cudaMemcpyDeviceToHost), "D2H");
+        ck(c, cudaMemcpy(sp.data(), c->out_a.get(), sp.size() * sizeof(int4), cudaMemcpyDeviceToHost), "D2H");
         std::vector<Node> next;
         next.reserve(nodes.size() + probs.size());
         size_t pi = 0;
@@ -928,12 +915,12 @@ int mm_align_batch(mm_align_ctx *c, const char *qbases, uint64_t n_q, const char
         probs.push_back(Prob{nd.q, nd.t, nd.ql, nd.tl, nd.score, (int)i, 0, off[i]});
       }
       if (!probs.empty()) {
-        ck(c, c->ops.ensure(off.back()), "op buffer allocation");
-        ck(c, c->out_n.ensure(nodes.size() * 4), "output allocation");
+        ck(c, c->ops.reserve(off.back()), "op buffer allocation");
+        ck(c, c->out_n.reserve(nodes.size() * 4), "output allocation");
         run_waves(c, probs, [nsym](const Prob &p) { return scratch_bytes(p.ql, nsym, (uint64_t)p.tl, 0); },
                   [&](const Prob *dp, int n, int grid, int blk) {
-                    k_align_leaf<<<grid, blk, 0, c->st>>>(dp, n, dq, dt, dc, nsym, c->scratch.as<uint8_t>(),
-                                                          c->ops.as<uint8_t>(), c->out_n.as<int>());
+                    k_align_leaf<<<grid, blk, 0, c->st>>>(dp, n, dq, dt, dc, nsym, c->scratch.get(),
+                                                          c->ops.get(), (int *)c->out_n.get());
                   });
       }
     }
@@ -943,9 +930,9 @@ int mm_align_batch(mm_align_ctx *c, const char *qbases, uint64_t n_q, const char
       for (size_t i = 0; i < nodes.size(); i++) any |= !failed[nodes[i].job] && nodes[i].ql && nodes[i].tl;
       if (any) {
         std::vector<int> dn(nodes.size());
-        ck(c, cudaMemcpyAsync(dn.data(), c->out_n.p, nodes.size() * 4, cudaMemcpyDeviceToHost, c->st), "D2H");
+        ck(c, cudaMemcpyAsync(dn.data(), c->out_n.get(), nodes.size() * 4, cudaMemcpyDeviceToHost, c->st), "D2H");
         std::vector<uint8_t> dops(off.back());
-        ck(c, cudaMemcpyAsync(dops.data(), c->ops.p, off.back(), cudaMemcpyDeviceToHost, c->st), "D2H");
+        ck(c, cudaMemcpyAsync(dops.data(), c->ops.get(), off.back(), cudaMemcpyDeviceToHost, c->st), "D2H");
         ck(c, cudaStreamSynchronize(c->st), "D2H");
         for (size_t i = 0; i < nodes.size(); i++)
           if (!failed[nodes[i].job] && nodes[i].ql && nodes[i].tl) {

@@ -15,6 +15,7 @@
 #include <string>
 #include <vector>
 
+#include "mm_devbuf.h"
 #include "mm_index_build.h"
 #include "mm_internal.h"
 #include <chrono>
@@ -30,58 +31,59 @@ struct mm_ctx {
   uint64_t launches = 0;
   uint64_t diag[8] = {0}; /* mm_ctx_diag: how often the rare paths ran (cumulative) */
 
-  /* index blob */
+  /* index blob: the context's own (own_blob), or a view of the one of share_src */
+  mm_devbuf<unsigned char> own_blob;
   unsigned char *blob = nullptr;
   uint64_t blob_bytes = 0;
-  bool blob_owned = false;
   bool blob_ready = false;
   mm_blob_header hdr{};
   mm_dev_index ix{};
   std::vector<int32_t> cutoffs, min_hits;
 
   /* batch */
-  uint8_t *d_bases = nullptr; uint64_t bases_cap = 0; uint64_t n_bases = 0;
-  uint8_t *d_packed = nullptr; uint64_t packed_cap = 0; /* nibbles, bytes */
+  mm_devbuf<uint8_t> d_bases; uint64_t n_bases = 0;
+  mm_devbuf<uint8_t> d_packed; /* nibbles */
   mm_built_index built{}; /* lookup arrays of an index built on the device, kept for mm_index_download (keep_lookup) */
   bool built_kept = false;
   bool batch_is_ascii = false; /* the resident batch came in as text: K0 (pack) runs in front of K1 */
   cudaEvent_t ev_pack = nullptr;
   float pack_ms = 0;
-  mm_segment *d_segs = nullptr; uint64_t segs_cap = 0; uint64_t n_segs = 0;
+  mm_devbuf<mm_segment> d_segs; uint64_t n_segs = 0;
   /* fragments longer than seg_length: K1 runs over d_work_segs = the caller's n_segs segments (a long one replaced by its
    * first piece), then the n_work - n_segs pieces the long ones are cut into; d_long lists them (n_long) */
-  mm_segment *d_work_segs = nullptr; uint64_t work_segs_cap = 0;
+  mm_devbuf<mm_segment> d_work_segs;
   uint64_t n_work = 0; uint32_t n_long = 0; uint64_t long_entries = 0;
-  uint64_t *d_sk_hash = nullptr; uint64_t *d_sk_val = nullptr; int2 *d_sk_pos = nullptr; int8_t *d_sk_strand = nullptr; uint64_t sk_cap = 0;
-  mm_segment_result *d_seg_res = nullptr;
-  uint32_t *d_sk_reject = nullptr;
+  mm_devbuf<uint64_t> d_sk_hash, d_sk_val; mm_devbuf<int2> d_sk_pos; mm_devbuf<int8_t> d_sk_strand;
+  mm_devbuf<mm_segment_result> d_seg_res;
+  mm_devbuf<uint32_t> d_sk_reject;
   int sk_mode = 0; /* 0 = fast sketch kernel + general kernel over its rejects; 1 = general kernel only (MM_SKETCH_TABLE=1) */
   /* fragments longer than seg_length: vote sums of the pieces, the fragment list and the merge area (K1); the live-table
    * offsets, the scan's work area and the live tables (K3) */
-  int32_t *d_sk_votes = nullptr; uint64_t votes_cap = 0;
-  mm_long_frag *d_long = nullptr; uint64_t long_cap = 0;
-  uint64_t *d_long_off = nullptr; uint64_t long_off_cap = 0;
-  unsigned char *d_long_tmp = nullptr; uint64_t long_tmp_cap = 0;
-  uint64_t *d_l2_long_off = nullptr; uint64_t l2_long_off_cap = 0;
-  unsigned char *d_long_scan_tmp = nullptr; uint64_t long_scan_tmp_cap = 0;
-  uint64_t *d_long_table = nullptr; uint64_t long_table_cap = 0;
-  mm_l1_candidate *d_cands = nullptr; uint64_t cand_cap = 0;
-  mm_l2_locus *d_loci = nullptr; uint64_t loci_cap = 0;
-  uint32_t *d_counters = nullptr;
+  mm_devbuf<int32_t> d_sk_votes;
+  mm_devbuf<mm_long_frag> d_long;
+  mm_devbuf<uint64_t> d_long_off;
+  mm_devbuf<unsigned char> d_long_tmp;
+  mm_devbuf<uint64_t> d_l2_long_off;
+  mm_devbuf<unsigned char> d_long_scan_tmp;
+  mm_devbuf<uint64_t> d_long_table;
+  mm_devbuf<mm_l1_candidate> d_cands;
+  mm_devbuf<mm_l2_locus> d_loci;
+  mm_devbuf<uint32_t> d_counters;
   bool blocking_wait = false;       /* MM_BLOCKING_WAIT=1: host waits block on an event instead of spinning (experiment) */
   cudaEvent_t ev_wait = nullptr;
   const mm_ctx *share_src = nullptr; /* mm_ctx_share_index: the context whose index image this one reads */
   mm_phase_hook hook = nullptr;
   void *hook_user = nullptr;
   uint32_t *h_pub = nullptr; /* pinned, device-mapped: kernels publish counters here (no copy engine involved) */
-  uint64_t *d_scratch = nullptr; uint64_t scratch_cap = 0; uint64_t scratch_slice = 0; uint64_t scratch_pool = 0;
+  mm_devbuf<uint64_t> d_scratch; uint64_t scratch_slice = 0; uint64_t scratch_pool = 0;
   uint32_t l1_grid = 0;
   uint64_t n_cands = 0, n_loci = 0;
-  mm_l2_range *d_l2_ranges = nullptr; uint64_t *d_l2_rec_off = nullptr; uint64_t l2_cand_cap = 0;
-  uint2 *d_l2_recs = nullptr; uint64_t l2_recs_cap = 0;
-  void *d_scan_tmp = nullptr; size_t scan_tmp_bytes = 0;
-  uint32_t *d_l1_slow = nullptr; uint64_t l1_slow_cap = 0;
-  void *d_l2_order = nullptr; size_t l2_order_bytes = 0; /* work area of the candidate ordering (mm_launch_l2_order) */
+  /* the L2 stream path's own work areas: the ranges, the record offsets, the scan's and the candidate ordering's
+   * (mm_launch_l2_order) temporaries are sized together, by d_l2_ranges' capacity; then the operation records */
+  mm_devbuf<mm_l2_range> d_l2_ranges; mm_devbuf<uint64_t> d_l2_rec_off;
+  mm_devbuf<unsigned char> d_scan_tmp, d_l2_order;
+  mm_devbuf<uint2> d_l2_recs;
+  mm_devbuf<uint32_t> d_l1_slow;
   int l1_warp = 1; /* 1 = warp-per-segment fast path + CTA path for big segments; 0 = CTA path only (MM_L1_CTA=1) */
   int l2_mode = 1; /* 1 = stream kernels (mm_l2_stream.cu), 0 = general kernel only (MM_L2_GENERAL=1) */
   bool batch_mapped = false;
@@ -110,17 +112,6 @@ int fail(mm_ctx *c, int code, const char *fmt, ...)
       return fail(c, e_ == cudaErrorMemoryAllocation ? MM_ENOMEM : MM_ECUDA, "%s: %s", #call,    \
                   cudaGetErrorString(e_));                                                       \
   } while (0)
-
-template <typename T>
-int grow(mm_ctx *c, T *&ptr, uint64_t &cap, uint64_t need, uint64_t pad = 0)
-{
-  if (need + pad <= cap && ptr) return MM_OK;
-  if (ptr) { cudaFree(ptr); ptr = nullptr; cap = 0; }
-  uint64_t n = need + pad;
-  CU(c, cudaMalloc((void **)&ptr, n * sizeof(T)));
-  cap = n;
-  return MM_OK;
-}
 
 uint64_t align_up(uint64_t x, uint64_t a) { return (x + a - 1) / a * a; }
 
@@ -167,6 +158,86 @@ int write_tables(mm_ctx *c)
   return MM_OK;
 }
 
+/* the context has no index afterwards: its own image is freed, a shared one is no longer read */
+void drop_index(mm_ctx *c)
+{
+  c->own_blob.reset();
+  c->blob = nullptr; c->blob_bytes = 0; c->blob_ready = false; c->share_src = nullptr;
+}
+
+/* an index upload or build that returns before its image is complete leaves the context with no index */
+struct image_guard {
+  mm_ctx *c;
+  ~image_guard() { if (!c->blob_ready) drop_index(c); }
+};
+
+/* lays out the index image for these counts (mm_internal.h) and allocates it as the context's own */
+int begin_image(mm_ctx *c, uint64_t n_mi, uint64_t n_keys, uint64_t n_points, int32_t n_contigs)
+{
+  mm_blob_header h{};
+  h.magic = MM_BLOB_MAGIC;
+  h.n_minmers = n_mi; h.n_keys = n_keys; h.n_points = n_points;
+  h.n_contigs = n_contigs; h.tab_log2 = 4;
+  while ((1ULL << h.tab_log2) < 2 * n_keys + 2) h.tab_log2++;
+  uint64_t o = align_up(sizeof(mm_blob_header), 256);
+  auto place = [&](uint64_t bytes) { uint64_t at = o; o = align_up(o + bytes, 256); return at; };
+  h.off_idx_hash = place((n_mi + 1) * 8);
+  h.off_idx_wpos = place((n_mi + 1) * 4);
+  h.off_idx_wend = place((n_mi + 1) * 4);
+  h.off_idx_strand = place(n_mi + 1);
+  h.off_contig_start = place(((uint64_t)n_contigs + 1) * 8);
+  h.off_idx2_hash = place((n_mi + 1) * 8);
+  h.off_idx2_wend = place((n_mi + 1) * 4);
+  h.off_tab = place((1ULL << h.tab_log2) * sizeof(mm_tab_slot));
+  h.off_pts = place((n_points + 1) * 8);
+  h.off_contig_len = place((uint64_t)n_contigs * 4);
+  h.off_contig_name_id = place((uint64_t)n_contigs * 4);
+  h.off_contig_group = place((uint64_t)n_contigs * 4);
+  h.off_cutoffs = place(TABLE_REGION_BYTES);
+  h.off_min_hits = place(TABLE_REGION_BYTES);
+  h.total_bytes = o;
+  if (c->own_blob.reserve(o) != cudaSuccess)
+    return fail(c, MM_ENOMEM, "cannot allocate the index image (%llu bytes)", (unsigned long long)o);
+  c->blob = c->own_blob.get(); c->blob_bytes = o; c->hdr = h;
+  return MM_OK;
+}
+
+/* Completes the image begun by begin_image once the caller has put the SoA index and the packed points in place (and
+ * flagged bad points in d_err, bit 1): contig starts, death order, lookup table from the device key lists, contig
+ * tables, header. Then the context reads it. */
+int finish_image(mm_ctx *c, const std::vector<uint64_t> &cstart, const uint64_t *d_keys, const uint64_t *d_offs,
+                 const uint8_t *d_freq, uint32_t *d_err, const int32_t *contig_len, const int32_t *contig_name_id,
+                 const int32_t *contig_group)
+{
+  const mm_blob_header &h = c->hdr;
+  const size_t n_contigs = (size_t)h.n_contigs;
+  CU(c, cudaMemcpyAsync(c->blob + h.off_contig_start, cstart.data(), cstart.size() * 8, cudaMemcpyHostToDevice, c->stream));
+  /* the same entries per contig in wpos_end order (device sort), for the L2 stream merge */
+  CU(c, mm_build_death_order((const uint64_t *)(c->blob + h.off_idx_hash), (const int32_t *)(c->blob + h.off_idx_wend),
+                             (const uint64_t *)(c->blob + h.off_contig_start), h.n_contigs, h.n_minmers,
+                             (uint64_t *)(c->blob + h.off_idx2_hash), (int32_t *)(c->blob + h.off_idx2_wend), c->stream));
+  /* open-addressing table, filled on the device */
+  CU(c, cudaMemsetAsync(c->blob + h.off_tab, 0, (1ULL << h.tab_log2) * sizeof(mm_tab_slot), c->stream));
+  CU(c, mm_upload_build_table(d_keys, d_offs, d_freq, h.n_keys, (mm_tab_slot *)(c->blob + h.off_tab), h.tab_log2, d_err, c->stream));
+  uint32_t err = 0;
+  CU(c, cudaMemcpyAsync(&err, d_err, 4, cudaMemcpyDeviceToHost, c->stream));
+  CU(c, cudaStreamSynchronize(c->stream));
+  if (err & 1) return fail(c, MM_EINVAL, "an interval point has a bad seqId or a negative position");
+  if (err & 2) return fail(c, MM_EINVAL, "a key has no or too many (>= 2^24) interval points, or offsets overflow");
+  if (err & 4) return fail(c, MM_EINVAL, "duplicate key in the lookup index");
+  CU(c, cudaMemcpyAsync(c->blob + h.off_contig_len, contig_len, n_contigs * 4, cudaMemcpyHostToDevice, c->stream));
+  std::vector<int32_t> tmp(n_contigs, -1);
+  CU(c, cudaMemcpyAsync(c->blob + h.off_contig_name_id, contig_name_id ? contig_name_id : tmp.data(), n_contigs * 4, cudaMemcpyHostToDevice, c->stream));
+  CU(c, cudaStreamSynchronize(c->stream)); /* tmp is rewritten below */
+  std::fill(tmp.begin(), tmp.end(), 0);
+  CU(c, cudaMemcpyAsync(c->blob + h.off_contig_group, contig_group ? contig_group : tmp.data(), n_contigs * 4, cudaMemcpyHostToDevice, c->stream));
+  CU(c, cudaMemcpyAsync(c->blob, &c->hdr, sizeof(c->hdr), cudaMemcpyHostToDevice, c->stream));
+  CU(c, cudaStreamSynchronize(c->stream));
+  resolve_index(c);
+  c->blob_ready = true;
+  return write_tables(c);
+}
+
 /* wait for the context's stream. Default: cudaStreamSynchronize (spins, lowest latency). With MM_BLOCKING_WAIT=1 the
  * thread sleeps on a blocking event instead -- for hosts with fewer usable CPUs than pipeline threads (DESIGN section 9). */
 cudaError_t wait_stream(mm_ctx *c)
@@ -210,37 +281,20 @@ int validate_segments(mm_ctx *c, const mm_segment *segs, uint64_t n_segs, uint64
 /* batch buffers that do not depend on the input format */
 int prepare_batch_buffers(mm_ctx *c, uint64_t n_bases, uint64_t n_segs)
 {
-  int rc;
   /* nibbles: n_bases/2 rounded up to 8-byte groups of 16 bases, + 256 so that the 16-byte-granular bulk copies of the
    * sketch kernel never leave the allocation */
-  const uint64_t pbytes = (n_bases + 15) / 16 * 8;
-  if (pbytes + 256 > c->packed_cap || !c->d_packed) {
-    if (c->d_packed) { cudaFree(c->d_packed); c->d_packed = nullptr; c->packed_cap = 0; }
-    CU(c, cudaMalloc((void **)&c->d_packed, pbytes + 256));
-    c->packed_cap = pbytes + 256;
-    CU(c, cudaMemsetAsync(c->d_packed, 0x88, c->packed_cap, c->stream));
-  }
-  if ((rc = grow(c, c->d_segs, c->segs_cap, n_segs, 1))) return rc;
-  const uint64_t S = (uint64_t)c->params.sketch_size;
-  if (n_segs * S + 1 > c->sk_cap || !c->d_sk_hash) {
-    if (c->d_sk_hash) cudaFree(c->d_sk_hash);
-    if (c->d_sk_val) cudaFree(c->d_sk_val);
-    if (c->d_sk_pos) cudaFree(c->d_sk_pos);
-    if (c->d_sk_strand) cudaFree(c->d_sk_strand);
-    if (c->d_seg_res) cudaFree(c->d_seg_res);
-    if (c->d_sk_reject) cudaFree(c->d_sk_reject);
-    c->d_sk_reject = nullptr;
-    c->d_sk_hash = nullptr; c->d_sk_val = nullptr; c->d_sk_pos = nullptr; c->d_sk_strand = nullptr; c->d_seg_res = nullptr; c->sk_cap = 0;
-    const uint64_t n = n_segs * S + 1;
-    CU(c, cudaMalloc((void **)&c->d_sk_hash, n * 8));
-    CU(c, cudaMalloc((void **)&c->d_sk_val, n * 8));
-    CU(c, cudaMalloc((void **)&c->d_sk_pos, n * 8));
-    CU(c, cudaMalloc((void **)&c->d_sk_strand, n));
-    CU(c, cudaMalloc((void **)&c->d_seg_res, (n_segs + 1) * sizeof(mm_segment_result)));
-    CU(c, cudaMalloc((void **)&c->d_sk_reject, (n_segs + 1) * 4));
-    c->sk_cap = n;
-  }
-  if (!c->d_counters) CU(c, cudaMalloc((void **)&c->d_counters, 64));
+  const uint64_t pbytes = (n_bases + 15) / 16 * 8, packed_had = c->d_packed.capacity();
+  CU(c, c->d_packed.reserve(pbytes + 256));
+  if (c->d_packed.capacity() != packed_had) CU(c, cudaMemsetAsync(c->d_packed.get(), 0x88, c->d_packed.capacity(), c->stream));
+  CU(c, c->d_segs.reserve(n_segs + 1));
+  const uint64_t n = n_segs * (uint64_t)c->params.sketch_size + 1;
+  CU(c, c->d_sk_hash.reserve(n));
+  CU(c, c->d_sk_val.reserve(n));
+  CU(c, c->d_sk_pos.reserve(n));
+  CU(c, c->d_sk_strand.reserve(n));
+  CU(c, c->d_seg_res.reserve(n_segs + 1));
+  CU(c, c->d_sk_reject.reserve(n_segs + 1));
+  CU(c, c->d_counters.reserve(16));
   return MM_OK;
 }
 
@@ -299,6 +353,10 @@ int upload_batch(mm_ctx *c, const void *bases, uint64_t n_bases, const mm_segmen
   int rc = validate_segments(c, segs, n_segs, n_bases);
   if (rc) return rc;
   CU(c, cudaSetDevice(c->device));
+  /* a failed upload leaves an empty batch, not counts that its buffers may no longer hold */
+  c->n_segs = c->n_work = 0;
+  c->n_long = 0;
+  c->batch_mapped = false;
   const uint64_t S = (uint64_t)c->params.sketch_size;
   const int L = c->params.seg_length, step = L - c->params.kmer_size + 1;
   std::vector<mm_segment> work;
@@ -324,27 +382,27 @@ int upload_batch(mm_ctx *c, const void *bases, uint64_t n_bases, const mm_segmen
     return fail(c, MM_EINVAL, "too many segments in one batch after cutting the long fragments into pieces");
   if ((rc = prepare_batch_buffers(c, n_bases, n_work))) return rc;
   if (!longs.empty()) {
-    if ((rc = grow(c, c->d_work_segs, c->work_segs_cap, n_work))) return rc;
-    CU(c, cudaMemcpyAsync(c->d_work_segs, work.data(), n_work * sizeof(mm_segment), cudaMemcpyHostToDevice, c->stream));
-    if ((rc = grow(c, c->d_sk_votes, c->votes_cap, c->sk_cap))) return rc;
-    if ((rc = grow(c, c->d_long, c->long_cap, longs.size()))) return rc;
-    if ((rc = grow(c, c->d_long_off, c->long_off_cap, entry_off.size()))) return rc;
-    if ((rc = grow(c, c->d_long_tmp, c->long_tmp_cap, mm_sketch_long_tmp_bytes(entry_off.back(), (uint32_t)longs.size())))) return rc;
-    CU(c, cudaMemcpyAsync(c->d_long, longs.data(), longs.size() * sizeof(mm_long_frag), cudaMemcpyHostToDevice, c->stream));
-    CU(c, cudaMemcpyAsync(c->d_long_off, entry_off.data(), entry_off.size() * 8, cudaMemcpyHostToDevice, c->stream));
+    CU(c, c->d_work_segs.reserve(n_work));
+    CU(c, cudaMemcpyAsync(c->d_work_segs.get(), work.data(), n_work * sizeof(mm_segment), cudaMemcpyHostToDevice, c->stream));
+    CU(c, c->d_sk_votes.reserve(c->d_sk_hash.capacity()));
+    CU(c, c->d_long.reserve(longs.size()));
+    CU(c, c->d_long_off.reserve(entry_off.size()));
+    CU(c, c->d_long_tmp.reserve(mm_sketch_long_tmp_bytes(entry_off.back(), (uint32_t)longs.size())));
+    CU(c, cudaMemcpyAsync(c->d_long.get(), longs.data(), longs.size() * sizeof(mm_long_frag), cudaMemcpyHostToDevice, c->stream));
+    CU(c, cudaMemcpyAsync(c->d_long_off.get(), entry_off.data(), entry_off.size() * 8, cudaMemcpyHostToDevice, c->stream));
   }
   CU(c, cudaEventRecord(c->ev[6], c->stream));
   if (packed) {
     const uint64_t pbytes = (n_bases + 1) / 2;
-    if ((rc = copy_in(c, c->d_packed, bases, pbytes))) return rc;
-    CU(c, cudaMemsetAsync(c->d_packed + pbytes, 0x88, 64, c->stream));
+    if ((rc = copy_in(c, c->d_packed.get(), bases, pbytes))) return rc;
+    CU(c, cudaMemsetAsync(c->d_packed.get() + pbytes, 0x88, 64, c->stream));
     if (n_bases & 1) { /* the unused high nibble of the last byte is whatever the caller had there: irrelevant (never a k-mer) */ }
   } else {
-    if ((rc = grow(c, c->d_bases, c->bases_cap, n_bases, 256))) return rc;
-    if ((rc = copy_in(c, c->d_bases, bases, n_bases))) return rc;
-    CU(c, cudaMemsetAsync(c->d_bases + n_bases, 'N', 256, c->stream));
+    CU(c, c->d_bases.reserve(n_bases + 256));
+    if ((rc = copy_in(c, c->d_bases.get(), bases, n_bases))) return rc;
+    CU(c, cudaMemsetAsync(c->d_bases.get() + n_bases, 'N', 256, c->stream));
   }
-  CU(c, cudaMemcpyAsync(c->d_segs, segs, n_segs * sizeof(mm_segment), cudaMemcpyHostToDevice, c->stream));
+  CU(c, cudaMemcpyAsync(c->d_segs.get(), segs, n_segs * sizeof(mm_segment), cudaMemcpyHostToDevice, c->stream));
   CU(c, cudaEventRecord(c->ev[7], c->stream));
   if (!longs.empty()) CU(c, cudaStreamSynchronize(c->stream)); /* work / longs / entry_off are about to go */
   c->n_bases = n_bases;
@@ -353,7 +411,6 @@ int upload_batch(mm_ctx *c, const void *bases, uint64_t n_bases, const mm_segmen
   c->n_long = (uint32_t)longs.size();
   c->long_entries = entry_off.back();
   c->batch_is_ascii = !packed;
-  c->batch_mapped = false;
   return MM_OK;
 }
 
@@ -361,7 +418,7 @@ int upload_batch(mm_ctx *c, const void *bases, uint64_t n_bases, const mm_segmen
 int launch_pack_if_ascii(mm_ctx *c)
 {
   if (!c->batch_is_ascii) { c->pack_ms = 0; return MM_OK; }
-  CU(c, mm_launch_pack_bases(c->d_bases, c->d_packed, c->n_bases, c->stream, c->sm_count));
+  CU(c, mm_launch_pack_bases(c->d_bases.get(), c->d_packed.get(), c->n_bases, c->stream, c->sm_count));
   c->launches++;
   return MM_OK;
 }
@@ -374,7 +431,7 @@ mm_dev_batch make_batch(mm_ctx *c);
 int launch_sketch_all(mm_ctx *c, bool probe)
 {
   mm_dev_batch b = make_batch(c);
-  if (c->n_long) b.segs = c->d_work_segs;
+  if (c->n_long) b.segs = c->d_work_segs.get();
   if (!probe) b.sk_val = nullptr;
   CU(c, mm_launch_sketch(c->params, c->ix, b, c->stream, c->sm_count, c->sk_mode));
   c->launches += c->sk_mode ? 1 : 2;
@@ -382,13 +439,13 @@ int launch_sketch_all(mm_ctx *c, bool probe)
     /* the pieces: general kernel (it writes the vote sums the merge needs), then the merge */
     const uint64_t S = (uint64_t)c->params.sketch_size, n0 = c->n_segs;
     mm_dev_batch bp = b;
-    bp.segs = c->d_work_segs + n0; bp.n_segs = (uint32_t)(c->n_work - n0);
-    bp.sk_hash = c->d_sk_hash + n0 * S; bp.sk_pos = c->d_sk_pos + n0 * S; bp.sk_strand = c->d_sk_strand + n0 * S;
-    bp.sk_votes = c->d_sk_votes + n0 * S; bp.seg_res = c->d_seg_res + n0; bp.sk_val = nullptr;
+    bp.segs = c->d_work_segs.get() + n0; bp.n_segs = (uint32_t)(c->n_work - n0);
+    bp.sk_hash = b.sk_hash + n0 * S; bp.sk_pos = b.sk_pos + n0 * S; bp.sk_strand = b.sk_strand + n0 * S;
+    bp.sk_votes = c->d_sk_votes.get() + n0 * S; bp.seg_res = b.seg_res + n0; bp.sk_val = nullptr;
     CU(c, mm_launch_sketch(c->params, c->ix, bp, c->stream, c->sm_count, 1));
-    b.sk_votes = c->d_sk_votes;
-    CU(c, mm_launch_sketch_long_merge(c->params, c->ix, b, c->d_long, c->d_long_off, c->n_long, (uint32_t)n0, c->long_entries,
-                                      c->d_long_tmp, c->long_tmp_cap, c->stream));
+    b.sk_votes = c->d_sk_votes.get();
+    CU(c, mm_launch_sketch_long_merge(c->params, c->ix, b, c->d_long.get(), c->d_long_off.get(), c->n_long, (uint32_t)n0,
+                                      c->long_entries, c->d_long_tmp.get(), c->d_long_tmp.capacity(), c->stream));
     c->launches += 3; /* pieces, prep, merge (the segmented sort is a library call, not counted) */
   }
   return MM_OK;
@@ -397,15 +454,16 @@ int launch_sketch_all(mm_ctx *c, bool probe)
 mm_dev_batch make_batch(mm_ctx *c)
 {
   mm_dev_batch b{};
-  b.bases = c->d_bases; b.packed = c->d_packed; b.segs = c->d_segs; b.n_segs = (uint32_t)c->n_segs;
-  b.sk_hash = c->d_sk_hash; b.sk_val = c->d_sk_val; b.sk_pos = c->d_sk_pos; b.sk_strand = c->d_sk_strand;
-  b.seg_res = c->d_seg_res; b.sk_reject = c->d_sk_reject;
-  b.cands = c->d_cands; b.cand_cap = (uint32_t)std::min<uint64_t>(c->cand_cap, 0xffffffffu);
-  b.loci = c->d_loci; b.loci_cap = (uint32_t)std::min<uint64_t>(c->loci_cap, 0xffffffffu);
-  b.counters = c->d_counters;
-  b.scratch = c->d_scratch; b.scratch_slice = c->scratch_slice; b.scratch_pool_off = c->scratch_pool;
-  b.scratch_cap = c->scratch_cap;
-  b.l2_ranges = c->d_l2_ranges; b.l2_rec_off = c->d_l2_rec_off; b.l2_recs = c->d_l2_recs; b.l2_recs_cap = c->l2_recs_cap;
+  b.bases = c->d_bases.get(); b.packed = c->d_packed.get(); b.segs = c->d_segs.get(); b.n_segs = (uint32_t)c->n_segs;
+  b.sk_hash = c->d_sk_hash.get(); b.sk_val = c->d_sk_val.get(); b.sk_pos = c->d_sk_pos.get(); b.sk_strand = c->d_sk_strand.get();
+  b.seg_res = c->d_seg_res.get(); b.sk_reject = c->d_sk_reject.get();
+  b.cands = c->d_cands.get(); b.cand_cap = (uint32_t)std::min<uint64_t>(c->d_cands.capacity(), 0xffffffffu);
+  b.loci = c->d_loci.get(); b.loci_cap = (uint32_t)std::min<uint64_t>(c->d_loci.capacity(), 0xffffffffu);
+  b.counters = c->d_counters.get();
+  b.scratch = c->d_scratch.get(); b.scratch_slice = c->scratch_slice; b.scratch_pool_off = c->scratch_pool;
+  b.scratch_cap = c->d_scratch.capacity();
+  b.l2_ranges = c->d_l2_ranges.get(); b.l2_rec_off = c->d_l2_rec_off.get();
+  b.l2_recs = c->d_l2_recs.get(); b.l2_recs_cap = c->d_l2_recs.capacity();
   b.l2_loci_per_cand = 2;
   return b;
 }
@@ -417,13 +475,9 @@ int ensure_scratch(mm_ctx *c, uint64_t pool_elems)
     if (c->l1_grid == 0) return fail(c, MM_ECUDA, "cannot size the L1 grid");
   }
   const uint64_t slice = 3ULL << 16; /* 65536 points per CTA slice */
-  const uint64_t need = slice * c->l1_grid + pool_elems;
-  if (c->d_scratch && c->scratch_cap >= need) return MM_OK;
-  if (c->d_scratch) { cudaFree(c->d_scratch); c->d_scratch = nullptr; }
-  CU(c, cudaMalloc((void **)&c->d_scratch, need * 8));
-  c->scratch_cap = need;
   c->scratch_slice = slice;
   c->scratch_pool = slice * c->l1_grid;
+  CU(c, c->d_scratch.reserve(c->scratch_pool + pool_elems));
   return MM_OK;
 }
 
@@ -450,8 +504,11 @@ int read_words(mm_ctx *c, const void *dev, uint32_t *out, int n_words)
 }
 #define RD(c, dev, out, n) do { int rc__ = read_words((c), (dev), (out), (n)); if (rc__) return rc__; } while (0)
 
+/* returned by run_l2_stream when its own work areas cannot be allocated: the general kernel maps the batch instead */
+constexpr int L2_STREAM_NO_ROOM = 1;
+
 /* K3 fast path (mm_l2_stream.cu): ranges+scan -> records -> lane-per-candidate scan -> general kernel for the
- * candidates that need more locus slots. Returns MM_ENOMEM if the record buffer cannot be allocated. */
+ * candidates that need more locus slots. */
 int run_l2_stream(mm_ctx *c, uint32_t *h_cnt)
 {
   const uint64_t nc = c->n_cands;
@@ -463,49 +520,30 @@ int run_l2_stream(mm_ctx *c, uint32_t *h_cnt)
     c->n_loci = 0;
     return MM_OK;
   }
-  if (nc + 1 > c->l2_cand_cap) {
-    if (c->d_l2_ranges) cudaFree(c->d_l2_ranges);
-    if (c->d_l2_rec_off) cudaFree(c->d_l2_rec_off);
-    if (c->d_scan_tmp) cudaFree(c->d_scan_tmp);
-    c->d_l2_ranges = nullptr; c->d_l2_rec_off = nullptr; c->d_scan_tmp = nullptr;
-    c->l2_cand_cap = nc + nc / 8 + 1024;
-    CU(c, cudaMalloc((void **)&c->d_l2_ranges, c->l2_cand_cap * sizeof(mm_l2_range)));
-    CU(c, cudaMalloc((void **)&c->d_l2_rec_off, (c->l2_cand_cap + 1) * 8));
-    c->scan_tmp_bytes = mm_l2_scan_tmp_bytes((uint32_t)c->l2_cand_cap);
-    CU(c, cudaMalloc(&c->d_scan_tmp, c->scan_tmp_bytes + 256));
-    if (c->d_l2_order) cudaFree(c->d_l2_order);
-    c->d_l2_order = nullptr;
-    c->l2_order_bytes = mm_l2_order_bytes((uint32_t)c->l2_cand_cap);
-    CU(c, cudaMalloc(&c->d_l2_order, c->l2_order_bytes));
+  if (nc + 1 > c->d_l2_ranges.capacity()) {
+    const uint64_t want = nc + nc / 8 + 1024;
+    if (c->d_l2_ranges.reserve(want) || c->d_l2_rec_off.reserve(want + 1) ||
+        c->d_scan_tmp.reserve(mm_l2_scan_tmp_bytes((uint32_t)want) + 256) ||
+        c->d_l2_order.reserve(mm_l2_order_bytes((uint32_t)want))) {
+      c->d_l2_ranges.reset(); /* its capacity stands for all four */
+      return L2_STREAM_NO_ROOM;
+    }
   }
-  if (c->loci_cap < nc * LPC + 1024) {
-    if (c->d_loci) cudaFree(c->d_loci);
-    c->d_loci = nullptr;
-    c->loci_cap = nc * LPC + nc / 8 + 4096;
-    CU(c, cudaMalloc((void **)&c->d_loci, c->loci_cap * sizeof(mm_l2_locus)));
-  }
+  if (c->d_loci.capacity() < nc * LPC + 1024) CU(c, c->d_loci.reserve(nc * LPC + nc / 8 + 4096));
   mm_dev_batch b = make_batch(c);
   const auto tk0 = std::chrono::steady_clock::now();
-  ZERO_WORDS(c, c->d_l2_rec_off + nc, 2);
-  CU(c, mm_launch_l2_ranges(c->params, c->ix, b, (uint32_t)nc, c->d_scan_tmp, c->scan_tmp_bytes + 256, c->stream));
+  ZERO_WORDS(c, c->d_l2_rec_off.get() + nc, 2);
+  CU(c, mm_launch_l2_ranges(c->params, c->ix, b, (uint32_t)nc, c->d_scan_tmp.get(), c->d_scan_tmp.capacity(), c->stream));
   uint64_t total = 0;
-  RD(c, c->d_l2_rec_off + nc, (uint32_t *)&total, 2);
+  RD(c, c->d_l2_rec_off.get() + nc, (uint32_t *)&total, 2);
   const auto tk1 = std::chrono::steady_clock::now();
   c->stage_ms[6] = std::chrono::duration<float, std::milli>(tk1 - tk0).count(); /* host view: ranges + scan + readback */
-  if (total + 64 > c->l2_recs_cap) { /* the scan's record readers run up to 2 * RING_CHUNKS + 2 records past a stream's end */
-    if (c->d_l2_recs) cudaFree(c->d_l2_recs);
-    c->d_l2_recs = nullptr; c->l2_recs_cap = 0;
-    const uint64_t want = total + total / 16 + 1024;
-    if (cudaMalloc((void **)&c->d_l2_recs, want * sizeof(uint2)) != cudaSuccess) {
-      cudaGetLastError();
-      return fail(c, MM_ENOMEM, "cannot allocate %llu L2 operation records", (unsigned long long)want);
-    }
-    c->l2_recs_cap = want;
-  }
+  /* the scan's record readers run up to 2 * RING_CHUNKS + 2 records past a stream's end */
+  if (total + 64 > c->d_l2_recs.capacity() && c->d_l2_recs.reserve(total + total / 16 + 1024)) return L2_STREAM_NO_ROOM;
   for (int attempt = 0; attempt < 4; attempt++) {
     b = make_batch(c);
-    ZERO_WORDS(c, c->d_counters + 1, 1);
-    ZERO_WORDS(c, c->d_counters + 6, 2);
+    ZERO_WORDS(c, c->d_counters.get() + 1, 1);
+    ZERO_WORDS(c, c->d_counters.get() + 6, 2);
     /* the record-preparation kernel is the bandwidth-bound one: no PCIe upload next to it (MM_PHASE_L2) */
     {
       struct phase_guard { /* the hook is always closed, whatever fails in between */
@@ -519,29 +557,27 @@ int run_l2_stream(mm_ctx *c, uint32_t *h_cnt)
       CU(c, cudaEventRecord(c->ev[9], c->stream));
       if (guard.open && c->blocking_wait) CU(c, cudaEventRecord(c->ev_wait, c->stream));
       uint32_t *perm = nullptr;
-      CU(c, mm_launch_l2_order(b, (uint32_t)nc, c->d_l2_order, c->l2_order_bytes, &perm, c->stream));
+      CU(c, mm_launch_l2_order(b, (uint32_t)nc, c->d_l2_order.get(), c->d_l2_order.capacity(), &perm, c->stream));
       b.l2_perm = perm;
       CU(c, mm_launch_l2_scan(c->params, c->ix, b, (uint32_t)nc, c->stream, c->sm_count));
       /* the scan is already queued behind it: waiting for the end of the preparation kernel costs no bubble */
       if (guard.open) CU(c, cudaEventSynchronize(c->blocking_wait ? c->ev_wait : c->ev[9]));
     }
     c->launches += 4; /* own kernels: ranges, prep, order keys, scan (the prefix sum and the sort are library calls, not counted) */
-    RD(c, c->d_counters, h_cnt, 16);
+    RD(c, c->d_counters.get(), h_cnt, 16);
     uint64_t extent = nc * LPC;
     if (h_cnt[7] > 0) { /* candidates with more than LPC loci: general kernel, loci appended after the fixed slots */
       c->diag[MM_DIAG_L2_GENERAL_CANDS] += h_cnt[7];
       const uint32_t base = (uint32_t)extent;
-      k_set_u32<<<1, 1, 0, c->stream>>>(c->d_counters + 6, base);
+      k_set_u32<<<1, 1, 0, c->stream>>>(c->d_counters.get() + 6, base);
       c->launches++;
       CU(c, mm_launch_l2_overflow(c->params, c->ix, b, (uint32_t)nc, c->stream, c->sm_count));
       c->launches += 1;
-      RD(c, c->d_counters, h_cnt, 16);
+      RD(c, c->d_counters.get(), h_cnt, 16);
       if (h_cnt[1] == 2) return fail(c, MM_ECUDA, "L2 live-set overflow in the general kernel");
-      if (h_cnt[1] == 1 || h_cnt[6] > c->loci_cap) { /* grow and redo prep+scan+overflow */
+      if (h_cnt[1] == 1 || h_cnt[6] > c->d_loci.capacity()) { /* grow and redo prep+scan+overflow */
         c->diag[MM_DIAG_L2_LOCI_REGROW]++;
-        cudaFree(c->d_loci); c->d_loci = nullptr;
-        c->loci_cap = (uint64_t)h_cnt[6] + h_cnt[6] / 4 + 1024;
-        CU(c, cudaMalloc((void **)&c->d_loci, c->loci_cap * sizeof(mm_l2_locus)));
+        CU(c, c->d_loci.reserve((uint64_t)h_cnt[6] + h_cnt[6] / 4 + 1024));
         continue;
       }
       extent = h_cnt[6];
@@ -563,34 +599,52 @@ int run_l2_long(mm_ctx *c, uint32_t *h_cnt)
 {
   const uint64_t nc = c->n_cands;
   if (c->n_long == 0 || nc == 0) return MM_OK;
-  int rc;
-  if ((rc = grow(c, c->d_l2_long_off, c->l2_long_off_cap, nc + 1))) return rc;
-  if ((rc = grow(c, c->d_long_scan_tmp, c->long_scan_tmp_cap, mm_l2_scan_tmp_bytes((uint32_t)nc) + 256))) return rc;
+  CU(c, c->d_l2_long_off.reserve(nc + 1));
+  CU(c, c->d_long_scan_tmp.reserve(mm_l2_scan_tmp_bytes((uint32_t)nc) + 256));
   mm_dev_batch b = make_batch(c);
-  CU(c, mm_launch_l2_long_ranges(c->params, c->ix, b, (uint32_t)nc, c->d_l2_long_off, c->d_long_scan_tmp, c->long_scan_tmp_cap,
-                                 c->stream));
+  CU(c, mm_launch_l2_long_ranges(c->params, c->ix, b, (uint32_t)nc, c->d_l2_long_off.get(), c->d_long_scan_tmp.get(),
+                                 c->d_long_scan_tmp.capacity(), c->stream));
   c->launches++;
   uint64_t words = 0;
-  RD(c, c->d_l2_long_off + nc, (uint32_t *)&words, 2);
+  RD(c, c->d_l2_long_off.get() + nc, (uint32_t *)&words, 2);
   if (words == 0) return MM_OK;
-  if ((rc = grow(c, c->d_long_table, c->long_table_cap, words))) return rc;
+  CU(c, c->d_long_table.reserve(words));
   for (int attempt = 0; attempt < 4; attempt++) {
     b = make_batch(c);
-    ZERO_WORDS(c, c->d_counters + 1, 1);
-    k_set_u32<<<1, 1, 0, c->stream>>>(c->d_counters + 6, (uint32_t)c->n_loci);
-    CU(c, mm_launch_l2_long(c->params, c->ix, b, (uint32_t)nc, c->d_l2_long_off, c->d_long_table, c->stream, c->sm_count));
+    ZERO_WORDS(c, c->d_counters.get() + 1, 1);
+    k_set_u32<<<1, 1, 0, c->stream>>>(c->d_counters.get() + 6, (uint32_t)c->n_loci);
+    CU(c, mm_launch_l2_long(c->params, c->ix, b, (uint32_t)nc, c->d_l2_long_off.get(), c->d_long_table.get(), c->stream,
+                            c->sm_count));
     c->launches += 2;
     CU(c, cudaEventRecord(c->ev[4], c->stream));
-    RD(c, c->d_counters, h_cnt, 16);
-    if (h_cnt[1] == 1 || h_cnt[6] > c->loci_cap) { /* a bigger locus buffer that keeps the loci already there, then again */
+    RD(c, c->d_counters.get(), h_cnt, 16);
+    if (h_cnt[1] == 1 || h_cnt[6] > c->d_loci.capacity()) { /* a bigger locus buffer that keeps the loci already there, then again */
       c->diag[MM_DIAG_L2_LOCI_REGROW]++;
-      const uint64_t cap = (uint64_t)h_cnt[6] + h_cnt[6] / 4 + 1024;
-      mm_l2_locus *p = nullptr;
-      CU(c, cudaMalloc((void **)&p, cap * sizeof(mm_l2_locus)));
-      if (c->n_loci) CU(c, cudaMemcpyAsync(p, c->d_loci, c->n_loci * sizeof(mm_l2_locus), cudaMemcpyDeviceToDevice, c->stream));
-      CU(c, cudaStreamSynchronize(c->stream));
-      cudaFree(c->d_loci);
-      c->d_loci = p; c->loci_cap = cap;
+      CU(c, c->d_loci.reserve_keep((uint64_t)h_cnt[6] + h_cnt[6] / 4 + 1024, c->n_loci, c->stream));
+      continue;
+    }
+    c->n_loci = h_cnt[6];
+    return MM_OK;
+  }
+  return fail(c, MM_ECUDA, "locus buffer kept overflowing");
+}
+
+/* K3 by the general kernel (mm_l2.cu), retried alone if the locus buffer is too small (it is idempotent) */
+int run_l2_general(mm_ctx *c, uint32_t *h_cnt)
+{
+  for (int attempt = 0; attempt < 4; attempt++) {
+    const mm_dev_batch b = make_batch(c);
+    ZERO_WORDS(c, c->d_counters.get() + 1, 1);
+    ZERO_WORDS(c, c->d_counters.get() + 6, 2);
+    CU(c, cudaEventRecord(c->ev[3], c->stream));
+    CU(c, mm_launch_l2(c->params, c->ix, b, (uint32_t)c->n_cands, c->stream, c->sm_count));
+    CU(c, cudaEventRecord(c->ev[4], c->stream));
+    if (c->n_cands) c->launches += 1;
+    RD(c, c->d_counters.get(), h_cnt, 16);
+    if (h_cnt[1] == 2) return fail(c, MM_ECUDA, "L2 live-set overflow: the reference index has more than "
+                                   "sketch_size+64 overlapping minmer windows at one position");
+    if (h_cnt[1] == 1 || h_cnt[6] > c->d_loci.capacity()) {
+      CU(c, c->d_loci.reserve((uint64_t)h_cnt[6] + h_cnt[6] / 4 + 1024));
       continue;
     }
     c->n_loci = h_cnt[6];
@@ -605,111 +659,61 @@ int run_pipeline(mm_ctx *c)
   int rc = check_ready(c);
   if (rc) return rc;
   CU(c, cudaSetDevice(c->device));
+  c->batch_mapped = false;
   const uint64_t n_segs = c->n_segs;
-  if (c->cand_cap < 2 * n_segs + 1024) {
-    if (c->d_cands) { cudaFree(c->d_cands); c->d_cands = nullptr; }
-    c->cand_cap = 2 * n_segs + 1024;
-    CU(c, cudaMalloc((void **)&c->d_cands, c->cand_cap * sizeof(mm_l1_candidate)));
-  }
-  if (c->loci_cap < 2 * c->cand_cap) {
-    if (c->d_loci) { cudaFree(c->d_loci); c->d_loci = nullptr; }
-    c->loci_cap = 2 * c->cand_cap;
-    CU(c, cudaMalloc((void **)&c->d_loci, c->loci_cap * sizeof(mm_l2_locus)));
-  }
+  CU(c, c->d_cands.reserve(2 * n_segs + 1024));
+  CU(c, c->d_loci.reserve(2 * c->d_cands.capacity()));
   uint64_t pool0 = 32ULL << 20; /* interval points the bump pool holds at first (grown on demand below) */
   if (const char *e = getenv("MM_L1_POOL_ELEMS")) pool0 = std::max<uint64_t>(1024, strtoull(e, nullptr, 10)); /* tests: force the regrow path */
-  if ((rc = ensure_scratch(c, c->scratch_cap ? c->scratch_cap - c->scratch_pool : pool0))) return rc;
-  if (c->l1_slow_cap < n_segs + 1) {
-    if (c->d_l1_slow) cudaFree(c->d_l1_slow);
-    c->d_l1_slow = nullptr;
-    c->l1_slow_cap = n_segs + n_segs / 8 + 1024;
-    CU(c, cudaMalloc((void **)&c->d_l1_slow, c->l1_slow_cap * 4));
-  }
+  if ((rc = ensure_scratch(c, c->d_scratch ? c->d_scratch.capacity() - c->scratch_pool : pool0))) return rc;
+  if (c->d_l1_slow.capacity() < n_segs + 1) CU(c, c->d_l1_slow.reserve(n_segs + n_segs / 8 + 1024));
 
   uint32_t h_cnt[16];
   for (int attempt = 0; attempt < 6; attempt++) {
     mm_dev_batch b = make_batch(c);
-    ZERO_WORDS(c, c->d_counters, 16);
+    ZERO_WORDS(c, c->d_counters.get(), 16);
     CU(c, cudaEventRecord(c->ev[0], c->stream));
     if ((rc = launch_pack_if_ascii(c))) return rc;
     CU(c, cudaEventRecord(c->ev_pack, c->stream));
     if ((rc = launch_sketch_all(c, true))) return rc;
     CU(c, cudaEventRecord(c->ev[1], c->stream));
     int l1_launches = 0;
-    CU(c, mm_launch_l1(c->params, c->ix, b, c->stream, c->sm_count, c->d_l1_slow, c->l1_warp, &l1_launches));
+    CU(c, mm_launch_l1(c->params, c->ix, b, c->stream, c->sm_count, c->d_l1_slow.get(), c->l1_warp, &l1_launches));
     if (c->n_long) { /* windowLen > 0: k_l1_long (mm_l1.cu), after the general path (it reuses its scratch slices) */
-      CU(c, mm_launch_l1_long(c->params, c->ix, b, c->d_long, c->n_long, c->stream, c->sm_count));
+      CU(c, mm_launch_l1_long(c->params, c->ix, b, c->d_long.get(), c->n_long, c->stream, c->sm_count));
       l1_launches++;
     }
     CU(c, cudaEventRecord(c->ev[2], c->stream));
     c->launches += (uint64_t)l1_launches;
-    RD(c, c->d_counters, h_cnt, 16);
+    RD(c, c->d_counters.get(), h_cnt, 16);
     const uint64_t need_cands = h_cnt[0];
     bool retry = false;
     c->diag[MM_DIAG_L1_CTA_SEGMENTS] += h_cnt[8];
     c->diag[MM_DIAG_SKETCH_GENERAL_SEGMENTS] += h_cnt[9];
-    if (h_cnt[3] || need_cands > c->cand_cap) {
+    if (h_cnt[3] || need_cands > c->d_cands.capacity()) {
       c->diag[MM_DIAG_CAND_REGROW]++;
-      cudaFree(c->d_cands); c->d_cands = nullptr;
-      c->cand_cap = need_cands + need_cands / 4 + 1024;
-      CU(c, cudaMalloc((void **)&c->d_cands, c->cand_cap * sizeof(mm_l1_candidate)));
+      CU(c, c->d_cands.reserve(need_cands + need_cands / 4 + 1024));
       retry = true;
     }
     if (h_cnt[2]) { /* scratch pool exhausted: quadruple it */
       c->diag[MM_DIAG_L1_POOL_REGROW]++;
-      const uint64_t pool = c->scratch_cap - c->scratch_pool;
-      cudaFree(c->d_scratch); c->d_scratch = nullptr; c->scratch_cap = 0;
-      if ((rc = ensure_scratch(c, pool * 4))) return rc;
+      if ((rc = ensure_scratch(c, (c->d_scratch.capacity() - c->scratch_pool) * 4))) return rc;
       retry = true;
     }
     if (retry) continue;
     c->n_cands = need_cands;
-    /* K3 */
-    if (c->l2_mode == 1) {
-      int rc2 = run_l2_stream(c, h_cnt);
-      if (rc2 == MM_OK && (rc2 = run_l2_long(c, h_cnt)) == MM_OK) {
-        if (c->batch_is_ascii) cudaEventElapsedTime(&c->pack_ms, c->ev[0], c->ev_pack);
-        cudaEventElapsedTime(&c->stage_ms[0], c->ev_pack, c->ev[1]);
-        cudaEventElapsedTime(&c->stage_ms[1], c->ev[1], c->ev[2]);
-        cudaEventElapsedTime(&c->stage_ms[2], c->ev[3], c->ev[4]);
-        cudaEventElapsedTime(&c->stage_ms[5], c->ev[0], c->ev[4]);
-        c->diag[MM_DIAG_LONG_FRAGMENTS] += c->n_long;
-        c->batch_mapped = true;
-        return MM_OK;
-      }
-      if (rc2 != MM_ENOMEM) return rc2;
-      /* not enough memory for the operation records: fall through to the general kernel */
-    }
-    /* general kernel, retried alone if the locus buffer is too small (it is idempotent) */
-    for (int a2 = 0; a2 < 4; a2++) {
-      b = make_batch(c);
-      ZERO_WORDS(c, c->d_counters + 1, 1);
-      ZERO_WORDS(c, c->d_counters + 6, 2);
-      CU(c, cudaEventRecord(c->ev[3], c->stream));
-      CU(c, mm_launch_l2(c->params, c->ix, b, (uint32_t)c->n_cands, c->stream, c->sm_count));
-      CU(c, cudaEventRecord(c->ev[4], c->stream));
-      if (c->n_cands) c->launches += 1;
-      RD(c, c->d_counters, h_cnt, 16);
-      if (h_cnt[1] == 2) return fail(c, MM_ECUDA, "L2 live-set overflow: the reference index has more than "
-                                     "sketch_size+64 overlapping minmer windows at one position");
-      if (h_cnt[1] == 1 || h_cnt[6] > c->loci_cap) {
-        cudaFree(c->d_loci); c->d_loci = nullptr;
-        c->loci_cap = (uint64_t)h_cnt[6] + h_cnt[6] / 4 + 1024;
-        CU(c, cudaMalloc((void **)&c->d_loci, c->loci_cap * sizeof(mm_l2_locus)));
-        continue;
-      }
-      c->n_loci = h_cnt[6];
-      if ((rc = run_l2_long(c, h_cnt))) return rc;
-      if (c->batch_is_ascii) cudaEventElapsedTime(&c->pack_ms, c->ev[0], c->ev_pack);
-      cudaEventElapsedTime(&c->stage_ms[0], c->ev_pack, c->ev[1]);
-      cudaEventElapsedTime(&c->stage_ms[1], c->ev[1], c->ev[2]);
-      cudaEventElapsedTime(&c->stage_ms[2], c->ev[3], c->ev[4]);
-      cudaEventElapsedTime(&c->stage_ms[5], c->ev[0], c->ev[4]); /* first launch -> last kernel end, incl. host gaps */
-      c->diag[MM_DIAG_LONG_FRAGMENTS] += c->n_long;
-      c->batch_mapped = true;
-      return MM_OK;
-    }
-    return fail(c, MM_ECUDA, "locus buffer kept overflowing");
+    /* K3: the stream kernels, or the general kernel where they are off or their own work areas do not fit */
+    rc = c->l2_mode == 1 ? run_l2_stream(c, h_cnt) : L2_STREAM_NO_ROOM;
+    if (rc == L2_STREAM_NO_ROOM) rc = run_l2_general(c, h_cnt);
+    if (rc || (rc = run_l2_long(c, h_cnt))) return rc;
+    if (c->batch_is_ascii) cudaEventElapsedTime(&c->pack_ms, c->ev[0], c->ev_pack);
+    cudaEventElapsedTime(&c->stage_ms[0], c->ev_pack, c->ev[1]);
+    cudaEventElapsedTime(&c->stage_ms[1], c->ev[1], c->ev[2]);
+    cudaEventElapsedTime(&c->stage_ms[2], c->ev[3], c->ev[4]);
+    cudaEventElapsedTime(&c->stage_ms[5], c->ev[0], c->ev[4]); /* first launch -> last kernel end, incl. host gaps */
+    c->diag[MM_DIAG_LONG_FRAGMENTS] += c->n_long;
+    c->batch_mapped = true;
+    return MM_OK;
   }
   return fail(c, MM_ECUDA, "candidate/scratch buffers kept overflowing");
 }
@@ -777,13 +781,6 @@ int mm_ctx_destroy(mm_ctx *c)
   if (!c) return MM_OK;
   cudaSetDevice(c->device);
   cudaStreamSynchronize(c->stream);
-  if (c->blob && c->blob_owned) cudaFree(c->blob);
-  mm_built_index_free(&c->built);
-  cudaFree(c->d_bases); cudaFree(c->d_packed); cudaFree(c->d_sk_reject); cudaFree(c->d_segs); cudaFree(c->d_sk_hash); cudaFree(c->d_sk_val); cudaFree(c->d_sk_pos); cudaFree(c->d_sk_strand);
-  cudaFree(c->d_seg_res); cudaFree(c->d_cands); cudaFree(c->d_loci); cudaFree(c->d_counters); cudaFree(c->d_scratch);
-  cudaFree(c->d_sk_votes); cudaFree(c->d_work_segs); cudaFree(c->d_long); cudaFree(c->d_long_off); cudaFree(c->d_long_tmp);
-  cudaFree(c->d_l2_long_off); cudaFree(c->d_long_scan_tmp); cudaFree(c->d_long_table);
-  cudaFree(c->d_l1_slow); cudaFree(c->d_l2_order); cudaFree(c->d_l2_ranges); cudaFree(c->d_l2_rec_off); cudaFree(c->d_l2_recs); cudaFree(c->d_scan_tmp);
   for (auto &ev : c->ev) cudaEventDestroy(ev);
   if (c->h_pub) cudaFreeHost(c->h_pub);
   if (c->ev_wait) cudaEventDestroy(c->ev_wait);
@@ -812,18 +809,8 @@ int mm_index_upload(mm_ctx *c, const mm_minmer *mi, uint64_t n_mi, const uint64_
   if (n_keys && (!keys || !offsets || !key_is_freq)) return fail(c, MM_EINVAL, "null lookup arrays");
   if (n_keys && offsets[n_keys] != n_points) return fail(c, MM_EINVAL, "offsets[n_keys] != n_points");
   CU(c, cudaSetDevice(c->device));
-  if (c->blob && c->blob_owned) { cudaFree(c->blob); }
-  c->blob = nullptr; c->blob_ready = false;
-  /* every early return below releases the temporaries (dev_tmp) and the half-built image (blob_guard) */
-  struct dev_tmp {
-    void *p = nullptr;
-    ~dev_tmp() { if (p) cudaFree(p); }
-  };
-  struct blob_guard {
-    mm_ctx *c;
-    bool done = false;
-    ~blob_guard() { if (!done && c->blob && c->blob_owned) { cudaFree(c->blob); c->blob = nullptr; c->blob_bytes = 0; c->blob_ready = false; } }
-  } guard{c};
+  drop_index(c);
+  image_guard guard{c};
 
   /* contig_start: first index entry of each contig; the index must be ordered by (seqId, wpos) */
   std::vector<uint64_t> cstart((size_t)n_contigs + 1, 0);
@@ -840,98 +827,45 @@ int mm_index_upload(mm_ctx *c, const mm_minmer *mi, uint64_t n_mi, const uint64_
     }
     for (int32_t s = 0; s < n_contigs; s++) cstart[(size_t)s + 1] += cstart[(size_t)s];
   }
-  int tab_log2 = 4;
-  while ((1ULL << tab_log2) < 2 * n_keys + 2) tab_log2++;
-  const uint64_t tab_slots = 1ULL << tab_log2;
+  int rc = begin_image(c, n_mi, n_keys, n_points, n_contigs);
+  if (rc) return rc;
+  const mm_blob_header &h = c->hdr;
+  mm_devbuf<uint32_t> d_err;
+  CU(c, d_err.reserve(1));
+  CU(c, cudaMemsetAsync(d_err.get(), 0, 4, c->stream));
 
-  mm_blob_header h{};
-  h.magic = MM_BLOB_MAGIC;
-  h.n_minmers = n_mi; h.n_keys = n_keys; h.n_points = n_points;
-  h.n_contigs = n_contigs; h.tab_log2 = tab_log2;
-  uint64_t o = align_up(sizeof(mm_blob_header), 256);
-  auto place = [&](uint64_t bytes) { uint64_t at = o; o = align_up(o + bytes, 256); return at; };
-  h.off_idx_hash = place((n_mi + 1) * 8);
-  h.off_idx_wpos = place((n_mi + 1) * 4);
-  h.off_idx_wend = place((n_mi + 1) * 4);
-  h.off_idx_strand = place(n_mi + 1);
-  h.off_contig_start = place(((uint64_t)n_contigs + 1) * 8);
-  h.off_idx2_hash = place((n_mi + 1) * 8);
-  h.off_idx2_wend = place((n_mi + 1) * 4);
-  h.off_tab = place(tab_slots * sizeof(mm_tab_slot));
-  h.off_pts = place((n_points + 1) * 8);
-  h.off_contig_len = place((uint64_t)n_contigs * 4);
-  h.off_contig_name_id = place((uint64_t)n_contigs * 4);
-  h.off_contig_group = place((uint64_t)n_contigs * 4);
-  h.off_cutoffs = place(TABLE_REGION_BYTES);
-  h.off_min_hits = place(TABLE_REGION_BYTES);
-  h.total_bytes = o;
-  CU(c, cudaMalloc((void **)&c->blob, o));
-  c->blob_bytes = o; c->blob_owned = true; c->hdr = h; c->share_src = nullptr;
-
-  /* AoS records go up in chunks and are re-laid out on the device (SoA index, packed points, hash table) */
+  /* AoS records go up in chunks and are re-laid out on the device (SoA index, packed points) */
   {
     const uint64_t CH = 1ULL << 24;
-    dev_tmp stage_buf;
-    CU(c, cudaMalloc(&stage_buf.p, CH * 24));
-    void *stage = stage_buf.p;
+    mm_devbuf<unsigned char> stage;
+    CU(c, stage.reserve(CH * 24));
     for (uint64_t at = 0; at < n_mi; at += CH) {
       const uint64_t n = std::min(CH, n_mi - at);
-      CU(c, cudaMemcpyAsync(stage, mi + at, n * sizeof(mm_minmer), cudaMemcpyHostToDevice, c->stream));
-      CU(c, mm_upload_split_minmers((const mm_minmer *)stage, n, (uint64_t *)(c->blob + h.off_idx_hash) + at,
+      CU(c, cudaMemcpyAsync(stage.get(), mi + at, n * sizeof(mm_minmer), cudaMemcpyHostToDevice, c->stream));
+      CU(c, mm_upload_split_minmers((const mm_minmer *)stage.get(), n, (uint64_t *)(c->blob + h.off_idx_hash) + at,
                                     (int32_t *)(c->blob + h.off_idx_wpos) + at, (int32_t *)(c->blob + h.off_idx_wend) + at,
                                     (int8_t *)(c->blob + h.off_idx_strand) + at, c->stream));
       CU(c, cudaStreamSynchronize(c->stream));
     }
-    CU(c, cudaMemcpyAsync(c->blob + h.off_contig_start, cstart.data(), cstart.size() * 8, cudaMemcpyHostToDevice, c->stream));
-    /* the same entries per contig in wpos_end order (device sort), for the L2 stream merge */
-    CU(c, mm_build_death_order((const uint64_t *)(c->blob + h.off_idx_hash), (const int32_t *)(c->blob + h.off_idx_wend),
-                               (const uint64_t *)(c->blob + h.off_contig_start), n_contigs, n_mi,
-                               (uint64_t *)(c->blob + h.off_idx2_hash), (int32_t *)(c->blob + h.off_idx2_wend), c->stream));
-    dev_tmp err_buf;
-    CU(c, cudaMalloc(&err_buf.p, 4));
-    uint32_t *d_err = (uint32_t *)err_buf.p;
-    CU(c, cudaMemsetAsync(d_err, 0, 4, c->stream));
     for (uint64_t at = 0; at < n_points; at += CH) {
       const uint64_t n = std::min(CH, n_points - at);
-      CU(c, cudaMemcpyAsync(stage, points + at, n * sizeof(mm_ipoint), cudaMemcpyHostToDevice, c->stream));
-      CU(c, mm_upload_pack_points((const mm_ipoint *)stage, n, n_contigs, (uint64_t *)(c->blob + h.off_pts) + at, d_err, c->stream));
+      CU(c, cudaMemcpyAsync(stage.get(), points + at, n * sizeof(mm_ipoint), cudaMemcpyHostToDevice, c->stream));
+      CU(c, mm_upload_pack_points((const mm_ipoint *)stage.get(), n, n_contigs, (uint64_t *)(c->blob + h.off_pts) + at,
+                                  d_err.get(), c->stream));
       CU(c, cudaStreamSynchronize(c->stream));
     }
-    cudaFree(stage_buf.p); stage_buf.p = nullptr;
-    /* open-addressing table, filled on the device */
-    CU(c, cudaMemsetAsync(c->blob + h.off_tab, 0, tab_slots * sizeof(mm_tab_slot), c->stream));
-    if (n_keys) {
-      dev_tmp keys_buf, offs_buf, freq_buf;
-      CU(c, cudaMalloc(&keys_buf.p, n_keys * 8));
-      CU(c, cudaMalloc(&offs_buf.p, (n_keys + 1) * 8));
-      CU(c, cudaMalloc(&freq_buf.p, n_keys));
-      uint64_t *d_keys = (uint64_t *)keys_buf.p, *d_offs = (uint64_t *)offs_buf.p;
-      uint8_t *d_freq = (uint8_t *)freq_buf.p;
-      CU(c, cudaMemcpyAsync(d_keys, keys, n_keys * 8, cudaMemcpyHostToDevice, c->stream));
-      CU(c, cudaMemcpyAsync(d_offs, offsets, (n_keys + 1) * 8, cudaMemcpyHostToDevice, c->stream));
-      CU(c, cudaMemcpyAsync(d_freq, key_is_freq, n_keys, cudaMemcpyHostToDevice, c->stream));
-      CU(c, mm_upload_build_table(d_keys, d_offs, d_freq, n_keys, (mm_tab_slot *)(c->blob + h.off_tab), tab_log2, d_err, c->stream));
-      CU(c, cudaStreamSynchronize(c->stream));
-    }
-    uint32_t err = 0;
-    CU(c, cudaMemcpyAsync(&err, d_err, 4, cudaMemcpyDeviceToHost, c->stream));
-    CU(c, cudaStreamSynchronize(c->stream));
-    if (err & 1) return fail(c, MM_EINVAL, "an interval point has a bad seqId or a negative position");
-    if (err & 2) return fail(c, MM_EINVAL, "a key has no or too many (>= 2^24) interval points, or offsets overflow");
-    if (err & 4) return fail(c, MM_EINVAL, "duplicate key in the lookup index");
   }
-  CU(c, cudaMemcpyAsync(c->blob + h.off_contig_len, contig_len, (size_t)n_contigs * 4, cudaMemcpyHostToDevice, c->stream));
-  std::vector<int32_t> tmp((size_t)n_contigs, -1);
-  CU(c, cudaMemcpyAsync(c->blob + h.off_contig_name_id, contig_name_id ? contig_name_id : tmp.data(), (size_t)n_contigs * 4, cudaMemcpyHostToDevice, c->stream));
-  CU(c, cudaStreamSynchronize(c->stream)); /* tmp is rewritten below */
-  std::fill(tmp.begin(), tmp.end(), 0);
-  CU(c, cudaMemcpyAsync(c->blob + h.off_contig_group, contig_group ? contig_group : tmp.data(), (size_t)n_contigs * 4, cudaMemcpyHostToDevice, c->stream));
-  CU(c, cudaMemcpyAsync(c->blob, &c->hdr, sizeof(c->hdr), cudaMemcpyHostToDevice, c->stream));
-  CU(c, cudaStreamSynchronize(c->stream));
-  resolve_index(c);
-  c->blob_ready = true;
-  guard.done = true;
-  return write_tables(c);
+  mm_devbuf<uint64_t> d_keys, d_offs;
+  mm_devbuf<uint8_t> d_freq;
+  if (n_keys) {
+    CU(c, d_keys.reserve(n_keys));
+    CU(c, d_offs.reserve(n_keys + 1));
+    CU(c, d_freq.reserve(n_keys));
+    CU(c, cudaMemcpyAsync(d_keys.get(), keys, n_keys * 8, cudaMemcpyHostToDevice, c->stream));
+    CU(c, cudaMemcpyAsync(d_offs.get(), offsets, (n_keys + 1) * 8, cudaMemcpyHostToDevice, c->stream));
+    CU(c, cudaMemcpyAsync(d_freq.get(), key_is_freq, n_keys, cudaMemcpyHostToDevice, c->stream));
+  }
+  return finish_image(c, cstart, d_keys.get(), d_offs.get(), d_freq.get(), d_err.get(), contig_len, contig_name_id, contig_group);
 }
 
 int mm_tables_upload(mm_ctx *c, const int32_t *cut, int32_t n_cut, const int32_t *mh, int32_t n_mh)
@@ -955,10 +889,9 @@ int mm_index_blob_alloc(mm_ctx *c, uint64_t n_bytes, void **blob)
 {
   if (!c || !blob || n_bytes < sizeof(mm_blob_header)) return MM_EINVAL;
   CU(c, cudaSetDevice(c->device));
-  if (c->blob && c->blob_owned) cudaFree(c->blob);
-  c->blob = nullptr; c->blob_ready = false;
-  CU(c, cudaMalloc((void **)&c->blob, n_bytes));
-  c->blob_bytes = n_bytes; c->blob_owned = true; c->share_src = nullptr;
+  drop_index(c);
+  CU(c, c->own_blob.reserve(n_bytes));
+  c->blob = c->own_blob.get(); c->blob_bytes = n_bytes;
   *blob = c->blob;
   return MM_OK;
 }
@@ -980,8 +913,9 @@ int mm_ctx_share_index(mm_ctx *c, const mm_ctx *src)
   if (!c || !src) return MM_EINVAL;
   if (!src->blob_ready) return fail(c, MM_ESTATE, "source context has no index");
   if (c->device != src->device) return fail(c, MM_EINVAL, "contexts are on different devices");
-  if (c->blob && c->blob_owned) { cudaSetDevice(c->device); cudaFree(c->blob); }
-  c->blob = src->blob; c->blob_bytes = src->blob_bytes; c->blob_owned = false;
+  cudaSetDevice(c->device);
+  drop_index(c);
+  c->blob = src->blob; c->blob_bytes = src->blob_bytes;
   c->hdr = src->hdr;
   c->cutoffs = src->cutoffs; c->min_hits = src->min_hits;
   c->share_src = src;
@@ -1025,9 +959,9 @@ int mm_batch_fetch(mm_ctx *c, mm_segment_result *seg_results, mm_l1_candidate *c
   if (cand_cap < c->n_cands || loci_cap < c->n_loci) return fail(c, MM_ECAPACITY, "output capacity too small");
   CU(c, cudaSetDevice(c->device));
   CU(c, cudaEventRecord(c->ev[5], c->stream));
-  if (seg_results) CU(c, cudaMemcpyAsync(seg_results, c->d_seg_res, c->n_segs * sizeof(mm_segment_result), cudaMemcpyDeviceToHost, c->stream));
-  if (cands && c->n_cands) CU(c, cudaMemcpyAsync(cands, c->d_cands, c->n_cands * sizeof(mm_l1_candidate), cudaMemcpyDeviceToHost, c->stream));
-  if (loci && c->n_loci) CU(c, cudaMemcpyAsync(loci, c->d_loci, c->n_loci * sizeof(mm_l2_locus), cudaMemcpyDeviceToHost, c->stream));
+  if (seg_results) CU(c, cudaMemcpyAsync(seg_results, c->d_seg_res.get(), c->n_segs * sizeof(mm_segment_result), cudaMemcpyDeviceToHost, c->stream));
+  if (cands && c->n_cands) CU(c, cudaMemcpyAsync(cands, c->d_cands.get(), c->n_cands * sizeof(mm_l1_candidate), cudaMemcpyDeviceToHost, c->stream));
+  if (loci && c->n_loci) CU(c, cudaMemcpyAsync(loci, c->d_loci.get(), c->n_loci * sizeof(mm_l2_locus), cudaMemcpyDeviceToHost, c->stream));
   CU(c, cudaEventRecord(c->ev[6], c->stream));
   CU(c, wait_stream(c));
   cudaEventElapsedTime(&c->stage_ms[4], c->ev[5], c->ev[6]);
@@ -1044,11 +978,11 @@ int mm_batch_fetch_sketch(mm_ctx *c, mm_minmer *out, int32_t *out_count)
   std::vector<int8_t> ss(n);
   std::vector<mm_segment_result> sr(c->n_segs);
   std::vector<mm_segment> sg(c->n_segs);
-  CU(c, cudaMemcpyAsync(hh.data(), c->d_sk_hash, n * 8, cudaMemcpyDeviceToHost, c->stream));
-  CU(c, cudaMemcpyAsync(pp.data(), c->d_sk_pos, n * 8, cudaMemcpyDeviceToHost, c->stream));
-  CU(c, cudaMemcpyAsync(ss.data(), c->d_sk_strand, n, cudaMemcpyDeviceToHost, c->stream));
-  CU(c, cudaMemcpyAsync(sr.data(), c->d_seg_res, c->n_segs * sizeof(mm_segment_result), cudaMemcpyDeviceToHost, c->stream));
-  CU(c, cudaMemcpyAsync(sg.data(), c->d_segs, c->n_segs * sizeof(mm_segment), cudaMemcpyDeviceToHost, c->stream));
+  CU(c, cudaMemcpyAsync(hh.data(), c->d_sk_hash.get(), n * 8, cudaMemcpyDeviceToHost, c->stream));
+  CU(c, cudaMemcpyAsync(pp.data(), c->d_sk_pos.get(), n * 8, cudaMemcpyDeviceToHost, c->stream));
+  CU(c, cudaMemcpyAsync(ss.data(), c->d_sk_strand.get(), n, cudaMemcpyDeviceToHost, c->stream));
+  CU(c, cudaMemcpyAsync(sr.data(), c->d_seg_res.get(), c->n_segs * sizeof(mm_segment_result), cudaMemcpyDeviceToHost, c->stream));
+  CU(c, cudaMemcpyAsync(sg.data(), c->d_segs.get(), c->n_segs * sizeof(mm_segment), cudaMemcpyDeviceToHost, c->stream));
   CU(c, cudaStreamSynchronize(c->stream));
   for (uint64_t s = 0; s < c->n_segs; s++) {
     out_count[s] = sr[s].sketch_size;
@@ -1068,7 +1002,7 @@ int mm_sketch_segments(mm_ctx *c, const char *bases, uint64_t n_bases, const mm_
   int rc = upload_batch(c, bases, n_bases, segs, n_segs, 0);
   if (rc) return rc;
   if ((rc = launch_pack_if_ascii(c))) return rc;
-  ZERO_WORDS(c, c->d_counters, 16);
+  ZERO_WORDS(c, c->d_counters.get(), 16);
   CU(c, cudaEventRecord(c->ev[0], c->stream));
   if ((rc = launch_sketch_all(c, false))) return rc; /* sketches only: no index needed */
   CU(c, cudaEventRecord(c->ev[1], c->stream));
@@ -1076,7 +1010,7 @@ int mm_sketch_segments(mm_ctx *c, const char *bases, uint64_t n_bases, const mm_
   cudaEventElapsedTime(&c->stage_ms[0], c->ev[0], c->ev[1]);
   {
     uint32_t h9 = 0;
-    if (cudaMemcpy(&h9, c->d_counters + 9, 4, cudaMemcpyDeviceToHost) == cudaSuccess) c->diag[MM_DIAG_SKETCH_GENERAL_SEGMENTS] += h9;
+    if (cudaMemcpy(&h9, c->d_counters.get() + 9, 4, cudaMemcpyDeviceToHost) == cudaSuccess) c->diag[MM_DIAG_SKETCH_GENERAL_SEGMENTS] += h9;
   }
   c->diag[MM_DIAG_LONG_FRAGMENTS] += c->n_long;
   c->batch_mapped = true; /* sketches only; fetch_sketch reads sketch_size == raw count */
@@ -1154,30 +1088,6 @@ int mm_host_alloc(void **ptr, uint64_t bytes)
 }
 int mm_host_free(void *ptr) { return cudaFreeHost(ptr) == cudaSuccess ? MM_OK : MM_ECUDA; }
 
-} // extern "C"
-
-namespace {
-__global__ void k_count_seq(uint64_t n, const int32_t *__restrict__ seq, unsigned long long *cnt)
-{
-  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) atomicAdd(&cnt[seq[i]], 1ULL);
-}
-__global__ void k_unpack_points(uint64_t n, const uint64_t *__restrict__ pts, const uint64_t *__restrict__ keys, const uint64_t *__restrict__ offs,
-                                uint64_t n_keys, mm_ipoint *out)
-{ /* packed point -> skch::IntervalPoint (the hash comes from the key whose list the point is in) */
-  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  uint64_t lo = 0, hi = n_keys; /* last key with offs <= i */
-  while (lo + 1 < hi) { const uint64_t mid = (lo + hi) >> 1; if (offs[mid] <= i) lo = mid; else hi = mid; }
-  mm_ipoint p;
-  memset(&p, 0, sizeof p);
-  p.pos = mm_point_pos(pts[i]); p.hash = keys[lo]; p.seqId = mm_point_seq(pts[i]); p.side = mm_point_open(pts[i]) ? 1 : -1;
-  out[i] = p;
-}
-} // namespace
-
-extern "C" {
-
 /* skch::Sketch's build + index + computeFreqHist + dropFreqSeedSet on the device (mm_index_build.cu) */
 int mm_index_build(mm_ctx *c, const char *seqs, int seqs_on_device, const uint64_t *contig_offsets, int32_t n_contigs,
                    const int32_t *contig_name_id, const int32_t *contig_group, float kmer_pct_threshold, int keep_lookup,
@@ -1187,103 +1097,56 @@ int mm_index_build(mm_ctx *c, const char *seqs, int seqs_on_device, const uint64
   if (n_contigs < 1 || !contig_offsets || !seqs) return fail(c, MM_EINVAL, "no contigs");
   CU(c, cudaSetDevice(c->device));
   const auto t0 = std::chrono::steady_clock::now();
-  if (c->blob && c->blob_owned) { cudaFree(c->blob); }
-  c->blob = nullptr; c->blob_ready = false;
-  mm_built_index_free(&c->built);
+  drop_index(c);
+  image_guard guard{c};
+  c->built = mm_built_index{};
   c->built_kept = false;
   const uint64_t total = contig_offsets[n_contigs];
-  uint8_t *d_seq = (uint8_t *)seqs;
-  uint8_t *staged = nullptr;
+  mm_devbuf<uint8_t> staged;
   if (!seqs_on_device) {
-    CU(c, cudaMalloc((void **)&staged, total + 64));
-    CU(c, cudaMemcpyAsync(staged, seqs, total, cudaMemcpyHostToDevice, c->stream));
-    d_seq = staged;
+    CU(c, staged.reserve(total + 64));
+    CU(c, cudaMemcpyAsync(staged.get(), seqs, total, cudaMemcpyHostToDevice, c->stream));
   }
   mm_built_index B;
   std::string err;
-  int rc = mm_build_index_device(c->params, d_seq, contig_offsets, n_contigs, kmer_pct_threshold, c->stream, c->sm_count, &B, err);
-  if (staged) cudaFree(staged);
-  if (rc != MM_OK) { mm_built_index_free(&B); return fail(c, rc, "index build: %s", err.c_str()); }
+  int rc = mm_build_index_device(c->params, seqs_on_device ? (const uint8_t *)seqs : staged.get(), contig_offsets, n_contigs,
+                                 kmer_pct_threshold, c->stream, c->sm_count, &B, err);
+  staged.reset();
+  if (rc != MM_OK) return fail(c, rc, "index build: %s", err.c_str());
   c->launches += 12;
 
   const uint64_t n_mi = B.n_minmers, n_keys = B.n_keys, n_points = B.n_points;
-  if (n_mi >= (1ULL << 32)) { mm_built_index_free(&B); return fail(c, MM_EINVAL, "more than 2^32 minmers"); }
+  if (n_mi >= (1ULL << 32)) return fail(c, MM_EINVAL, "more than 2^32 minmers");
   /* contig_start from the seqId column */
   std::vector<uint64_t> cstart((size_t)n_contigs + 1, 0);
   if (n_mi) {
-    unsigned long long *d_cnt = nullptr;
-    CU(c, cudaMalloc((void **)&d_cnt, ((size_t)n_contigs + 1) * 8));
-    CU(c, cudaMemsetAsync(d_cnt, 0, ((size_t)n_contigs + 1) * 8, c->stream));
-    k_count_seq<<<(uint32_t)((n_mi + 255) / 256), 256, 0, c->stream>>>(n_mi, B.seq, d_cnt);
+    mm_devbuf<unsigned long long> d_cnt;
+    CU(c, d_cnt.reserve((size_t)n_contigs + 1));
+    CU(c, cudaMemsetAsync(d_cnt.get(), 0, ((size_t)n_contigs + 1) * 8, c->stream));
+    CU(c, mm_index_count_seq(n_mi, B.seq.get(), d_cnt.get(), c->stream));
     std::vector<unsigned long long> cnt((size_t)n_contigs + 1);
-    CU(c, cudaMemcpyAsync(cnt.data(), d_cnt, ((size_t)n_contigs + 1) * 8, cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaMemcpyAsync(cnt.data(), d_cnt.get(), ((size_t)n_contigs + 1) * 8, cudaMemcpyDeviceToHost, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
-    cudaFree(d_cnt);
     for (int32_t q = 0; q < n_contigs; q++) cstart[(size_t)q + 1] = cstart[(size_t)q] + cnt[(size_t)q];
   }
-  int tab_log2 = 4;
-  while ((1ULL << tab_log2) < 2 * n_keys + 2) tab_log2++;
-  const uint64_t tab_slots = 1ULL << tab_log2;
-  mm_blob_header h{};
-  h.magic = MM_BLOB_MAGIC;
-  h.n_minmers = n_mi; h.n_keys = n_keys; h.n_points = n_points;
-  h.n_contigs = n_contigs; h.tab_log2 = tab_log2;
-  uint64_t o = align_up(sizeof(mm_blob_header), 256);
-  auto place = [&](uint64_t bytes) { uint64_t at = o; o = align_up(o + bytes, 256); return at; };
-  h.off_idx_hash = place((n_mi + 1) * 8);
-  h.off_idx_wpos = place((n_mi + 1) * 4);
-  h.off_idx_wend = place((n_mi + 1) * 4);
-  h.off_idx_strand = place(n_mi + 1);
-  h.off_contig_start = place(((uint64_t)n_contigs + 1) * 8);
-  h.off_idx2_hash = place((n_mi + 1) * 8);
-  h.off_idx2_wend = place((n_mi + 1) * 4);
-  h.off_tab = place(tab_slots * sizeof(mm_tab_slot));
-  h.off_pts = place((n_points + 1) * 8);
-  h.off_contig_len = place((uint64_t)n_contigs * 4);
-  h.off_contig_name_id = place((uint64_t)n_contigs * 4);
-  h.off_contig_group = place((uint64_t)n_contigs * 4);
-  h.off_cutoffs = place(TABLE_REGION_BYTES);
-  h.off_min_hits = place(TABLE_REGION_BYTES);
-  h.total_bytes = o;
-  if (cudaMalloc((void **)&c->blob, o) != cudaSuccess) { cudaGetLastError(); mm_built_index_free(&B); return fail(c, MM_ENOMEM, "cannot allocate the index image (%llu bytes)", (unsigned long long)o); }
-  c->blob_bytes = o; c->blob_owned = true; c->hdr = h; c->share_src = nullptr;
+  if ((rc = begin_image(c, n_mi, n_keys, n_points, n_contigs))) return rc;
+  const mm_blob_header &h = c->hdr;
   if (n_mi) {
-    CU(c, cudaMemcpyAsync(c->blob + h.off_idx_hash, B.hash, n_mi * 8, cudaMemcpyDeviceToDevice, c->stream));
-    CU(c, cudaMemcpyAsync(c->blob + h.off_idx_wpos, B.wpos, n_mi * 4, cudaMemcpyDeviceToDevice, c->stream));
-    CU(c, cudaMemcpyAsync(c->blob + h.off_idx_wend, B.wend, n_mi * 4, cudaMemcpyDeviceToDevice, c->stream));
-    CU(c, cudaMemcpyAsync(c->blob + h.off_idx_strand, B.strand, n_mi, cudaMemcpyDeviceToDevice, c->stream));
+    CU(c, cudaMemcpyAsync(c->blob + h.off_idx_hash, B.hash.get(), n_mi * 8, cudaMemcpyDeviceToDevice, c->stream));
+    CU(c, cudaMemcpyAsync(c->blob + h.off_idx_wpos, B.wpos.get(), n_mi * 4, cudaMemcpyDeviceToDevice, c->stream));
+    CU(c, cudaMemcpyAsync(c->blob + h.off_idx_wend, B.wend.get(), n_mi * 4, cudaMemcpyDeviceToDevice, c->stream));
+    CU(c, cudaMemcpyAsync(c->blob + h.off_idx_strand, B.strand.get(), n_mi, cudaMemcpyDeviceToDevice, c->stream));
   }
-  CU(c, cudaMemcpyAsync(c->blob + h.off_contig_start, cstart.data(), cstart.size() * 8, cudaMemcpyHostToDevice, c->stream));
+  if (n_points) CU(c, cudaMemcpyAsync(c->blob + h.off_pts, B.pts.get(), n_points * 8, cudaMemcpyDeviceToDevice, c->stream));
   CU(c, cudaStreamSynchronize(c->stream));
-  cudaFree(B.hash); cudaFree(B.wpos); cudaFree(B.wend); cudaFree(B.seq); cudaFree(B.strand);
-  B.hash = nullptr; B.wpos = nullptr; B.wend = nullptr; B.seq = nullptr; B.strand = nullptr;
-  CU(c, mm_build_death_order((const uint64_t *)(c->blob + h.off_idx_hash), (const int32_t *)(c->blob + h.off_idx_wend),
-                             (const uint64_t *)(c->blob + h.off_contig_start), n_contigs, n_mi,
-                             (uint64_t *)(c->blob + h.off_idx2_hash), (int32_t *)(c->blob + h.off_idx2_wend), c->stream));
-  if (n_points) CU(c, cudaMemcpyAsync(c->blob + h.off_pts, B.pts, n_points * 8, cudaMemcpyDeviceToDevice, c->stream));
-  CU(c, cudaMemsetAsync(c->blob + h.off_tab, 0, tab_slots * sizeof(mm_tab_slot), c->stream));
-  if (n_keys) {
-    uint32_t *d_err = nullptr;
-    CU(c, cudaMalloc((void **)&d_err, 4));
-    CU(c, cudaMemsetAsync(d_err, 0, 4, c->stream));
-    CU(c, mm_upload_build_table(B.keys, B.offs, B.is_freq, n_keys, (mm_tab_slot *)(c->blob + h.off_tab), tab_log2, d_err, c->stream));
-    uint32_t e = 0;
-    CU(c, cudaMemcpyAsync(&e, d_err, 4, cudaMemcpyDeviceToHost, c->stream));
-    CU(c, cudaStreamSynchronize(c->stream));
-    cudaFree(d_err);
-    if (e) { mm_built_index_free(&B); return fail(c, MM_EINVAL, "lookup table build failed (code %u)", e); }
-  }
-  std::vector<int32_t> clen((size_t)n_contigs), tmp((size_t)n_contigs, -1);
+  B.hash.reset(); B.wpos.reset(); B.wend.reset(); B.seq.reset(); B.strand.reset(); /* before the death order's sort */
+  mm_devbuf<uint32_t> d_err;
+  CU(c, d_err.reserve(1));
+  CU(c, cudaMemsetAsync(d_err.get(), 0, 4, c->stream));
+  std::vector<int32_t> clen((size_t)n_contigs);
   for (int32_t q = 0; q < n_contigs; q++) clen[(size_t)q] = (int32_t)(contig_offsets[q + 1] - contig_offsets[q]);
-  CU(c, cudaMemcpyAsync(c->blob + h.off_contig_len, clen.data(), (size_t)n_contigs * 4, cudaMemcpyHostToDevice, c->stream));
-  CU(c, cudaMemcpyAsync(c->blob + h.off_contig_name_id, contig_name_id ? contig_name_id : tmp.data(), (size_t)n_contigs * 4, cudaMemcpyHostToDevice, c->stream));
-  CU(c, cudaStreamSynchronize(c->stream));
-  std::fill(tmp.begin(), tmp.end(), 0);
-  CU(c, cudaMemcpyAsync(c->blob + h.off_contig_group, contig_group ? contig_group : tmp.data(), (size_t)n_contigs * 4, cudaMemcpyHostToDevice, c->stream));
-  CU(c, cudaMemcpyAsync(c->blob, &c->hdr, sizeof(c->hdr), cudaMemcpyHostToDevice, c->stream));
-  CU(c, cudaStreamSynchronize(c->stream));
-  resolve_index(c);
-  c->blob_ready = true;
+  rc = finish_image(c, cstart, B.keys.get(), B.offs.get(), B.is_freq.get(), d_err.get(), clen.data(), contig_name_id, contig_group);
+  if (!c->blob_ready) return rc; /* else rc is write_tables': the index stands either way */
   if (stats) {
     memset(stats, 0, sizeof *stats);
     stats->n_minmers = n_mi; stats->n_minmers_before_filter = B.n_minmers_before_filter; stats->n_keys = n_keys; stats->n_points = n_points;
@@ -1292,9 +1155,8 @@ int mm_index_build(mm_ctx *c, const char *seqs, int seqs_on_device, const uint64
     stats->hist_max_keys = B.hist_max_keys; stats->ms_scan = B.ms_scan; stats->ms_post = B.ms_post; stats->ms_lookup = B.ms_lookup;
     stats->ms_total = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
   }
-  if (keep_lookup) { c->built = B; c->built_kept = true; }
-  else mm_built_index_free(&B);
-  return write_tables(c);
+  if (keep_lookup) { c->built = std::move(B); c->built_kept = true; }
+  return rc;
 }
 
 /* host copies of what mm_index_build left on the device (needs keep_lookup); any output may be NULL */
@@ -1321,16 +1183,16 @@ int mm_index_download(mm_ctx *c, mm_minmer *mi, uint64_t *keys, uint64_t *offset
     }
   }
   const mm_built_index &B = c->built;
-  if (keys && B.n_keys) CU(c, cudaMemcpy(keys, B.keys, B.n_keys * 8, cudaMemcpyDeviceToHost));
-  if (offsets) CU(c, cudaMemcpy(offsets, B.offs, (B.n_keys + 1) * 8, cudaMemcpyDeviceToHost));
-  if (is_freq && B.n_keys) CU(c, cudaMemcpy(is_freq, B.is_freq, B.n_keys, cudaMemcpyDeviceToHost));
+  if (keys && B.n_keys) CU(c, cudaMemcpy(keys, B.keys.get(), B.n_keys * 8, cudaMemcpyDeviceToHost));
+  if (offsets) CU(c, cudaMemcpy(offsets, B.offs.get(), (B.n_keys + 1) * 8, cudaMemcpyDeviceToHost));
+  if (is_freq && B.n_keys) CU(c, cudaMemcpy(is_freq, B.is_freq.get(), B.n_keys, cudaMemcpyDeviceToHost));
   if (points && B.n_points) {
-    mm_ipoint *d = nullptr;
-    CU(c, cudaMalloc((void **)&d, B.n_points * sizeof(mm_ipoint)));
-    k_unpack_points<<<(uint32_t)((B.n_points + 255) / 256), 256, 0, c->stream>>>(B.n_points, (const uint64_t *)(c->blob + h.off_pts), B.keys, B.offs, B.n_keys, d);
-    CU(c, cudaMemcpyAsync(points, d, B.n_points * sizeof(mm_ipoint), cudaMemcpyDeviceToHost, c->stream));
+    mm_devbuf<mm_ipoint> d;
+    CU(c, d.reserve(B.n_points));
+    CU(c, mm_index_unpack_points(B.n_points, (const uint64_t *)(c->blob + h.off_pts), B.keys.get(), B.offs.get(), B.n_keys, d.get(),
+                                 c->stream));
+    CU(c, cudaMemcpyAsync(points, d.get(), B.n_points * sizeof(mm_ipoint), cudaMemcpyDeviceToHost, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
-    cudaFree(d);
   }
   return MM_OK;
 }

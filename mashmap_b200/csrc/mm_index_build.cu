@@ -465,19 +465,101 @@ void launch_fix(const uint8_t *seq, const uint64_t *off, const wb_chunk *chunks,
   k_window_fix<K><<<(n_chains + 63) / 64, 64, 0, st>>>(seq, off, chunks, chains, n_chains, w, s, warm, slabs, L, fix, fix_cap, outs, ex, stride);
 }
 
+/* ---- the index image (mm_capi.cu writes it from these) ---- */
+__global__ void k_fill_death_keys(const int32_t *idx_wend, const uint64_t *contig_start, int32_t n_contigs, uint64_t n,
+                                  uint64_t *keys, uint32_t *vals)
+{
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  int lo = 0, hi = n_contigs; /* contig of entry i: last c with contig_start[c] <= i */
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (contig_start[mid] <= i) lo = mid; else hi = mid;
+  }
+  keys[i] = ((uint64_t)(uint32_t)lo << 32) | (uint64_t)(uint32_t)idx_wend[i];
+  vals[i] = (uint32_t)i;
+}
+__global__ void k_gather_death(const uint64_t *idx_hash, const uint64_t *keys_sorted, const uint32_t *vals_sorted, uint64_t n,
+                               uint64_t *idx2_hash, int32_t *idx2_wend)
+{
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  idx2_hash[i] = idx_hash[vals_sorted[i]];
+  idx2_wend[i] = (int32_t)(uint32_t)keys_sorted[i];
+}
+
+__global__ void k_split_minmers(const mm_minmer *aos, uint64_t n, uint64_t *hash, int32_t *wpos, int32_t *wend, int8_t *strand)
+{
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const mm_minmer m = aos[i];
+  hash[i] = m.hash; wpos[i] = m.wpos; wend[i] = m.wpos_end; strand[i] = (int8_t)m.strand;
+}
+__global__ void k_pack_points(const mm_ipoint *aos, uint64_t n, int32_t n_contigs, uint64_t *packed, uint32_t *err)
+{
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const mm_ipoint p = aos[i];
+  if (p.seqId < 0 || p.seqId >= n_contigs || p.pos < 0) atomicOr(err, 1u);
+  packed[i] = mm_pack_point(p.seqId, p.pos, p.side > 0);
+}
+/* keys are distinct: a slot is claimed by CAS on its value word, the key is written afterwards (no reader yet) */
+__global__ void k_build_table(const uint64_t *keys, const uint64_t *offs, const uint8_t *is_freq, uint64_t n_keys, mm_tab_slot *tab,
+                              int tab_log2, uint32_t *err)
+{
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_keys) return;
+  uint64_t cnt = offs[i + 1] - offs[i];
+  if (is_freq[i] && cnt > MM_VAL_CNT_MASK) cnt = MM_VAL_CNT_MASK; /* a frequent seed's list is never gathered: only the flag is read */
+  if (cnt == 0 || cnt > MM_VAL_CNT_MASK || offs[i] >= (1ULL << (64 - MM_VAL_OFF_SHIFT))) { atomicOr(err, 2u); return; }
+  const uint64_t val = (offs[i] << MM_VAL_OFF_SHIFT) | (cnt << 1) | (is_freq[i] ? 1ULL : 0ULL);
+  const uint32_t mask = (1u << tab_log2) - 1u;
+  uint32_t slot = mm_tab_slot_of(keys[i], tab_log2);
+  for (uint32_t probe = 0; probe <= mask; probe++) {
+    const unsigned long long old = atomicCAS((unsigned long long *)&tab[slot].val, 0ULL, (unsigned long long)val);
+    if (old == 0ULL) { tab[slot].key = keys[i]; return; }
+    slot = (slot + 1) & mask;
+  }
+  atomicOr(err, 2u);
+}
+/* duplicates would occupy two slots: detect them after the build */
+__global__ void k_check_table_dups(const mm_tab_slot *tab, int tab_log2, uint32_t *err)
+{
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const uint64_t slots = 1ULL << tab_log2;
+  if (i >= slots || tab[i].val == 0) return;
+  const uint32_t mask = (uint32_t)(slots - 1);
+  uint32_t j = ((uint32_t)i + 1) & mask;
+  while (tab[j].val != 0) { /* the probe run that follows */
+    if (tab[j].key == tab[i].key) { atomicOr(err, 4u); return; }
+    j = (j + 1) & mask;
+    if (j == (uint32_t)i) return;
+  }
+}
+
+__global__ void k_count_seq(uint64_t n, const int32_t *__restrict__ seq, unsigned long long *cnt)
+{
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) atomicAdd(&cnt[seq[i]], 1ULL);
+}
+__global__ void k_unpack_points(uint64_t n, const uint64_t *__restrict__ pts, const uint64_t *__restrict__ keys, const uint64_t *__restrict__ offs,
+                                uint64_t n_keys, mm_ipoint *out)
+{ /* packed point -> skch::IntervalPoint (the hash comes from the key whose list the point is in) */
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  uint64_t lo = 0, hi = n_keys; /* last key with offs <= i */
+  while (lo + 1 < hi) { const uint64_t mid = (lo + hi) >> 1; if (offs[mid] <= i) lo = mid; else hi = mid; }
+  mm_ipoint p;
+  memset(&p, 0, sizeof p);
+  p.pos = mm_point_pos(pts[i]); p.hash = keys[lo]; p.seqId = mm_point_seq(pts[i]); p.side = mm_point_open(pts[i]) ? 1 : -1;
+  out[i] = p;
+}
+
 } // namespace
 
 #define MM_FOR_EACH_K(X) \
   X(8) X(9) X(10) X(11) X(12) X(13) X(14) X(15) X(16) X(17) X(18) X(19) X(20) X(21) X(22) X(23) X(24) X(25) X(26) X(27) \
   X(28) X(29) X(30) X(31) X(32)
-
-void mm_built_index_free(mm_built_index *b)
-{
-  if (!b) return;
-  cudaFree(b->hash); cudaFree(b->wpos); cudaFree(b->wend); cudaFree(b->seq); cudaFree(b->strand);
-  cudaFree(b->keys); cudaFree(b->offs); cudaFree(b->is_freq); cudaFree(b->pts);
-  *b = mm_built_index{};
-}
 
 int mm_build_index_device(const mm_params &p, const uint8_t *d_seq, const uint64_t *h_contig_off, int32_t n_contigs,
                           float kmer_pct_threshold, cudaStream_t st, int sm_count, mm_built_index *out, std::string &err)
@@ -746,7 +828,6 @@ int mm_build_index_device(const mm_params &p, const uint8_t *d_seq, const uint64
   uint64_t *keys = nullptr, *offs = nullptr, *pts = nullptr; uint8_t *is_freq = nullptr;
   int32_t threshold = 0x7fffffff;
   uint64_t n_final = 0;
-  uint64_t *f_hash = nullptr; int32_t *f_wpos = nullptr, *f_wend = nullptr, *f_seq = nullptr; int8_t *f_strand = nullptr;
   if (n_mi) {
     uint64_t *hk = nullptr, *hs = nullptr; uint32_t *va = nullptr, *perm = nullptr;
     CE(dv.alloc(hk, n_mi)); CE(dv.alloc(hs, n_mi)); CE(dv.alloc(va, n_mi)); CE(dv.alloc(perm, n_mi));
@@ -764,7 +845,8 @@ int mm_build_index_device(const mm_params &p, const uint8_t *d_seq, const uint64
     n_keys = lk + fk;
     n_points = 2 * (lr + fr);
     /* exclusive scans give, at a start flag, the index of the new key / run; at other records index + 1 of the current one */
-    CE(dv.alloc(keys, n_keys)); CE(dv.alloc(offs, n_keys + 1)); CE(dv.alloc(pts, n_points + 1)); CE(dv.alloc(is_freq, n_keys));
+    CE(out->keys.reserve(n_keys)); CE(out->offs.reserve(n_keys + 1)); CE(out->pts.reserve(n_points + 1)); CE(out->is_freq.reserve(n_keys));
+    keys = out->keys.get(); offs = out->offs.get(); pts = out->pts.get(); is_freq = out->is_freq.get();
     k_lookup_emit<<<blocks(n_mi), 256, 0, st>>>(n_mi, hs, perm, m_wpos, m_wend, m_seq, key_start, run_start, key_idx, run_idx, keys, offs, pts, rec_key);
     CE(cudaGetLastError());
     CE(cudaMemcpyAsync(offs + n_keys, &n_points, 8, cudaMemcpyHostToDevice, st));
@@ -822,8 +904,10 @@ int mm_build_index_device(const mm_params &p, const uint8_t *d_seq, const uint64
     CE(cudaMemcpy(&lo, koff + n_mi - 1, 8, cudaMemcpyDeviceToHost)); CE(cudaMemcpy(&lu, keep + n_mi - 1, 4, cudaMemcpyDeviceToHost));
     n_final = lo + lu;
     dv.free_now(perm); dv.free_now(rec_key);
-    CE(dv.alloc(f_hash, n_final)); CE(dv.alloc(f_wpos, n_final)); CE(dv.alloc(f_wend, n_final)); CE(dv.alloc(f_seq, n_final)); CE(dv.alloc(f_strand, n_final));
-    k_compact5<<<blocks(n_mi), 256, 0, st>>>(n_mi, keep, koff, m_hash, m_wpos, m_wend, m_seq, m_strand, f_hash, f_wpos, f_wend, f_seq, f_strand);
+    CE(out->hash.reserve(n_final)); CE(out->wpos.reserve(n_final)); CE(out->wend.reserve(n_final)); CE(out->seq.reserve(n_final));
+    CE(out->strand.reserve(n_final));
+    k_compact5<<<blocks(n_mi), 256, 0, st>>>(n_mi, keep, koff, m_hash, m_wpos, m_wend, m_seq, m_strand, out->hash.get(), out->wpos.get(),
+                                             out->wend.get(), out->seq.get(), out->strand.get());
     CE(cudaGetLastError());
     CE(cudaStreamSynchronize(st));
     dv.free_now(keep); dv.free_now(koff);
@@ -837,9 +921,67 @@ int mm_build_index_device(const mm_params &p, const uint8_t *d_seq, const uint64
   for (auto &e : ev) cudaEventDestroy(e);
 
   out->n_minmers = n_final; out->n_keys = n_keys; out->n_points = n_points; out->freq_threshold = threshold;
-  out->hash = f_hash; out->wpos = f_wpos; out->wend = f_wend; out->seq = f_seq; out->strand = f_strand;
-  out->keys = keys; out->offs = offs; out->is_freq = is_freq; out->pts = pts;
-  for (void *x : {(void *)f_hash, (void *)f_wpos, (void *)f_wend, (void *)f_seq, (void *)f_strand, (void *)keys, (void *)offs, (void *)is_freq, (void *)pts})
-    dv.release(x); /* now owned by *out (mm_built_index_free) */
   return MM_OK;
+}
+
+cudaError_t mm_upload_split_minmers(const mm_minmer *aos, uint64_t n, uint64_t *hash, int32_t *wpos, int32_t *wend, int8_t *strand,
+                                    cudaStream_t st)
+{
+  if (n == 0) return cudaSuccess;
+  k_split_minmers<<<(uint32_t)((n + 255) / 256), 256, 0, st>>>(aos, n, hash, wpos, wend, strand);
+  return cudaGetLastError();
+}
+cudaError_t mm_upload_pack_points(const mm_ipoint *aos, uint64_t n, int32_t n_contigs, uint64_t *packed, uint32_t *err, cudaStream_t st)
+{
+  if (n == 0) return cudaSuccess;
+  k_pack_points<<<(uint32_t)((n + 255) / 256), 256, 0, st>>>(aos, n, n_contigs, packed, err);
+  return cudaGetLastError();
+}
+cudaError_t mm_upload_build_table(const uint64_t *keys, const uint64_t *offs, const uint8_t *is_freq, uint64_t n_keys, mm_tab_slot *tab,
+                                  int tab_log2, uint32_t *err, cudaStream_t st)
+{
+  if (n_keys == 0) return cudaSuccess;
+  k_build_table<<<(uint32_t)((n_keys + 255) / 256), 256, 0, st>>>(keys, offs, is_freq, n_keys, tab, tab_log2, err);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  const uint64_t slots = 1ULL << tab_log2;
+  k_check_table_dups<<<(uint32_t)((slots + 255) / 256), 256, 0, st>>>(tab, tab_log2, err);
+  return cudaGetLastError();
+}
+
+/* per contig, entries sorted by wpos_end (stable): one device radix sort on (seqId, wpos_end) */
+cudaError_t mm_build_death_order(const uint64_t *idx_hash, const int32_t *idx_wend, const uint64_t *contig_start,
+                                 int32_t n_contigs, uint64_t n, uint64_t *idx2_hash, int32_t *idx2_wend, cudaStream_t st)
+{
+  if (n == 0) return cudaSuccess;
+  if (n >= (1ULL << 32)) return cudaErrorInvalidValue;
+  mm_devbuf<uint64_t> keys, keys2;
+  mm_devbuf<uint32_t> vals, vals2;
+  mm_devbuf<unsigned char> tmp;
+  size_t tmp_bytes = 0;
+  cudaError_t e;
+  if ((e = keys.reserve(n)) != cudaSuccess || (e = keys2.reserve(n)) != cudaSuccess || (e = vals.reserve(n)) != cudaSuccess ||
+      (e = vals2.reserve(n)) != cudaSuccess)
+    return e;
+  const uint32_t grid = (uint32_t)((n + 255) / 256);
+  k_fill_death_keys<<<grid, 256, 0, st>>>(idx_wend, contig_start, n_contigs, n, keys.get(), vals.get());
+  int end_bit = 32;
+  while ((1LL << (end_bit - 32)) < (long long)n_contigs + 1) end_bit++;
+  cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys.get(), keys2.get(), vals.get(), vals2.get(), (int64_t)n, 0, end_bit, st);
+  if ((e = tmp.reserve(tmp_bytes)) != cudaSuccess) return e;
+  e = cub::DeviceRadixSort::SortPairs(tmp.get(), tmp_bytes, keys.get(), keys2.get(), vals.get(), vals2.get(), (int64_t)n, 0, end_bit, st);
+  if (e == cudaSuccess) k_gather_death<<<grid, 256, 0, st>>>(idx_hash, keys2.get(), vals2.get(), n, idx2_hash, idx2_wend);
+  const cudaError_t s = cudaStreamSynchronize(st); /* before the temporaries go */
+  return e != cudaSuccess ? e : s != cudaSuccess ? s : cudaGetLastError();
+}
+cudaError_t mm_index_count_seq(uint64_t n, const int32_t *seq, unsigned long long *cnt, cudaStream_t st)
+{
+  k_count_seq<<<(uint32_t)((n + 255) / 256), 256, 0, st>>>(n, seq, cnt);
+  return cudaGetLastError();
+}
+cudaError_t mm_index_unpack_points(uint64_t n, const uint64_t *pts, const uint64_t *keys, const uint64_t *offs, uint64_t n_keys,
+                                   mm_ipoint *out, cudaStream_t st)
+{
+  k_unpack_points<<<(uint32_t)((n + 255) / 256), 256, 0, st>>>(n, pts, keys, offs, n_keys, out);
+  return cudaGetLastError();
 }

@@ -6,15 +6,16 @@
 
 #include <string>
 
+#include "mm_devbuf.h"
 #include "mm_internal.h"
 
-/* device arrays the builder leaves behind (owned by the struct: mm_built_index_free) */
+/* device arrays the builder leaves behind (owned by the struct) */
 struct mm_built_index {
   uint64_t n_minmers = 0, n_keys = 0, n_points = 0;
   /* minmerIndex after the frequent-seed drop, in reference order (seqId, wpos, wpos_end, emission order) */
-  uint64_t *hash = nullptr; int32_t *wpos = nullptr, *wend = nullptr, *seq = nullptr; int8_t *strand = nullptr;
+  mm_devbuf<uint64_t> hash; mm_devbuf<int32_t> wpos, wend, seq; mm_devbuf<int8_t> strand;
   /* minmerPosLookupIndex, keys ascending: keys[n_keys], offs[n_keys + 1], pts[n_points] (packed, mm_pack_point), is_freq[n_keys] */
-  uint64_t *keys = nullptr, *offs = nullptr, *pts = nullptr; uint8_t *is_freq = nullptr;
+  mm_devbuf<uint64_t> keys, offs, pts; mm_devbuf<uint8_t> is_freq;
   int32_t freq_threshold = 0x7fffffff;
   /* statistics */
   uint64_t n_minmers_before_filter = 0;
@@ -23,7 +24,6 @@ struct mm_built_index {
   unsigned long long hist_min_keys = 0, hist_max_keys = 0;
   float ms_scan = 0, ms_post = 0, ms_lookup = 0;
 };
-void mm_built_index_free(mm_built_index *b);
 /* d_seq: the contigs as text, back to back, on the device (readable up to h_contig_off[n_contigs]); returns MM_OK or MM_E* */
 int mm_build_index_device(const mm_params &p, const uint8_t *d_seq, const uint64_t *h_contig_off, int32_t n_contigs,
                           float kmer_pct_threshold, cudaStream_t st, int sm_count, mm_built_index *out, std::string &err);

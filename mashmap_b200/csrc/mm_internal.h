@@ -194,7 +194,7 @@ cudaError_t mm_launch_l2_scan(const mm_params &p, const mm_dev_index &ix, const 
                               cudaStream_t st, int sm_count);
 cudaError_t mm_launch_l2_overflow(const mm_params &p, const mm_dev_index &ix, const mm_dev_batch &b, uint32_t n_cands,
                                   cudaStream_t st, int sm_count);
-/* index upload helpers (mm_l2_stream.cu): AoS -> device layouts */
+/* index image helpers (mm_index_build.cu): AoS -> device layouts, and back */
 cudaError_t mm_upload_split_minmers(const mm_minmer *aos, uint64_t n, uint64_t *hash, int32_t *wpos, int32_t *wend,
                                     int8_t *strand, cudaStream_t st);
 cudaError_t mm_upload_pack_points(const mm_ipoint *aos, uint64_t n, int32_t n_contigs, uint64_t *packed, uint32_t *err,
@@ -204,6 +204,11 @@ cudaError_t mm_upload_build_table(const uint64_t *keys, const uint64_t *offs, co
 /* death-order arrays of the index (device-side sort) */
 cudaError_t mm_build_death_order(const uint64_t *idx_hash, const int32_t *idx_wend, const uint64_t *contig_start,
                                  int32_t n_contigs, uint64_t n, uint64_t *idx2_hash, int32_t *idx2_wend, cudaStream_t st);
+/* cnt[q] += number of entries of seq[0, n) equal to q */
+cudaError_t mm_index_count_seq(uint64_t n, const int32_t *seq, unsigned long long *cnt, cudaStream_t st);
+/* the n packed points back to skch::IntervalPoint, with the hash of the key whose list (keys, offs) holds each */
+cudaError_t mm_index_unpack_points(uint64_t n, const uint64_t *pts, const uint64_t *keys, const uint64_t *offs, uint64_t n_keys,
+                                   mm_ipoint *out, cudaStream_t st);
 uint32_t mm_l1_grid_size(const mm_params &p, int sm_count);
 int mm_sketch_kmer_supported(int k);
 /* dynamic shared memory the sketch kernel needs for (seg_length, sketch_size, kmer_size); 0 if unsupported */

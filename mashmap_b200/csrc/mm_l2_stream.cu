@@ -415,132 +415,7 @@ k_l2_scan(const mm_params prm, const mm_dev_index ix, const mm_dev_batch b, uint
   }
 }
 
-__global__ void k_fill_death_keys(const int32_t *idx_wend, const uint64_t *contig_start, int32_t n_contigs, uint64_t n,
-                                  uint64_t *keys, uint32_t *vals)
-{
-  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  int lo = 0, hi = n_contigs; /* contig of entry i: last c with contig_start[c] <= i */
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (contig_start[mid] <= i) lo = mid; else hi = mid;
-  }
-  keys[i] = ((uint64_t)(uint32_t)lo << 32) | (uint64_t)(uint32_t)idx_wend[i];
-  vals[i] = (uint32_t)i;
-}
-__global__ void k_gather_death(const uint64_t *idx_hash, const uint64_t *keys_sorted, const uint32_t *vals_sorted, uint64_t n,
-                               uint64_t *idx2_hash, int32_t *idx2_wend)
-{
-  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  idx2_hash[i] = idx_hash[vals_sorted[i]];
-  idx2_wend[i] = (int32_t)(uint32_t)keys_sorted[i];
-}
-
-__global__ void k_split_minmers(const mm_minmer *aos, uint64_t n, uint64_t *hash, int32_t *wpos, int32_t *wend, int8_t *strand)
-{
-  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const mm_minmer m = aos[i];
-  hash[i] = m.hash; wpos[i] = m.wpos; wend[i] = m.wpos_end; strand[i] = (int8_t)m.strand;
-}
-__global__ void k_pack_points(const mm_ipoint *aos, uint64_t n, int32_t n_contigs, uint64_t *packed, uint32_t *err)
-{
-  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const mm_ipoint p = aos[i];
-  if (p.seqId < 0 || p.seqId >= n_contigs || p.pos < 0) atomicOr(err, 1u);
-  packed[i] = mm_pack_point(p.seqId, p.pos, p.side > 0);
-}
-/* keys are distinct: a slot is claimed by CAS on its value word, the key is written afterwards (no reader yet) */
-__global__ void k_build_table(const uint64_t *keys, const uint64_t *offs, const uint8_t *is_freq, uint64_t n_keys, mm_tab_slot *tab,
-                              int tab_log2, uint32_t *err)
-{
-  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n_keys) return;
-  uint64_t cnt = offs[i + 1] - offs[i];
-  if (is_freq[i] && cnt > MM_VAL_CNT_MASK) cnt = MM_VAL_CNT_MASK; /* a frequent seed's list is never gathered: only the flag is read */
-  if (cnt == 0 || cnt > MM_VAL_CNT_MASK || offs[i] >= (1ULL << (64 - MM_VAL_OFF_SHIFT))) { atomicOr(err, 2u); return; }
-  const uint64_t val = (offs[i] << MM_VAL_OFF_SHIFT) | (cnt << 1) | (is_freq[i] ? 1ULL : 0ULL);
-  const uint32_t mask = (1u << tab_log2) - 1u;
-  uint32_t slot = mm_tab_slot_of(keys[i], tab_log2);
-  for (uint32_t probe = 0; probe <= mask; probe++) {
-    const unsigned long long old = atomicCAS((unsigned long long *)&tab[slot].val, 0ULL, (unsigned long long)val);
-    if (old == 0ULL) { tab[slot].key = keys[i]; return; }
-    slot = (slot + 1) & mask;
-  }
-  atomicOr(err, 2u);
-}
-/* duplicates would occupy two slots: detect them after the build */
-__global__ void k_check_table_dups(const mm_tab_slot *tab, int tab_log2, uint32_t *err)
-{
-  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const uint64_t slots = 1ULL << tab_log2;
-  if (i >= slots || tab[i].val == 0) return;
-  const uint32_t mask = (uint32_t)(slots - 1);
-  uint32_t j = ((uint32_t)i + 1) & mask;
-  while (tab[j].val != 0) { /* the probe run that follows */
-    if (tab[j].key == tab[i].key) { atomicOr(err, 4u); return; }
-    j = (j + 1) & mask;
-    if (j == (uint32_t)i) return;
-  }
-}
-
 } // namespace
-
-cudaError_t mm_upload_split_minmers(const mm_minmer *aos, uint64_t n, uint64_t *hash, int32_t *wpos, int32_t *wend, int8_t *strand,
-                                    cudaStream_t st)
-{
-  if (n == 0) return cudaSuccess;
-  k_split_minmers<<<(uint32_t)((n + 255) / 256), 256, 0, st>>>(aos, n, hash, wpos, wend, strand);
-  return cudaGetLastError();
-}
-cudaError_t mm_upload_pack_points(const mm_ipoint *aos, uint64_t n, int32_t n_contigs, uint64_t *packed, uint32_t *err, cudaStream_t st)
-{
-  if (n == 0) return cudaSuccess;
-  k_pack_points<<<(uint32_t)((n + 255) / 256), 256, 0, st>>>(aos, n, n_contigs, packed, err);
-  return cudaGetLastError();
-}
-cudaError_t mm_upload_build_table(const uint64_t *keys, const uint64_t *offs, const uint8_t *is_freq, uint64_t n_keys, mm_tab_slot *tab,
-                                  int tab_log2, uint32_t *err, cudaStream_t st)
-{
-  if (n_keys == 0) return cudaSuccess;
-  k_build_table<<<(uint32_t)((n_keys + 255) / 256), 256, 0, st>>>(keys, offs, is_freq, n_keys, tab, tab_log2, err);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return e;
-  const uint64_t slots = 1ULL << tab_log2;
-  k_check_table_dups<<<(uint32_t)((slots + 255) / 256), 256, 0, st>>>(tab, tab_log2, err);
-  return cudaGetLastError();
-}
-
-/* per contig, entries sorted by wpos_end (stable): one device radix sort on (seqId, wpos_end) */
-cudaError_t mm_build_death_order(const uint64_t *idx_hash, const int32_t *idx_wend, const uint64_t *contig_start,
-                                 int32_t n_contigs, uint64_t n, uint64_t *idx2_hash, int32_t *idx2_wend, cudaStream_t st)
-{
-  if (n == 0) return cudaSuccess;
-  if (n >= (1ULL << 32)) return cudaErrorInvalidValue;
-  uint64_t *keys = nullptr, *keys2 = nullptr;
-  uint32_t *vals = nullptr, *vals2 = nullptr;
-  void *tmp = nullptr;
-  size_t tmp_bytes = 0;
-  cudaError_t e;
-  if ((e = cudaMalloc(&keys, n * 8)) != cudaSuccess) return e;
-  if ((e = cudaMalloc(&keys2, n * 8)) != cudaSuccess) return e;
-  if ((e = cudaMalloc(&vals, n * 4)) != cudaSuccess) return e;
-  if ((e = cudaMalloc(&vals2, n * 4)) != cudaSuccess) return e;
-  const uint32_t grid = (uint32_t)((n + 255) / 256);
-  k_fill_death_keys<<<grid, 256, 0, st>>>(idx_wend, contig_start, n_contigs, n, keys, vals);
-  int end_bit = 32;
-  while ((1LL << (end_bit - 32)) < (long long)n_contigs + 1) end_bit++;
-  cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys, keys2, vals, vals2, (int64_t)n, 0, end_bit, st);
-  if ((e = cudaMalloc(&tmp, tmp_bytes)) != cudaSuccess) return e;
-  e = cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys, keys2, vals, vals2, (int64_t)n, 0, end_bit, st);
-  if (e != cudaSuccess) return e;
-  k_gather_death<<<grid, 256, 0, st>>>(idx_hash, keys2, vals2, n, idx2_hash, idx2_wend);
-  e = cudaStreamSynchronize(st);
-  cudaFree(keys); cudaFree(keys2); cudaFree(vals); cudaFree(vals2); cudaFree(tmp);
-  return e != cudaSuccess ? e : cudaGetLastError();
-}
 
 size_t mm_l2_scan_tmp_bytes(uint32_t n_cands)
 {
