@@ -116,9 +116,10 @@ typedef struct mm_ctx mm_ctx;
 /* ---- lifetime ---------------------------------------------------------------------------------- */
 
 /* Replaces nothing in the reference (it has no device); one context per GPU / per process rank. */
-/* Are these parameters inside the limits of the device path (k in 8..32; one segment's nibbles, twice, plus the sketch
- * kernel's selection tables within 227 KB of shared memory)? Needs no device: a caller checks BEFORE it reads and
- * indexes a reference. MM_OK, or MM_EINVAL with mm_last_error(NULL) saying which limit. */
+/* Are these parameters inside the limits of the device path (k in 8..32; every mapping kernel launchable: one segment's
+ * nibbles, twice, plus the sketch kernel's selection tables, and the L1 / L2 kernels' per-sketch state, each within 227 KB
+ * of shared memory)? Needs no device: a caller checks BEFORE it reads and indexes a reference. MM_OK, or MM_EINVAL with
+ * mm_last_error(NULL) naming the kernel that does not fit and the largest sketch size accepted for the segment length. */
 int mm_params_check(const mm_params *params);
 int mm_ctx_create(int device, const mm_params *params, mm_ctx **out);
 int mm_ctx_destroy(mm_ctx *ctx);

@@ -122,6 +122,14 @@ EXPORTED_SYMBOLS = [
 ]
 
 
+def params_check(kmer_size, seg_length, sketch_size):
+    """mm_params_check: (MM_OK, "") if a context with these parameters can launch every mapping kernel, else (MM_EINVAL,
+    the message naming the kernel that does not fit). Needs no device."""
+    L = lib()
+    rc = L.mm_params_check(C.byref(Params(kmer_size, seg_length, sketch_size)))
+    return rc, ("" if rc == MM_OK else L.mm_last_error(None).decode())
+
+
 def _ptr(a):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
 

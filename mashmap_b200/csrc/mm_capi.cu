@@ -718,6 +718,16 @@ int run_pipeline(mm_ctx *c)
   return fail(c, MM_ECUDA, "candidate/scratch buffers kept overflowing");
 }
 
+/* the first mapping kernel that cannot be launched for these sizes, or nullptr if all of them can */
+const char *kernel_that_does_not_fit(int seg_length, int sketch_size, int kmer_size)
+{
+  if (mm_sketch_smem_bytes(seg_length, sketch_size, kmer_size, nullptr, nullptr) == 0) return "the sketch kernel (K1)";
+  if (mm_l1_cta_smem(sketch_size) == 0) return "the general L1 kernel (K2)";
+  if (mm_l2_general_smem(sketch_size, nullptr) == 0) return "the general L2 kernel (K3)";
+  if (mm_l2_long_smem(sketch_size) == 0) return "the L2 kernel of fragments longer than a segment (K3)";
+  return nullptr;
+}
+
 } // namespace
 
 extern "C" {
@@ -729,10 +739,20 @@ int mm_params_check(const mm_params *params)
     return fail(nullptr, MM_EINVAL, "k-mer size %d is not compiled in (8..32)", params->kmer_size);
   if (params->sketch_size < 1 || params->seg_length < params->kmer_size)
     return fail(nullptr, MM_EINVAL, "bad sketch_size / seg_length");
-  if (mm_sketch_smem_bytes(params->seg_length, params->sketch_size, params->kmer_size, nullptr, nullptr) == 0)
-    return fail(nullptr, MM_EINVAL, "seg_length %d / sketch_size %d exceed the shared-memory budget of the sketch kernel",
-                params->seg_length, params->sketch_size);
-  return MM_OK;
+  const int L = params->seg_length, S = params->sketch_size, k = params->kmer_size;
+  const char *stage = kernel_that_does_not_fit(L, S, k);
+  if (!stage) return MM_OK;
+  /* the largest sketch size that fits: every size is smaller than S, and acceptance falls off once in S */
+  int lo = 0, hi = S; /* lo fits (or is 0), hi does not */
+  while (hi - lo > 1) {
+    const int mid = lo + (hi - lo) / 2;
+    if (kernel_that_does_not_fit(L, mid, k)) hi = mid; else lo = mid;
+  }
+  if (lo == 0)
+    return fail(nullptr, MM_EINVAL, "seg_length %d / sketch_size %d exceed the shared-memory budget of %s; no sketch size "
+                "is accepted for seg_length %d (k = %d)", L, S, stage, L, k);
+  return fail(nullptr, MM_EINVAL, "seg_length %d / sketch_size %d exceed the shared-memory budget of %s; the largest sketch "
+              "size accepted for seg_length %d (k = %d) is %d", L, S, stage, L, k, lo);
 }
 
 int mm_ctx_create(int device, const mm_params *params, mm_ctx **out)

@@ -211,7 +211,17 @@ cudaError_t mm_index_unpack_points(uint64_t n, const uint64_t *pts, const uint64
                                    mm_ipoint *out, cudaStream_t st);
 uint32_t mm_l1_grid_size(const mm_params &p, int sm_count);
 int mm_sketch_kmer_supported(int k);
-/* dynamic shared memory the sketch kernel needs for (seg_length, sketch_size, kmer_size); 0 if unsupported */
+/* Shared memory one block may have on sm_90 (dynamic and static together), and the dynamic shared memory each kernel
+ * whose size depends on the parameters is launched with; 0 where it cannot launch. The launchers and mm_params_check
+ * both call these. */
+constexpr size_t MM_SMEM_PER_BLOCK = 227 * 1024;
+/* K1 (k_sketch_table) for (seg_length, sketch_size, kmer_size), its table and list capacities */
 size_t mm_sketch_smem_bytes(int seg_length, int sketch_size, int kmer_size, int *table_cap, int *list_cap);
+/* K2's general path (k_l1_cta, k_l1_long) */
+size_t mm_l1_cta_smem(int sketch_size);
+/* K3's general kernel (k_l2) and the live-set capacity it is launched with */
+size_t mm_l2_general_smem(int sketch_size, int *live_cap);
+/* K3 of the fragments longer than a segment (k_l2_long) */
+size_t mm_l2_long_smem(int sketch_size);
 
 #endif

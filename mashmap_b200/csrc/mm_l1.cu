@@ -752,17 +752,20 @@ k_l1_long(const mm_params prm, const mm_dev_index ix, const mm_dev_batch b, cons
     l1_segment<128, L1_LOCAL_CANDS_CTA, L1_CTA_POINTS, true>(prm, ix, b, longs[w].seg, hits, skeys, scopn, shead, sginfo, sh, blockIdx.x);
 }
 
-size_t l1_cta_smem(const mm_params &p)
-{
-  return (((size_t)p.sketch_size * sizeof(l1_hit) + 15) & ~(size_t)15) + (size_t)L1_CTA_POINTS * (8 + 4 + 4 + 4);
-}
-
 } // namespace
+
+/* hit list | keys | copn | head | ginfo; the kernels' l1_shared is static shared memory on top */
+size_t mm_l1_cta_smem(int sketch_size)
+{
+  const size_t smem = (((size_t)sketch_size * sizeof(l1_hit) + 15) & ~(size_t)15) + (size_t)L1_CTA_POINTS * (8 + 4 + 4 + 4);
+  return smem + sizeof(l1_shared<128, L1_LOCAL_CANDS_CTA>) > MM_SMEM_PER_BLOCK ? 0 : smem;
+}
 
 /* CTAs of the persistent general-path grid (the scratch area holds one slice per CTA) */
 uint32_t mm_l1_grid_size(const mm_params &p, int sm_count)
 {
-  const size_t smem = l1_cta_smem(p);
+  const size_t smem = mm_l1_cta_smem(p.sketch_size);
+  if (smem == 0) return 0;
   if (cudaFuncSetAttribute(k_l1_cta, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return 0;
   int occ = 0;
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_l1_cta, 128, smem) != cudaSuccess) return 0;
@@ -780,7 +783,7 @@ cudaError_t mm_launch_l1(const mm_params &p, const mm_dev_index &ix, const mm_de
   if (grid == 0) return cudaErrorInvalidValue;
   const size_t wsmem = l1_warp_smem(p.sketch_size) * L1_WARPS_PER_CTA;
   if (!use_warp_path || !slow_list || wsmem > 227 * 1024) {
-    k_l1_cta<<<min(grid, b.n_segs), 128, l1_cta_smem(p), st>>>(p, ix, b, nullptr);
+    k_l1_cta<<<min(grid, b.n_segs), 128, mm_l1_cta_smem(p.sketch_size), st>>>(p, ix, b, nullptr);
     if (n_launched) *n_launched = 1;
     return cudaGetLastError();
   }
@@ -795,7 +798,7 @@ cudaError_t mm_launch_l1(const mm_params &p, const mm_dev_index &ix, const mm_de
   e = cudaGetLastError();
   if (e != cudaSuccess) return e;
   /* the general path reads its work count from counters[8] on the device: no host round trip in between */
-  k_l1_cta<<<grid, 128, l1_cta_smem(p), st>>>(p, ix, b, slow_list);
+  k_l1_cta<<<grid, 128, mm_l1_cta_smem(p.sketch_size), st>>>(p, ix, b, slow_list);
   if (n_launched) *n_launched = 2;
   return cudaGetLastError();
 }
@@ -808,7 +811,7 @@ cudaError_t mm_launch_l1_long(const mm_params &p, const mm_dev_index &ix, const 
   if (n_long == 0) return cudaSuccess;
   const uint32_t grid = mm_l1_grid_size(p, sm_count);
   if (grid == 0) return cudaErrorInvalidValue;
-  const size_t smem = l1_cta_smem(p);
+  const size_t smem = mm_l1_cta_smem(p.sketch_size);
   cudaError_t e = cudaFuncSetAttribute(k_l1_long, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
   k_l1_long<<<min(grid, n_long), 128, smem, st>>>(p, ix, b, longs, n_long);

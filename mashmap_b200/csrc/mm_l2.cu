@@ -637,17 +637,34 @@ k_l2_long(const mm_params prm, const mm_dev_index ix, const mm_dev_batch b, uint
 
 } // namespace
 
+/* four warps of: query sketch (hash, nbi, act, sv, strand) | live set (k_l2 only) | locus staging area, as the kernels
+ * lay them out. k_l2's live set is one 64-bit occupancy mask per lane (l2_scan): at most 64 x 32 entries. */
+size_t mm_l2_general_smem(int sketch_size, int *live_cap)
+{
+  const int cap = ((sketch_size + L2_LIVE_SLACK + 31) / 32) * 32;
+  if (cap > 64 * 32) return 0;
+  const size_t per_warp = ((size_t)(sketch_size + 2) * (8 + 4 + 4 + 4 + 1) + (size_t)cap * 8 +
+                           L2_STAGE_LOCI * sizeof(mm_l2_locus) + 63) & ~(size_t)15;
+  const size_t smem = per_warp * L2_WARPS;
+  if (smem > MM_SMEM_PER_BLOCK) return 0;
+  if (live_cap) *live_cap = cap;
+  return smem;
+}
+
+size_t mm_l2_long_smem(int sketch_size)
+{
+  const size_t per_warp = ((size_t)(sketch_size + 2) * (8 + 4 + 4 + 4 + 1) + L2_STAGE_LOCI * sizeof(mm_l2_locus) + 63) & ~(size_t)15;
+  const size_t smem = per_warp * L2_WARPS;
+  return smem > MM_SMEM_PER_BLOCK ? 0 : smem;
+}
+
 static cudaError_t launch_general(const mm_params &p, const mm_dev_index &ix, const mm_dev_batch &b, uint32_t n_cands,
                                   cudaStream_t st, int sm_count, int only_flagged)
 {
   if (n_cands == 0) return cudaSuccess;
-  const int S = p.sketch_size;
-  const int live_cap = ((S + L2_LIVE_SLACK + 31) / 32) * 32;
-  if (live_cap > 64 * 32) return cudaErrorInvalidValue;
-  const size_t per_warp = ((size_t)(S + 2) * (8 + 4 + 4 + 4 + 1) + (size_t)live_cap * 8 +
-                           L2_STAGE_LOCI * sizeof(mm_l2_locus) + 63) & ~(size_t)15;
-  const size_t smem = per_warp * L2_WARPS;
-  if (smem > 227 * 1024) return cudaErrorInvalidValue;
+  int live_cap = 0;
+  const size_t smem = mm_l2_general_smem(p.sketch_size, &live_cap);
+  if (smem == 0) return cudaErrorInvalidValue;
   cudaError_t e = cudaFuncSetAttribute(k_l2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
   int occ = 0;
@@ -691,10 +708,8 @@ cudaError_t mm_launch_l2_long(const mm_params &p, const mm_dev_index &ix, const 
                               const uint64_t *table_off, uint64_t *table, cudaStream_t st, int sm_count)
 {
   if (n_cands == 0) return cudaSuccess;
-  const int S = p.sketch_size;
-  const size_t per_warp = ((size_t)(S + 2) * (8 + 4 + 4 + 4 + 1) + L2_STAGE_LOCI * sizeof(mm_l2_locus) + 63) & ~(size_t)15;
-  const size_t smem = per_warp * L2_WARPS;
-  if (smem > 227 * 1024) return cudaErrorInvalidValue;
+  const size_t smem = mm_l2_long_smem(p.sketch_size);
+  if (smem == 0) return cudaErrorInvalidValue;
   cudaError_t e = cudaFuncSetAttribute(k_l2_long, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
   uint32_t grid = (uint32_t)sm_count * 4u;

@@ -295,6 +295,7 @@ k_l2_scan(const mm_params prm, const mm_dev_index ix, const mm_dev_batch b, uint
     }
     __syncwarp();
     int pivot = n, pivRank = n, shared = 0, votes = 0;
+    int pos_votes = 0; /* votes before the deletes of the current insert's position (computeMap.hpp:1342 precedes :1344) */
     bool sv_overflow = false;
     int best = 1; /* bestSketchSize (computeMap.hpp:1317) */
     bool in_cand = false, has_back = false;
@@ -341,7 +342,7 @@ k_l2_scan(const mm_params prm, const mm_dev_index ix, const mm_dev_batch b, uint
         const uint2 v = ring_fetch(do_del ? sm_d : sm_i, do_del ? g_d : g_i, p);
         const int slot = (int)(info & MM_L2_SLOT_MASK);
         const bool match = (info & MM_L2_MATCH) != 0;
-        const int prev_votes = votes; /* computeMap.hpp:1342 (only read after an insert) */
+        const int prev_votes = pos_votes; /* only read after an insert */
         if (slot <= n) {
           /* insert_minmer / delete_minmer (slidingMap.hpp:125-165, :171-211) as one straight-line update: the four
            * cases (insert/delete x hash in the query sketch or not) are selected with predicates, so the 32 candidates of
@@ -392,7 +393,7 @@ k_l2_scan(const mm_params prm, const mm_dev_index ix, const mm_dev_batch b, uint
         }
         /* consume the record */
         if (do_del) { p_d = p; drec = v; d++; }
-        else { p_i = p; irec = inext; inext = v; i++; }
+        else { p_i = p; irec = inext; inext = v; i++; pos_votes = votes; }
       }
     }
     if (valid) {
