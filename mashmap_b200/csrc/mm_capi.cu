@@ -12,6 +12,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -21,6 +22,12 @@
 #include <chrono>
 
 static thread_local std::string g_create_error;
+
+/* the slots of mm_last_stage_ms, as include/mashmap_b200.h documents them */
+enum stage_slot { ST_SKETCH = 0, ST_L1 = 1, ST_L2 = 2, ST_H2D = 3, ST_D2H = 4, ST_KERNELS = 5, ST_L2_PREP = 6, ST_L2_SCAN = 7, N_STAGE_SLOTS = 8 };
+/* stage boundaries, recorded on the context's stream; K1 starts where K0 (the packing of a text batch) ends */
+enum stage_event { EV_MAP_START, EV_K1_START, EV_K1_END, EV_K2_END, EV_K3_START, EV_K3_END, EV_PREP_START, EV_PREP_END,
+                   EV_UPLOAD_START, EV_UPLOAD_END, EV_FETCH_START, EV_FETCH_END, N_STAGE_EVENTS };
 
 struct mm_ctx {
   int device = -1;
@@ -46,7 +53,6 @@ struct mm_ctx {
   mm_built_index built{}; /* lookup arrays of an index built on the device, kept for mm_index_download (keep_lookup) */
   bool built_kept = false;
   bool batch_is_ascii = false; /* the resident batch came in as text: K0 (pack) runs in front of K1 */
-  cudaEvent_t ev_pack = nullptr;
   float pack_ms = 0;
   mm_devbuf<mm_segment> d_segs; uint64_t n_segs = 0;
   /* fragments longer than seg_length: K1 runs over d_work_segs = the caller's n_segs segments (a long one replaced by its
@@ -68,7 +74,7 @@ struct mm_ctx {
   mm_devbuf<uint64_t> d_long_table;
   mm_devbuf<mm_l1_candidate> d_cands;
   mm_devbuf<mm_l2_locus> d_loci;
-  mm_devbuf<uint32_t> d_counters;
+  mm_devbuf<mm_counters> d_counters;
   bool blocking_wait = false;       /* MM_BLOCKING_WAIT=1: host waits block on an event instead of spinning (experiment) */
   cudaEvent_t ev_wait = nullptr;
   const mm_ctx *share_src = nullptr; /* mm_ctx_share_index: the context whose index image this one reads */
@@ -88,8 +94,17 @@ struct mm_ctx {
   int l2_mode = 1; /* 1 = stream kernels (mm_l2_stream.cu), 0 = general kernel only (MM_L2_GENERAL=1) */
   bool batch_mapped = false;
 
-  cudaEvent_t ev[10]{};
-  float stage_ms[8]{};
+  cudaEvent_t ev[N_STAGE_EVENTS]{};
+  float stage_ms[N_STAGE_SLOTS]{};
+
+  /* the one release path of all but its device memory (mm_devbufs): for mm_ctx_destroy and every failed mm_ctx_create */
+  ~mm_ctx()
+  {
+    for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
+    if (ev_wait) cudaEventDestroy(ev_wait);
+    if (h_pub) cudaFreeHost(h_pub);
+    if (stream) cudaStreamDestroy(stream);
+  }
 };
 
 namespace {
@@ -294,7 +309,7 @@ int prepare_batch_buffers(mm_ctx *c, uint64_t n_bases, uint64_t n_segs)
   CU(c, c->d_sk_strand.reserve(n));
   CU(c, c->d_seg_res.reserve(n_segs + 1));
   CU(c, c->d_sk_reject.reserve(n_segs + 1));
-  CU(c, c->d_counters.reserve(16));
+  CU(c, c->d_counters.reserve(1));
   return MM_OK;
 }
 
@@ -391,7 +406,7 @@ int upload_batch(mm_ctx *c, const void *bases, uint64_t n_bases, const mm_segmen
     CU(c, cudaMemcpyAsync(c->d_long.get(), longs.data(), longs.size() * sizeof(mm_long_frag), cudaMemcpyHostToDevice, c->stream));
     CU(c, cudaMemcpyAsync(c->d_long_off.get(), entry_off.data(), entry_off.size() * 8, cudaMemcpyHostToDevice, c->stream));
   }
-  CU(c, cudaEventRecord(c->ev[6], c->stream));
+  CU(c, cudaEventRecord(c->ev[EV_UPLOAD_START], c->stream));
   if (packed) {
     const uint64_t pbytes = (n_bases + 1) / 2;
     if ((rc = copy_in(c, c->d_packed.get(), bases, pbytes))) return rc;
@@ -403,7 +418,7 @@ int upload_batch(mm_ctx *c, const void *bases, uint64_t n_bases, const mm_segmen
     CU(c, cudaMemsetAsync(c->d_bases.get() + n_bases, 'N', 256, c->stream));
   }
   CU(c, cudaMemcpyAsync(c->d_segs.get(), segs, n_segs * sizeof(mm_segment), cudaMemcpyHostToDevice, c->stream));
-  CU(c, cudaEventRecord(c->ev[7], c->stream));
+  CU(c, cudaEventRecord(c->ev[EV_UPLOAD_END], c->stream));
   if (!longs.empty()) CU(c, cudaStreamSynchronize(c->stream)); /* work / longs / entry_off are about to go */
   c->n_bases = n_bases;
   c->n_segs = n_segs;
@@ -493,29 +508,63 @@ __global__ void k_set_u32(uint32_t *dst, uint32_t v) { *dst = v; }
 __global__ void k_zero_words(uint32_t *dst, int n) { if ((int)threadIdx.x < n) dst[threadIdx.x] = 0; }
 #define ZERO_WORDS(c, ptr, n) do { k_zero_words<<<1, 32, 0, (c)->stream>>>((uint32_t *)(ptr), (n)); (c)->launches++; CU((c), cudaGetLastError()); } while (0)
 
-int read_words(mm_ctx *c, const void *dev, uint32_t *out, int n_words)
+int read_back(mm_ctx *c, const void *dev, void *out, size_t bytes) /* bytes: whole words, at most 32 of them */
 {
-  k_publish<<<1, 32, 0, c->stream>>>((const uint32_t *)dev, c->h_pub, n_words);
+  k_publish<<<1, 32, 0, c->stream>>>((const uint32_t *)dev, c->h_pub, (int)(bytes / 4));
   c->launches++;
   CU(c, cudaGetLastError());
   CU(c, wait_stream(c));
-  for (int i = 0; i < n_words; i++) out[i] = c->h_pub[i];
+  memcpy(out, c->h_pub, bytes);
   return MM_OK;
 }
-#define RD(c, dev, out, n) do { int rc__ = read_words((c), (dev), (out), (n)); if (rc__) return rc__; } while (0)
+#define RD(c, dev, out) do { int rc__ = read_back((c), (dev), (out), sizeof *(out)); if (rc__) return rc__; } while (0)
 
 /* returned by run_l2_stream when its own work areas cannot be allocated: the general kernel maps the batch instead */
 constexpr int L2_STREAM_NO_ROOM = 1;
+constexpr int L2_NONE_APPENDED = 2; /* see run_l2_loci */
 
-/* K3 fast path (mm_l2_stream.cu): ranges+scan -> records -> lane-per-candidate scan -> general kernel for the
- * candidates that need more locus slots. */
-int run_l2_stream(mm_ctx *c, uint32_t *h_cnt)
+/* K3's locus overflow policy, for each of its drivers. An attempt clears the overflow flag, runs `before` (L2_NONE_APPENDED:
+ * no loci to append, done), starts the locus counter at `base`, queues `append` (kernels appending loci at the counter)
+ * and reads the counters back. A live-set overflow is an error; loci that did not fit grow the locus buffer (keeping
+ * [0, base) when `keep`) and the attempt is repeated. On success c->n_loci is the end of the loci. */
+template <class Before, class Append>
+int run_l2_loci(mm_ctx *c, uint64_t base, bool keep, Before &&before, Append &&append)
+{
+  mm_counters *dc = c->d_counters.get();
+  for (int attempt = 0; attempt < 4; attempt++) {
+    ZERO_WORDS(c, &dc->l2_overflow, 1);
+    const int rc = before(make_batch(c));
+    if (rc == L2_NONE_APPENDED) { c->n_loci = base; return MM_OK; }
+    if (rc) return rc;
+    k_set_u32<<<1, 1, 0, c->stream>>>(&dc->loci_needed, (uint32_t)base);
+    c->launches++;
+    CU(c, cudaGetLastError());
+    if (int rc2 = append(make_batch(c))) return rc2;
+    mm_counters cnt;
+    RD(c, dc, &cnt);
+    if (cnt.l2_overflow == MM_L2_LIVE_SET_OVERFLOW)
+      return fail(c, MM_ECUDA, "L2 live-set overflow: the reference index has more than sketch_size+64 overlapping minmer "
+                  "windows at one position");
+    if (cnt.l2_overflow != MM_L2_LOCI_OVERFLOW && cnt.loci_needed <= c->d_loci.capacity()) {
+      c->n_loci = cnt.loci_needed;
+      return MM_OK;
+    }
+    c->diag[MM_DIAG_L2_LOCI_REGROW]++;
+    const uint64_t want = (uint64_t)cnt.loci_needed + cnt.loci_needed / 4 + 1024;
+    CU(c, keep ? c->d_loci.reserve_keep(want, base, c->stream) : c->d_loci.reserve(want));
+  }
+  return fail(c, MM_ECUDA, "locus buffer kept overflowing");
+}
+
+/* K3 fast path (mm_l2_stream.cu): ranges+scan -> records -> lane-per-candidate scan into the fixed locus slots ->
+ * general kernel for the candidates that need more, their loci appended after the fixed slots. */
+int run_l2_stream(mm_ctx *c)
 {
   const uint64_t nc = c->n_cands;
   const uint32_t LPC = 2;
-  CU(c, cudaEventRecord(c->ev[3], c->stream));
+  CU(c, cudaEventRecord(c->ev[EV_K3_START], c->stream));
   if (nc == 0) {
-    CU(c, cudaEventRecord(c->ev[4], c->stream));
+    CU(c, cudaEventRecord(c->ev[EV_K3_END], c->stream));
     CU(c, wait_stream(c));
     c->n_loci = 0;
     return MM_OK;
@@ -530,20 +579,16 @@ int run_l2_stream(mm_ctx *c, uint32_t *h_cnt)
     }
   }
   if (c->d_loci.capacity() < nc * LPC + 1024) CU(c, c->d_loci.reserve(nc * LPC + nc / 8 + 4096));
-  mm_dev_batch b = make_batch(c);
-  const auto tk0 = std::chrono::steady_clock::now();
   ZERO_WORDS(c, c->d_l2_rec_off.get() + nc, 2);
-  CU(c, mm_launch_l2_ranges(c->params, c->ix, b, (uint32_t)nc, c->d_scan_tmp.get(), c->d_scan_tmp.capacity(), c->stream));
+  CU(c, mm_launch_l2_ranges(c->params, c->ix, make_batch(c), (uint32_t)nc, c->d_scan_tmp.get(), c->d_scan_tmp.capacity(),
+                            c->stream));
   uint64_t total = 0;
-  RD(c, c->d_l2_rec_off.get() + nc, (uint32_t *)&total, 2);
-  const auto tk1 = std::chrono::steady_clock::now();
-  c->stage_ms[6] = std::chrono::duration<float, std::milli>(tk1 - tk0).count(); /* host view: ranges + scan + readback */
+  RD(c, c->d_l2_rec_off.get() + nc, &total);
   /* the scan's record readers run up to 2 * RING_CHUNKS + 2 records past a stream's end */
   if (total + 64 > c->d_l2_recs.capacity() && c->d_l2_recs.reserve(total + total / 16 + 1024)) return L2_STREAM_NO_ROOM;
-  for (int attempt = 0; attempt < 4; attempt++) {
-    b = make_batch(c);
-    ZERO_WORDS(c, c->d_counters.get() + 1, 1);
-    ZERO_WORDS(c, c->d_counters.get() + 6, 2);
+  /* the general kernel overwrites the flags of the candidates it redoes: every attempt runs the stream kernels too */
+  auto stream_pass = [&](mm_dev_batch b) {
+    ZERO_WORDS(c, &b.counters->l2_redo, 1);
     /* the record-preparation kernel is the bandwidth-bound one: no PCIe upload next to it (MM_PHASE_L2) */
     {
       struct phase_guard { /* the hook is always closed, whatever fails in between */
@@ -552,105 +597,71 @@ int run_l2_stream(mm_ctx *c, uint32_t *h_cnt)
         void close() { if (open) { c->hook(c->hook_user, MM_PHASE_L2, 0); open = false; } }
         ~phase_guard() { close(); }
       } guard(c);
-      CU(c, cudaEventRecord(c->ev[8], c->stream));
+      CU(c, cudaEventRecord(c->ev[EV_PREP_START], c->stream));
       CU(c, mm_launch_l2_prep(c->params, c->ix, b, (uint32_t)nc, c->stream, c->sm_count));
-      CU(c, cudaEventRecord(c->ev[9], c->stream));
+      CU(c, cudaEventRecord(c->ev[EV_PREP_END], c->stream));
       if (guard.open && c->blocking_wait) CU(c, cudaEventRecord(c->ev_wait, c->stream));
       uint32_t *perm = nullptr;
       CU(c, mm_launch_l2_order(b, (uint32_t)nc, c->d_l2_order.get(), c->d_l2_order.capacity(), &perm, c->stream));
       b.l2_perm = perm;
       CU(c, mm_launch_l2_scan(c->params, c->ix, b, (uint32_t)nc, c->stream, c->sm_count));
       /* the scan is already queued behind it: waiting for the end of the preparation kernel costs no bubble */
-      if (guard.open) CU(c, cudaEventSynchronize(c->blocking_wait ? c->ev_wait : c->ev[9]));
+      if (guard.open) CU(c, cudaEventSynchronize(c->blocking_wait ? c->ev_wait : c->ev[EV_PREP_END]));
     }
     c->launches += 4; /* own kernels: ranges, prep, order keys, scan (the prefix sum and the sort are library calls, not counted) */
-    RD(c, c->d_counters.get(), h_cnt, 16);
-    uint64_t extent = nc * LPC;
-    if (h_cnt[7] > 0) { /* candidates with more than LPC loci: general kernel, loci appended after the fixed slots */
-      c->diag[MM_DIAG_L2_GENERAL_CANDS] += h_cnt[7];
-      const uint32_t base = (uint32_t)extent;
-      k_set_u32<<<1, 1, 0, c->stream>>>(c->d_counters.get() + 6, base);
-      c->launches++;
-      CU(c, mm_launch_l2_overflow(c->params, c->ix, b, (uint32_t)nc, c->stream, c->sm_count));
-      c->launches += 1;
-      RD(c, c->d_counters.get(), h_cnt, 16);
-      if (h_cnt[1] == 2) return fail(c, MM_ECUDA, "L2 live-set overflow in the general kernel");
-      if (h_cnt[1] == 1 || h_cnt[6] > c->d_loci.capacity()) { /* grow and redo prep+scan+overflow */
-        c->diag[MM_DIAG_L2_LOCI_REGROW]++;
-        CU(c, c->d_loci.reserve((uint64_t)h_cnt[6] + h_cnt[6] / 4 + 1024));
-        continue;
-      }
-      extent = h_cnt[6];
-    }
-    CU(c, cudaEventRecord(c->ev[4], c->stream));
-    CU(c, wait_stream(c));
-    cudaEventElapsedTime(&c->stage_ms[6], c->ev[8], c->ev[9]); /* k_l2_prep */
-    cudaEventElapsedTime(&c->stage_ms[7], c->ev[9], c->ev[4]); /* k_l2_scan (+ overflow kernel) */
-    c->n_loci = extent;
+    mm_counters cnt;
+    RD(c, b.counters, &cnt);
+    if (cnt.l2_redo == 0) return L2_NONE_APPENDED;
+    c->diag[MM_DIAG_L2_GENERAL_CANDS] += cnt.l2_redo;
     return MM_OK;
-  }
-  return fail(c, MM_ECUDA, "locus buffer kept overflowing");
+  };
+  int rc = run_l2_loci(c, nc * LPC, false, stream_pass, [&](const mm_dev_batch &b) {
+    CU(c, mm_launch_l2_overflow(c->params, c->ix, b, (uint32_t)nc, c->stream, c->sm_count));
+    c->launches += 1;
+    return MM_OK;
+  });
+  if (rc) return rc;
+  CU(c, cudaEventRecord(c->ev[EV_K3_END], c->stream));
+  CU(c, wait_stream(c));
+  cudaEventElapsedTime(&c->stage_ms[ST_L2_PREP], c->ev[EV_PREP_START], c->ev[EV_PREP_END]);
+  cudaEventElapsedTime(&c->stage_ms[ST_L2_SCAN], c->ev[EV_PREP_END], c->ev[EV_K3_END]); /* k_l2_scan (+ overflow kernel) */
+  return MM_OK;
 }
 
 /* K3 of the candidates of fragments longer than seg_length (k_l2_long, mm_l2.cu), after the loci of the others, which end
- * at c->n_loci: live-table sizes -> offsets -> (host reads the total) -> the scans, appending at counters[6]. Records
- * ev[4] again at its end. */
-int run_l2_long(mm_ctx *c, uint32_t *h_cnt)
+ * at c->n_loci: live-table sizes -> offsets -> (host reads the total) -> the scans, appending at c->n_loci. */
+int run_l2_long(mm_ctx *c)
 {
   const uint64_t nc = c->n_cands;
   if (c->n_long == 0 || nc == 0) return MM_OK;
   CU(c, c->d_l2_long_off.reserve(nc + 1));
   CU(c, c->d_long_scan_tmp.reserve(mm_l2_scan_tmp_bytes((uint32_t)nc) + 256));
-  mm_dev_batch b = make_batch(c);
-  CU(c, mm_launch_l2_long_ranges(c->params, c->ix, b, (uint32_t)nc, c->d_l2_long_off.get(), c->d_long_scan_tmp.get(),
+  CU(c, mm_launch_l2_long_ranges(c->params, c->ix, make_batch(c), (uint32_t)nc, c->d_l2_long_off.get(), c->d_long_scan_tmp.get(),
                                  c->d_long_scan_tmp.capacity(), c->stream));
   c->launches++;
   uint64_t words = 0;
-  RD(c, c->d_l2_long_off.get() + nc, (uint32_t *)&words, 2);
+  RD(c, c->d_l2_long_off.get() + nc, &words);
   if (words == 0) return MM_OK;
   CU(c, c->d_long_table.reserve(words));
-  for (int attempt = 0; attempt < 4; attempt++) {
-    b = make_batch(c);
-    ZERO_WORDS(c, c->d_counters.get() + 1, 1);
-    k_set_u32<<<1, 1, 0, c->stream>>>(c->d_counters.get() + 6, (uint32_t)c->n_loci);
+  return run_l2_loci(c, c->n_loci, true, [](const mm_dev_batch &) { return MM_OK; }, [&](const mm_dev_batch &b) {
     CU(c, mm_launch_l2_long(c->params, c->ix, b, (uint32_t)nc, c->d_l2_long_off.get(), c->d_long_table.get(), c->stream,
                             c->sm_count));
-    c->launches += 2;
-    CU(c, cudaEventRecord(c->ev[4], c->stream));
-    RD(c, c->d_counters.get(), h_cnt, 16);
-    if (h_cnt[1] == 1 || h_cnt[6] > c->d_loci.capacity()) { /* a bigger locus buffer that keeps the loci already there, then again */
-      c->diag[MM_DIAG_L2_LOCI_REGROW]++;
-      CU(c, c->d_loci.reserve_keep((uint64_t)h_cnt[6] + h_cnt[6] / 4 + 1024, c->n_loci, c->stream));
-      continue;
-    }
-    c->n_loci = h_cnt[6];
+    c->launches++;
+    CU(c, cudaEventRecord(c->ev[EV_K3_END], c->stream));
     return MM_OK;
-  }
-  return fail(c, MM_ECUDA, "locus buffer kept overflowing");
+  });
 }
 
-/* K3 by the general kernel (mm_l2.cu), retried alone if the locus buffer is too small (it is idempotent) */
-int run_l2_general(mm_ctx *c, uint32_t *h_cnt)
+/* K3 by the general kernel (mm_l2.cu) alone; it is idempotent, so a retry is the kernel again */
+int run_l2_general(mm_ctx *c)
 {
-  for (int attempt = 0; attempt < 4; attempt++) {
-    const mm_dev_batch b = make_batch(c);
-    ZERO_WORDS(c, c->d_counters.get() + 1, 1);
-    ZERO_WORDS(c, c->d_counters.get() + 6, 2);
-    CU(c, cudaEventRecord(c->ev[3], c->stream));
+  return run_l2_loci(c, 0, false, [](const mm_dev_batch &) { return MM_OK; }, [&](const mm_dev_batch &b) {
+    CU(c, cudaEventRecord(c->ev[EV_K3_START], c->stream));
     CU(c, mm_launch_l2(c->params, c->ix, b, (uint32_t)c->n_cands, c->stream, c->sm_count));
-    CU(c, cudaEventRecord(c->ev[4], c->stream));
+    CU(c, cudaEventRecord(c->ev[EV_K3_END], c->stream));
     if (c->n_cands) c->launches += 1;
-    RD(c, c->d_counters.get(), h_cnt, 16);
-    if (h_cnt[1] == 2) return fail(c, MM_ECUDA, "L2 live-set overflow: the reference index has more than "
-                                   "sketch_size+64 overlapping minmer windows at one position");
-    if (h_cnt[1] == 1 || h_cnt[6] > c->d_loci.capacity()) {
-      CU(c, c->d_loci.reserve((uint64_t)h_cnt[6] + h_cnt[6] / 4 + 1024));
-      continue;
-    }
-    c->n_loci = h_cnt[6];
     return MM_OK;
-  }
-  return fail(c, MM_ECUDA, "locus buffer kept overflowing");
+  });
 }
 
 /* K1 -> K2 -> K3 on the resident batch, growing output buffers and retrying on overflow */
@@ -668,34 +679,34 @@ int run_pipeline(mm_ctx *c)
   if ((rc = ensure_scratch(c, c->d_scratch ? c->d_scratch.capacity() - c->scratch_pool : pool0))) return rc;
   if (c->d_l1_slow.capacity() < n_segs + 1) CU(c, c->d_l1_slow.reserve(n_segs + n_segs / 8 + 1024));
 
-  uint32_t h_cnt[16];
   for (int attempt = 0; attempt < 6; attempt++) {
     mm_dev_batch b = make_batch(c);
-    ZERO_WORDS(c, c->d_counters.get(), 16);
-    CU(c, cudaEventRecord(c->ev[0], c->stream));
+    ZERO_WORDS(c, c->d_counters.get(), sizeof(mm_counters) / 4);
+    CU(c, cudaEventRecord(c->ev[EV_MAP_START], c->stream));
     if ((rc = launch_pack_if_ascii(c))) return rc;
-    CU(c, cudaEventRecord(c->ev_pack, c->stream));
+    CU(c, cudaEventRecord(c->ev[EV_K1_START], c->stream));
     if ((rc = launch_sketch_all(c, true))) return rc;
-    CU(c, cudaEventRecord(c->ev[1], c->stream));
+    CU(c, cudaEventRecord(c->ev[EV_K1_END], c->stream));
     int l1_launches = 0;
     CU(c, mm_launch_l1(c->params, c->ix, b, c->stream, c->sm_count, c->d_l1_slow.get(), c->l1_warp, &l1_launches));
     if (c->n_long) { /* windowLen > 0: k_l1_long (mm_l1.cu), after the general path (it reuses its scratch slices) */
       CU(c, mm_launch_l1_long(c->params, c->ix, b, c->d_long.get(), c->n_long, c->stream, c->sm_count));
       l1_launches++;
     }
-    CU(c, cudaEventRecord(c->ev[2], c->stream));
+    CU(c, cudaEventRecord(c->ev[EV_K2_END], c->stream));
     c->launches += (uint64_t)l1_launches;
-    RD(c, c->d_counters.get(), h_cnt, 16);
-    const uint64_t need_cands = h_cnt[0];
+    mm_counters cnt;
+    RD(c, c->d_counters.get(), &cnt);
+    const uint64_t need_cands = cnt.cands_needed;
     bool retry = false;
-    c->diag[MM_DIAG_L1_CTA_SEGMENTS] += h_cnt[8];
-    c->diag[MM_DIAG_SKETCH_GENERAL_SEGMENTS] += h_cnt[9];
-    if (h_cnt[3] || need_cands > c->d_cands.capacity()) {
+    c->diag[MM_DIAG_L1_CTA_SEGMENTS] += cnt.l1_cta_segments;
+    c->diag[MM_DIAG_SKETCH_GENERAL_SEGMENTS] += cnt.sketch_rejects;
+    if (cnt.cand_overflow || need_cands > c->d_cands.capacity()) {
       c->diag[MM_DIAG_CAND_REGROW]++;
       CU(c, c->d_cands.reserve(need_cands + need_cands / 4 + 1024));
       retry = true;
     }
-    if (h_cnt[2]) { /* scratch pool exhausted: quadruple it */
+    if (cnt.scratch_overflow) { /* quadruple the pool */
       c->diag[MM_DIAG_L1_POOL_REGROW]++;
       if ((rc = ensure_scratch(c, (c->d_scratch.capacity() - c->scratch_pool) * 4))) return rc;
       retry = true;
@@ -703,14 +714,15 @@ int run_pipeline(mm_ctx *c)
     if (retry) continue;
     c->n_cands = need_cands;
     /* K3: the stream kernels, or the general kernel where they are off or their own work areas do not fit */
-    rc = c->l2_mode == 1 ? run_l2_stream(c, h_cnt) : L2_STREAM_NO_ROOM;
-    if (rc == L2_STREAM_NO_ROOM) rc = run_l2_general(c, h_cnt);
-    if (rc || (rc = run_l2_long(c, h_cnt))) return rc;
-    if (c->batch_is_ascii) cudaEventElapsedTime(&c->pack_ms, c->ev[0], c->ev_pack);
-    cudaEventElapsedTime(&c->stage_ms[0], c->ev_pack, c->ev[1]);
-    cudaEventElapsedTime(&c->stage_ms[1], c->ev[1], c->ev[2]);
-    cudaEventElapsedTime(&c->stage_ms[2], c->ev[3], c->ev[4]);
-    cudaEventElapsedTime(&c->stage_ms[5], c->ev[0], c->ev[4]); /* first launch -> last kernel end, incl. host gaps */
+    c->stage_ms[ST_L2_PREP] = c->stage_ms[ST_L2_SCAN] = 0; /* timed by the stream path only */
+    rc = c->l2_mode == 1 ? run_l2_stream(c) : L2_STREAM_NO_ROOM;
+    if (rc == L2_STREAM_NO_ROOM) rc = run_l2_general(c);
+    if (rc || (rc = run_l2_long(c))) return rc;
+    if (c->batch_is_ascii) cudaEventElapsedTime(&c->pack_ms, c->ev[EV_MAP_START], c->ev[EV_K1_START]);
+    cudaEventElapsedTime(&c->stage_ms[ST_SKETCH], c->ev[EV_K1_START], c->ev[EV_K1_END]);
+    cudaEventElapsedTime(&c->stage_ms[ST_L1], c->ev[EV_K1_END], c->ev[EV_K2_END]);
+    cudaEventElapsedTime(&c->stage_ms[ST_L2], c->ev[EV_K3_START], c->ev[EV_K3_END]);
+    cudaEventElapsedTime(&c->stage_ms[ST_KERNELS], c->ev[EV_MAP_START], c->ev[EV_K3_END]); /* incl. host gaps */
     c->diag[MM_DIAG_LONG_FRAGMENTS] += c->n_long;
     c->batch_mapped = true;
     return MM_OK;
@@ -769,30 +781,23 @@ int mm_ctx_create(int device, const mm_params *params, mm_ctx **out)
   if (prop.major != 9 || prop.minor != 0)
     return fail(nullptr, MM_ENODEVICE, "device %d is sm_%d%d; this build is sm_90a only", device, prop.major, prop.minor);
   if (int rc = mm_params_check(params)) return rc;
-  mm_ctx *c = new mm_ctx();
+  std::unique_ptr<mm_ctx> c(new mm_ctx()); /* a failure below releases what was made so far (~mm_ctx) */
   c->device = device;
   c->params = *params;
   c->sm_count = prop.multiProcessorCount;
-  if (cudaSetDevice(device) != cudaSuccess || cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess) {
-    delete c;
+  if (cudaSetDevice(device) != cudaSuccess || cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess)
     return fail(nullptr, MM_ECUDA, "cannot create stream");
-  }
-  for (auto &ev : c->ev) cudaEventCreate(&ev);
-  cudaEventCreate(&c->ev_pack);
-  if (cudaHostAlloc((void **)&c->h_pub, 256, cudaHostAllocMapped | cudaHostAllocPortable) != cudaSuccess) {
-    cudaStreamDestroy(c->stream);
-    delete c;
+  for (cudaEvent_t &ev : c->ev)
+    if (cudaEventCreate(&ev) != cudaSuccess) return fail(nullptr, MM_ECUDA, "cannot create the stage timing events");
+  if (cudaHostAlloc((void **)&c->h_pub, 256, cudaHostAllocMapped | cudaHostAllocPortable) != cudaSuccess)
     return fail(nullptr, MM_ENOMEM, "cannot allocate the pinned counter page");
-  }
-  if (const char *g = getenv("MM_BLOCKING_WAIT")) {
-    if (g[0] == '1' && cudaEventCreateWithFlags(&c->ev_wait, cudaEventBlockingSync | cudaEventDisableTiming) == cudaSuccess)
-      c->blocking_wait = true;
-  }
+  if (const char *g = getenv("MM_BLOCKING_WAIT"))
+    if (g[0] == '1' && mm_ctx_set_wait_mode(c.get(), 1)) return fail(nullptr, MM_ECUDA, "%s", c->error.c_str());
   if (const char *g = getenv("MM_L2_GENERAL")) c->l2_mode = (g[0] == '1') ? 0 : 1; /* test hook: general kernel only */
   if (const char *g = getenv("MM_SKETCH_TABLE")) c->sk_mode = (g[0] == '1') ? 1 : 0; /* test hook: general sketch kernel only */
   if (const char *g = getenv("MM_L1_CTA")) c->l1_warp = (g[0] == '1') ? 0 : 1; /* test hook: general L1 path only */
   if (params->sketch_size > 1000) c->l2_mode = 0; /* the stream kernel packs its counters in 11 bits */
-  *out = c;
+  *out = c.release();
   return MM_OK;
 }
 
@@ -801,10 +806,6 @@ int mm_ctx_destroy(mm_ctx *c)
   if (!c) return MM_OK;
   cudaSetDevice(c->device);
   cudaStreamSynchronize(c->stream);
-  for (auto &ev : c->ev) cudaEventDestroy(ev);
-  if (c->h_pub) cudaFreeHost(c->h_pub);
-  if (c->ev_wait) cudaEventDestroy(c->ev_wait);
-  cudaStreamDestroy(c->stream);
   delete c;
   return MM_OK;
 }
@@ -950,7 +951,7 @@ static int batch_upload_any(mm_ctx *c, const void *bases, uint64_t n_bases, cons
   int rc = upload_batch(c, bases, n_bases, segs, n_segs, packed);
   if (rc) return rc;
   CU(c, wait_stream(c));
-  cudaEventElapsedTime(&c->stage_ms[3], c->ev[6], c->ev[7]);
+  cudaEventElapsedTime(&c->stage_ms[ST_H2D], c->ev[EV_UPLOAD_START], c->ev[EV_UPLOAD_END]);
   return MM_OK;
 }
 int mm_batch_upload(mm_ctx *c, const char *bases, uint64_t n_bases, const mm_segment *segs, uint64_t n_segs)
@@ -978,13 +979,13 @@ int mm_batch_fetch(mm_ctx *c, mm_segment_result *seg_results, mm_l1_candidate *c
   if (!c || !c->batch_mapped) return fail(c, MM_ESTATE, "no mapped batch");
   if (cand_cap < c->n_cands || loci_cap < c->n_loci) return fail(c, MM_ECAPACITY, "output capacity too small");
   CU(c, cudaSetDevice(c->device));
-  CU(c, cudaEventRecord(c->ev[5], c->stream));
+  CU(c, cudaEventRecord(c->ev[EV_FETCH_START], c->stream));
   if (seg_results) CU(c, cudaMemcpyAsync(seg_results, c->d_seg_res.get(), c->n_segs * sizeof(mm_segment_result), cudaMemcpyDeviceToHost, c->stream));
   if (cands && c->n_cands) CU(c, cudaMemcpyAsync(cands, c->d_cands.get(), c->n_cands * sizeof(mm_l1_candidate), cudaMemcpyDeviceToHost, c->stream));
   if (loci && c->n_loci) CU(c, cudaMemcpyAsync(loci, c->d_loci.get(), c->n_loci * sizeof(mm_l2_locus), cudaMemcpyDeviceToHost, c->stream));
-  CU(c, cudaEventRecord(c->ev[6], c->stream));
+  CU(c, cudaEventRecord(c->ev[EV_FETCH_END], c->stream));
   CU(c, wait_stream(c));
-  cudaEventElapsedTime(&c->stage_ms[4], c->ev[5], c->ev[6]);
+  cudaEventElapsedTime(&c->stage_ms[ST_D2H], c->ev[EV_FETCH_START], c->ev[EV_FETCH_END]);
   return MM_OK;
 }
 
@@ -1022,16 +1023,14 @@ int mm_sketch_segments(mm_ctx *c, const char *bases, uint64_t n_bases, const mm_
   int rc = upload_batch(c, bases, n_bases, segs, n_segs, 0);
   if (rc) return rc;
   if ((rc = launch_pack_if_ascii(c))) return rc;
-  ZERO_WORDS(c, c->d_counters.get(), 16);
-  CU(c, cudaEventRecord(c->ev[0], c->stream));
+  ZERO_WORDS(c, c->d_counters.get(), sizeof(mm_counters) / 4);
+  CU(c, cudaEventRecord(c->ev[EV_K1_START], c->stream));
   if ((rc = launch_sketch_all(c, false))) return rc; /* sketches only: no index needed */
-  CU(c, cudaEventRecord(c->ev[1], c->stream));
-  CU(c, cudaStreamSynchronize(c->stream));
-  cudaEventElapsedTime(&c->stage_ms[0], c->ev[0], c->ev[1]);
-  {
-    uint32_t h9 = 0;
-    if (cudaMemcpy(&h9, c->d_counters.get() + 9, 4, cudaMemcpyDeviceToHost) == cudaSuccess) c->diag[MM_DIAG_SKETCH_GENERAL_SEGMENTS] += h9;
-  }
+  CU(c, cudaEventRecord(c->ev[EV_K1_END], c->stream));
+  mm_counters cnt;
+  RD(c, c->d_counters.get(), &cnt);
+  cudaEventElapsedTime(&c->stage_ms[ST_SKETCH], c->ev[EV_K1_START], c->ev[EV_K1_END]);
+  c->diag[MM_DIAG_SKETCH_GENERAL_SEGMENTS] += cnt.sketch_rejects;
   c->diag[MM_DIAG_LONG_FRAGMENTS] += c->n_long;
   c->batch_mapped = true; /* sketches only; fetch_sketch reads sketch_size == raw count */
   rc = mm_batch_fetch_sketch(c, out, out_count);
@@ -1047,7 +1046,7 @@ static int map_segments_any(mm_ctx *c, const void *bases, uint64_t n_bases, cons
   int rc = upload_batch(c, bases, n_bases, segs, n_segs, packed);
   if (rc) return rc;
   if ((rc = run_pipeline(c))) return rc;
-  cudaEventElapsedTime(&c->stage_ms[3], c->ev[6], c->ev[7]);
+  cudaEventElapsedTime(&c->stage_ms[ST_H2D], c->ev[EV_UPLOAD_START], c->ev[EV_UPLOAD_END]);
   *n_candidates = c->n_cands;
   *n_loci = c->n_loci;
   if (cand_cap < c->n_cands || loci_cap < c->n_loci) return fail(c, MM_ECAPACITY, "need %llu candidates, %llu loci", (unsigned long long)c->n_cands, (unsigned long long)c->n_loci);
@@ -1090,7 +1089,7 @@ int mm_ctx_set_phase_hook(mm_ctx *c, mm_phase_hook hook, void *user)
 int mm_last_stage_ms(const mm_ctx *c, float ms[8])
 {
   if (!c || !ms) return MM_EINVAL;
-  for (int i = 0; i < 8; i++) ms[i] = c->stage_ms[i];
+  for (int i = 0; i < N_STAGE_SLOTS; i++) ms[i] = c->stage_ms[i];
   return MM_OK;
 }
 int mm_last_pack_ms(const mm_ctx *c, float *ms)

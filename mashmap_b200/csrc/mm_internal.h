@@ -19,6 +19,7 @@
 #define MM_INTERNAL_H
 
 #include <cuda_runtime.h>
+#include <stddef.h>
 #include <stdint.h>
 #include "../../include/mashmap_b200.h"
 #include "mm_hash.h"
@@ -69,6 +70,26 @@ struct mm_dev_index {
   int32_t n_min_hits;
 };
 
+/* The per-batch counters in device memory: written by the kernels, zeroed by the host before K1 and read back by it as
+ * one block (k_publish, mm_capi.cu: one word per lane of one warp). */
+struct mm_counters {
+  uint32_t cands_needed;        /* K2: candidates of the batch, including those past cand_cap                          */
+  uint32_t l2_overflow;         /* K3: MM_L2_LOCI_OVERFLOW or MM_L2_LIVE_SET_OVERFLOW (the latter wins), 0 = none       */
+  uint32_t scratch_overflow;    /* K2: the scratch pool is exhausted (1)                                               */
+  uint32_t cand_overflow;       /* K2: candidates past cand_cap were dropped (1)                                       */
+  unsigned long long pool_used; /* K2: bump pointer into the scratch pool, in u64 elements                              */
+  uint32_t loci_needed;         /* K3 (k_l2, k_l2_long): end of the loci appended; the host sets where they start      */
+  uint32_t l2_redo;             /* K3 (k_l2_scan): candidates flagged for the general kernel                           */
+  uint32_t l1_cta_segments;     /* K2: segments the warp path handed to the CTA path (the CTA path's work count)       */
+  uint32_t sketch_rejects;      /* K1: segments the fast sketch kernel handed to the general one (its work count)      */
+  uint32_t _unused[6];
+};
+static_assert(offsetof(mm_counters, pool_used) == 16 && offsetof(mm_counters, pool_used) % 8 == 0,
+              "the pool bump pointer is one 8-byte-aligned u64 atomic");
+static_assert(sizeof(mm_counters) <= 16 * 4, "the counter block is read back by one warp, one word per lane");
+constexpr uint32_t MM_L2_LOCI_OVERFLOW = 1;     /* the locus buffer is too small: grow it and run again */
+constexpr uint32_t MM_L2_LIVE_SET_OVERFLOW = 2; /* more live index entries than the general kernel holds: an error */
+
 /* Per-batch device buffers. */
 struct mm_dev_batch {
   const uint8_t *bases;       /* ASCII bases (only when the batch came in as text), padded by 256 bytes          */
@@ -85,16 +106,12 @@ struct mm_dev_batch {
   int32_t *sk_votes;          /* optional (nullptr = not written; general sketch kernel only): the vote SUM of every     */
                               /* sketch slot, which the merge of a long fragment's pieces needs (sk_strand: its sign)   */
   mm_segment_result *seg_res;
-  uint32_t *sk_reject;        /* work list of the general sketch kernel: segments the fast kernel handed over (count in counters[9]) */
+  uint32_t *sk_reject;        /* work list of the general sketch kernel: segments the fast kernel handed over          */
   mm_l1_candidate *cands;
   uint32_t cand_cap;
   mm_l2_locus *loci;
   uint32_t loci_cap;
-  uint32_t *counters;         /* [0] candidates needed, [1] loci overflow (1) / live-set overflow (2), */
-                              /* [2] scratch overflow, [3] candidate overflow,                         */
-                              /* [4..5] u64 bump pointer into the scratch pool, [6] loci needed,       */
-                              /* [7] L2 candidates to redo, [8] segments handed to the general L1 path, */
-                              /* [9] segments handed to the general sketch kernel                     */
+  mm_counters *counters;
   uint64_t *scratch;          /* global-memory work area for segments with many interval points:       */
                               /* one slice per CTA of the L1 grid, then a bump-allocated pool          */
   uint64_t scratch_slice;     /* u64 elements per CTA slice                                            */

@@ -521,8 +521,8 @@ __device__ bool l1_segment(const mm_params &prm, const mm_dev_index &ix, const m
       keys = b.scratch + (size_t)scratch_slot * b.scratch_slice; /* this CTA's slice, reused per segment */
     } else {
       if (tid == 0) {
-        const unsigned long long at = b.scratch_pool_off + atomicAdd((unsigned long long *)(b.counters + 4), need);
-        if (at + need > b.scratch_cap) { sh.fail = 1; atomicExch(b.counters + 2, 1u); }
+        const unsigned long long at = b.scratch_pool_off + atomicAdd(&b.counters->pool_used, need);
+        if (at + need > b.scratch_cap) { sh.fail = 1; atomicExch(&b.counters->scratch_overflow, 1u); }
         sh.scratch_base = at;
       }
       grp<NT>::sync();
@@ -642,8 +642,8 @@ __device__ bool l1_segment(const mm_params &prm, const mm_dev_index &ix, const m
       if (tid == 0) {
         uint32_t basec = 0;
         if (n_out > 0) {
-          basec = atomicAdd(b.counters + 0, n_out);
-          if ((unsigned long long)basec + n_out > b.cand_cap) atomicExch(b.counters + 3, 1u);
+          basec = atomicAdd(&b.counters->cands_needed, n_out);
+          if ((unsigned long long)basec + n_out > b.cand_cap) atomicExch(&b.counters->cand_overflow, 1u);
         }
         sh.cand_base = basec;
       }
@@ -712,7 +712,7 @@ k_l1_warp(const mm_params prm, const mm_dev_index ix, const mm_dev_batch b, uint
   for (uint32_t seg = blockIdx.x * L1_WARPS_PER_CTA + wid; seg < b.n_segs; seg += gridDim.x * L1_WARPS_PER_CTA) {
     __syncwarp();
     const bool done = l1_segment<32, L1_LOCAL_CANDS_WARP, L1_WARP_POINTS>(prm, ix, b, seg, hits, keys, copn, head, ginfo, sh, 0);
-    if (!done && lane == 0) slow_list[atomicAdd(b.counters + 8, 1u)] = seg;
+    if (!done && lane == 0) slow_list[atomicAdd(&b.counters->l1_cta_segments, 1u)] = seg;
   }
 }
 
@@ -728,7 +728,7 @@ k_l1_cta(const mm_params prm, const mm_dev_index ix, const mm_dev_batch b, const
   uint32_t *shead = scopn + L1_CTA_POINTS;
   uint32_t *sginfo = shead + L1_CTA_POINTS;
   __shared__ l1_shared<128, L1_LOCAL_CANDS_CTA> sh;
-  const uint32_t n_work = slow_list ? b.counters[8] : b.n_segs;
+  const uint32_t n_work = slow_list ? b.counters->l1_cta_segments : b.n_segs;
   for (uint32_t w = blockIdx.x; w < n_work; w += gridDim.x) {
     const uint32_t seg = slow_list ? slow_list[w] : w;
     l1_segment<128, L1_LOCAL_CANDS_CTA, L1_CTA_POINTS>(prm, ix, b, seg, hits, skeys, scopn, shead, sginfo, sh, blockIdx.x);
@@ -773,7 +773,7 @@ uint32_t mm_l1_grid_size(const mm_params &p, int sm_count)
   return (uint32_t)sm_count * (uint32_t)occ;
 }
 
-/* slow_list: device array of n_segs u32 (work list of the general path); counters[8] must be 0 */
+/* slow_list: device array of n_segs u32 (work list of the general path); b.counters->l1_cta_segments must be 0 */
 cudaError_t mm_launch_l1(const mm_params &p, const mm_dev_index &ix, const mm_dev_batch &b, cudaStream_t st, int sm_count,
                          uint32_t *slow_list, int use_warp_path, int *n_launched)
 {
@@ -797,7 +797,7 @@ cudaError_t mm_launch_l1(const mm_params &p, const mm_dev_index &ix, const mm_de
   k_l1_warp<<<wgrid, L1_WARPS_PER_CTA * 32, wsmem, st>>>(p, ix, b, slow_list);
   e = cudaGetLastError();
   if (e != cudaSuccess) return e;
-  /* the general path reads its work count from counters[8] on the device: no host round trip in between */
+  /* the general path reads its work count from b.counters->l1_cta_segments on the device: no host round trip in between */
   k_l1_cta<<<grid, 128, mm_l1_cta_smem(p.sketch_size), st>>>(p, ix, b, slow_list);
   if (n_launched) *n_launched = 2;
   return cudaGetLastError();

@@ -348,14 +348,14 @@ k_l2(const mm_params prm, const mm_dev_index ix, const mm_dev_batch b, uint32_t 
     int cnt = l2_scan(prm, ix, cd, m, n, live_cap, stage, L2_STAGE_LOCI);
     uint32_t first = 0;
     if (cnt < 0) {
-      if (lane == 0) atomicExch(b.counters + 1, 2u); /* live-set overflow: reported as an error */
+      if (lane == 0) atomicExch(&b.counters->l2_overflow, MM_L2_LIVE_SET_OVERFLOW);
       cnt = 0;
     } else if (cnt > 0) {
-      if (lane == 0) first = atomicAdd(b.counters + 6, (uint32_t)cnt);
+      if (lane == 0) first = atomicAdd(&b.counters->loci_needed, (uint32_t)cnt);
       first = __shfl_sync(0xffffffffu, first, 0);
       const bool fits = (unsigned long long)first + (uint32_t)cnt <= b.loci_cap;
       if (!fits) {
-        if (lane == 0) atomicMax(b.counters + 1, 1u);
+        if (lane == 0) atomicMax(&b.counters->l2_overflow, MM_L2_LOCI_OVERFLOW);
       } else if (cnt <= L2_STAGE_LOCI) {
         __syncwarp();
         for (int k = lane; k < cnt; k += 32) b.loci[first + k] = stage[k];
@@ -616,10 +616,10 @@ k_l2_long(const mm_params prm, const mm_dev_index ix, const mm_dev_batch b, uint
     int cnt = l2_scan_long(prm, ix, cd, m, n, window_len, lt, stage, L2_STAGE_LOCI);
     uint32_t first = 0;
     if (cnt > 0) {
-      if (lane == 0) first = atomicAdd(b.counters + 6, (uint32_t)cnt);
+      if (lane == 0) first = atomicAdd(&b.counters->loci_needed, (uint32_t)cnt);
       first = __shfl_sync(0xffffffffu, first, 0);
       if ((unsigned long long)first + (uint32_t)cnt > b.loci_cap) {
-        if (lane == 0) atomicMax(b.counters + 1, 1u);
+        if (lane == 0) atomicMax(&b.counters->l2_overflow, MM_L2_LOCI_OVERFLOW);
       } else if (cnt <= L2_STAGE_LOCI) {
         __syncwarp();
         for (int k = lane; k < cnt; k += 32) b.loci[first + k] = stage[k];
@@ -703,7 +703,7 @@ cudaError_t mm_launch_l2_long_ranges(const mm_params &p, const mm_dev_index &ix,
   return cub::DeviceScan::ExclusiveSum(scan_tmp, scan_tmp_bytes, table_off, table_off, (int)n_cands + 1, st);
 }
 
-/* the windowed scan of every candidate whose table_off range is not empty; loci appended at counters[6] */
+/* the windowed scan of every candidate whose table_off range is not empty; loci appended at b.counters->loci_needed */
 cudaError_t mm_launch_l2_long(const mm_params &p, const mm_dev_index &ix, const mm_dev_batch &b, uint32_t n_cands,
                               const uint64_t *table_off, uint64_t *table, cudaStream_t st, int sm_count)
 {

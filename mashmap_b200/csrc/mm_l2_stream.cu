@@ -405,7 +405,7 @@ k_l2_scan(const mm_params prm, const mm_dev_index ix, const mm_dev_batch b, uint
       }
       if (has_back) { store(n_loci, back); n_loci++; }
       if (n_loci > LPC || sv_overflow) {
-        atomicAdd(b.counters + 7, 1u); /* redo by the general kernel */
+        atomicAdd(&b.counters->l2_redo, 1u); /* redo by the general kernel */
         b.cands[c].first_locus = 0;
         b.cands[c].n_loci = 0xFFFFFFFFu;
       } else {

@@ -1037,16 +1037,16 @@ cudaError_t launch_k(const mm_params &p, const mm_dev_index &ix, const mm_dev_ba
   uint32_t fgrid = (uint32_t)sm_count * (uint32_t)focc; /* persistent: a whole number of CTAs per SM */
   if (fgrid > b.n_segs) fgrid = b.n_segs;
   k_sketch<K><<<fgrid, SK_THREADS, FL.total, st>>>(b.packed, b.segs, b.n_segs, p.sketch_size, p.seg_length, NC, CAP, b.sk_hash, b.sk_pos,
-                                                   b.sk_strand, b.seg_res, b.sk_reject, b.counters + 9, ix.tab, ix.tab_log2,
-                                                   b.sk_val);
+                                                   b.sk_strand, b.seg_res, b.sk_reject, &b.counters->sketch_rejects, ix.tab,
+                                                   ix.tab_log2, b.sk_val);
   e = cudaGetLastError();
   if (e != cudaSuccess) return e;
   /* the rejects: the count is read on the device; a grid of one CTA per SM is enough for a fraction of a per cent */
   uint32_t rgrid = (uint32_t)sm_count;
   if (rgrid > b.n_segs) rgrid = b.n_segs;
-  k_sketch_table<K><<<rgrid, SK_THREADS, smem, st>>>(b.packed, b.segs, b.n_segs, b.sk_reject, b.counters + 9, p.sketch_size, p.seg_length,
-                                                     C, CAP, b.sk_hash, b.sk_pos, b.sk_strand, b.sk_votes, b.seg_res, ix.tab,
-                                                     ix.tab_log2, b.sk_val);
+  k_sketch_table<K><<<rgrid, SK_THREADS, smem, st>>>(b.packed, b.segs, b.n_segs, b.sk_reject, &b.counters->sketch_rejects,
+                                                     p.sketch_size, p.seg_length, C, CAP, b.sk_hash, b.sk_pos, b.sk_strand,
+                                                     b.sk_votes, b.seg_res, ix.tab, ix.tab_log2, b.sk_val);
   return cudaGetLastError();
 }
 
@@ -1226,7 +1226,7 @@ cudaError_t mm_launch_pack_bases(const uint8_t *ascii, uint8_t *packed, uint64_t
 }
 
 /* mode 0: fast kernel + general kernel over its rejects (2 launches); mode 1: general kernel over everything (1 launch).
- * b.counters[9] must be 0 and b.sk_reject must hold n_segs entries. */
+ * b.counters->sketch_rejects must be 0 and b.sk_reject must hold n_segs entries. */
 cudaError_t mm_launch_sketch(const mm_params &p, const mm_dev_index &ix, const mm_dev_batch &b, cudaStream_t st, int sm_count,
                              int mode)
 {
