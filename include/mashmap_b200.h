@@ -177,6 +177,26 @@ typedef struct mm_index_stats {
 int mm_index_build(mm_ctx *ctx, const char *seqs, int seqs_on_device, const uint64_t *contig_offsets, int32_t n_contigs,
                    const int32_t *contig_name_id, const int32_t *contig_group, float kmer_pct_threshold, int keep_lookup,
                    mm_index_stats *stats);
+/* A reference index sharded by contig (DESIGN.md, "Index shards"): each shard is one context's image of a contiguous range
+ * of contigs, built in two passes so that the frequent seeds are those of the WHOLE reference (computeFreqHist counts a
+ * hash's interval points over all contigs, winSketch.hpp:410-453).
+ * Pass 1, mm_index_key_counts: the shard's distinct hashes, ascending, and each one's number of interval points
+ * (contig_offsets as mm_index_build's, for the shard's contigs only). keys[cap], counts[cap]; on MM_ECAPACITY *n_keys is
+ * the count and the result stays in the context: call again with seqs == NULL and room to take it. The device arrays
+ * are freed when the result is taken or the context is destroyed. stats (may be NULL): filled by the call that builds
+ * (n_minmers_before_filter, n_keys, n_points and the timings; nothing is filtered).
+ * Pass 2, mm_index_build_shard: the image of contigs [first_contig, first_contig + n_shard_contigs) of a reference of
+ * n_contigs (seqs / contig_offsets: the shard's contigs only; contig_len / contig_name_id / contig_group: all n_contigs).
+ * Its records carry GLOBAL seqIds and its contig tables cover every contig. freq_hashes[n_freq] (strictly ascending) are
+ * the reference's frequent hashes: exactly those are flagged and dropped, and those the shard does not contain are added
+ * to its lookup keys (after its own keys, mm_index_download) as frequent keys with no points, so that every shard
+ * removes the same hashes from a query sketch (computeMap.hpp:834-839). Threshold tables: mm_tables_upload. */
+int mm_index_key_counts(mm_ctx *ctx, const char *seqs, int seqs_on_device, const uint64_t *contig_offsets, int32_t n_contigs,
+                        uint64_t *keys, uint32_t *counts, uint64_t cap, uint64_t *n_keys, mm_index_stats *stats);
+int mm_index_build_shard(mm_ctx *ctx, const char *seqs, int seqs_on_device, const uint64_t *contig_offsets, int32_t first_contig,
+                         int32_t n_shard_contigs, const int32_t *contig_len, const int32_t *contig_name_id,
+                         const int32_t *contig_group, int32_t n_contigs, const uint64_t *freq_hashes, uint64_t n_freq,
+                         int keep_lookup, mm_index_stats *stats);
 /* Host copies of the index mm_index_build left on the device, in mm_index_upload's argument formats (any pointer may be
  * NULL; the lookup arrays need keep_lookup). Sizes: mm_index_stats. */
 int mm_index_download(mm_ctx *ctx, mm_minmer *minmer_index, uint64_t *keys, uint64_t *offsets, mm_ipoint *points,
@@ -241,6 +261,20 @@ int mm_batch_upload(mm_ctx *ctx, const char *bases, uint64_t n_bases,
 int mm_batch_upload_packed(mm_ctx *ctx, const uint8_t *nibbles, uint64_t n_bases,
                            const mm_segment *segments, uint64_t n_segments);
 int mm_map_resident(mm_ctx *ctx, uint64_t *n_candidates, uint64_t *n_loci);
+/* mm_map_resident on one shard of a contig-sharded index, in two phases. Without skip_prefix one
+ * computeL1CandidateRegions call sweeps every contig: its bestIntersectionSize (sweep #1) decides the early return and
+ * the hypergeometric raise of minimumHits (computeMap.hpp:982-998), so over a shard it must be the best over ALL shards;
+ * and its sweep #2 tests each position group when it reaches the next one (:1026-1027), so a shard's last group is tested
+ * when a later shard has points of the fragment (it matters for fragments longer than a segment, whose overlap does not
+ * drop to zero at a contig's end). Phase 1 (K1 and K2's first sweep) writes best[n_segs], each segment's uncapped best
+ * over this shard's points (> 0 iff the shard has points of it), and emits nothing; the sketches stay resident. Phase 2
+ * (K2, K3) maps the batch as mm_map_resident does, with the caller's best[] (the maximum over the shards) in place of its
+ * own and points_after[n_segs] != 0 where a later shard has points of the segment. With skip_prefix every reference
+ * group is swept on its own and never spans two shards whose cuts fall between groups: mm_map_resident is exact there,
+ * and phase 1 refuses (MM_EINVAL). Fetch with mm_batch_fetch. */
+int mm_map_resident_l1_best(mm_ctx *ctx, int32_t *best);
+int mm_map_resident_with_best(mm_ctx *ctx, const int32_t *best, const uint8_t *points_after, uint64_t *n_candidates,
+                              uint64_t *n_loci);
 int mm_batch_fetch(mm_ctx *ctx, mm_segment_result *seg_results,
                    mm_l1_candidate *candidates, uint64_t cand_cap,
                    mm_l2_locus *loci, uint64_t loci_cap);

@@ -105,6 +105,10 @@ def lib():
         L.mm_map_segments_packed.argtypes = [vp, vp, u64, vp, u64, vp, vp, u64, C.POINTER(u64), vp, u64, C.POINTER(u64)]
         L.mm_last_pack_ms.argtypes = [vp, C.POINTER(C.c_float)]
         L.mm_map_resident.argtypes = [vp, C.POINTER(u64), C.POINTER(u64)]
+        L.mm_map_resident_l1_best.argtypes = [vp, vp]
+        L.mm_map_resident_with_best.argtypes = [vp, vp, vp, C.POINTER(u64), C.POINTER(u64)]
+        L.mm_index_key_counts.argtypes = [vp, vp, C.c_int, vp, i32, vp, vp, u64, C.POINTER(u64), C.POINTER(IndexStats)]
+        L.mm_index_build_shard.argtypes = [vp, vp, C.c_int, vp, i32, i32, vp, vp, vp, i32, vp, u64, C.c_int, C.POINTER(IndexStats)]
         L.mm_batch_fetch.argtypes = [vp, vp, vp, u64, vp, u64]
         L.mm_batch_fetch_sketch.argtypes = [vp, vp, vp]
         L.mm_last_stage_ms.argtypes = [vp, C.POINTER(C.c_float * 8)]
@@ -119,6 +123,7 @@ EXPORTED_SYMBOLS = [
     "mm_tables_upload", "mm_index_build", "mm_index_download", "mm_index_blob", "mm_index_blob_alloc", "mm_index_adopt_blob", "mm_ctx_share_index", "mm_sketch_segments",
     "mm_map_segments", "mm_map_segments_packed", "mm_batch_upload", "mm_batch_upload_packed", "mm_last_pack_ms", "mm_map_resident", "mm_batch_fetch", "mm_batch_fetch_sketch",
     "mm_last_stage_ms", "mm_ctx_set_phase_hook", "mm_ctx_set_wait_mode", "mm_params_check", "mm_host_alloc", "mm_host_free",
+    "mm_index_key_counts", "mm_index_build_shard", "mm_map_resident_l1_best", "mm_map_resident_with_best",
 ]
 
 
@@ -265,6 +270,36 @@ class Context:
         self._index_stats = st.as_dict()
         return self._index_stats
 
+    def index_key_counts(self, seqs, contig_offsets):
+        """pass 1 of a contig-sharded index (mm_index_key_counts): (distinct hashes ascending, their interval-point counts,
+        statistics) of the contigs seqs / contig_offsets"""
+        a = np.ascontiguousarray(seqs, dtype=np.uint8)
+        offs = _c(contig_offsets, np.uint64)
+        n, st = C.c_uint64(), IndexStats()
+        rc = self._L.mm_index_key_counts(self._h, _ptr(a), 0, _ptr(offs), len(offs) - 1, None, None, 0, C.byref(n), C.byref(st))
+        keys, counts = np.zeros(n.value, dtype=np.uint64), np.zeros(n.value, dtype=np.uint32)
+        if rc == MM_ECAPACITY:
+            rc = self._L.mm_index_key_counts(self._h, None, 0, None, 0, _ptr(keys), _ptr(counts), n.value, C.byref(n), None)
+        self._check(rc)
+        return keys, counts, st.as_dict()
+
+    def index_build_shard(self, seqs, contig_offsets, first_contig, contig_len, freq_hashes, contig_name_id=None,
+                          contig_group=None, keep_lookup=False):
+        """pass 2 (mm_index_build_shard): the image of contigs [first_contig, first_contig + len(contig_offsets) - 1) of a
+        reference whose contig lengths are contig_len (all of them), with exactly freq_hashes (ascending) frequent"""
+        a = np.ascontiguousarray(seqs, dtype=np.uint8)
+        offs = _c(contig_offsets, np.uint64)
+        cl = _c(contig_len, np.int32)
+        fr = _c(freq_hashes, np.uint64)
+        cn = None if contig_name_id is None else _c(contig_name_id, np.int32)
+        cg = None if contig_group is None else _c(contig_group, np.int32)
+        st = IndexStats()
+        self._check(self._L.mm_index_build_shard(self._h, _ptr(a), 0, _ptr(offs), int(first_contig), len(offs) - 1, _ptr(cl),
+                                                 _ptr(cn), _ptr(cg), len(cl), _ptr(fr), len(fr), 1 if keep_lookup else 0,
+                                                 C.byref(st)))
+        self._index_stats = st.as_dict()
+        return self._index_stats
+
     def index_download(self):
         """host copies of the device-built index (needs keep_lookup=True): (minmers, keys, offsets, points, is_freq)"""
         st = self._index_stats
@@ -374,6 +409,22 @@ class Context:
     def map_resident(self):
         nc, nl = C.c_uint64(), C.c_uint64()
         self._check(self._L.mm_map_resident(self._h, C.byref(nc), C.byref(nl)))
+        self._nc, self._nl = nc.value, nl.value
+        return nc.value, nl.value
+
+    def map_resident_l1_best(self):
+        """phase 1 on a shard (mm_map_resident_l1_best): each segment's best intersection over this shard"""
+        best = np.zeros(max(self._n_segs, 1), dtype=np.int32)
+        self._check(self._L.mm_map_resident_l1_best(self._h, _ptr(best)))
+        return best[: self._n_segs]
+
+    def map_resident_with_best(self, best, points_after):
+        """phase 2 (mm_map_resident_with_best): map with the best over all shards; points_after[seg]: a later shard has
+        points of the segment"""
+        b = _c(best, np.int32)
+        a = _c(points_after, np.uint8)
+        nc, nl = C.c_uint64(), C.c_uint64()
+        self._check(self._L.mm_map_resident_with_best(self._h, _ptr(b), _ptr(a), C.byref(nc), C.byref(nl)))
         self._nc, self._nl = nc.value, nl.value
         return nc.value, nl.value
 

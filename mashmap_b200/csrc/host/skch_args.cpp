@@ -33,7 +33,7 @@ const OptDef kOptions[] = {
     {"reportPercentage", nullptr, false},
     // B200-specific
     {"device", nullptr, true}, {"devices", nullptr, true}, {"hostIndex", nullptr, false}, {"batchBases", nullptr, true}, {"subBatchBases", nullptr, true},
-    {"align", nullptr, false}, {"alignMaxLen", nullptr, true},
+    {"align", nullptr, false}, {"alignMaxLen", nullptr, true}, {"indexShards", nullptr, true},
 };
 
 [[noreturn]] void usage_error(const std::string &msg)
@@ -82,6 +82,7 @@ void printCmdOptions(const Parameters &p)
   std::cerr << "[mashmap-b200] Mapping output file = " << p.outFileName << std::endl;
   std::cerr << "[mashmap-b200] Filter mode = " << p.filterMode << " (1 = map, 2 = one-to-one, 3 = none)" << std::endl;
   std::cerr << "[mashmap-b200] Host threads = " << p.threads << ", CUDA device = " << p.device << std::endl;
+  if (p.index_shards > 1) std::cerr << "[mashmap-b200] Index shards = " << p.index_shards << std::endl;
   if (p.align)
     std::cerr << "[mashmap-b200] Alignment = NM:i and cg:Z from edlib NW over each mapping's region, regions up to "
               << p.align_max_len << " bp" << std::endl;
@@ -113,7 +114,9 @@ void parseandSave(int argc, char **argv, Parameters &parameters)
   if (found("version")) { std::cerr << fixed::VERSION << std::endl; exit(0); }
   if (found("help")) {
     std::cerr << "mashmap-b200 -r ref.fa -q seq.fq [OPTIONS]   (options as in MashMap v3.1.3, plus --device N | --devices 0-7, --batchBases N,\n"
-                 "    --align [--alignMaxLen N, default 100000]: append NM:i and cg:Z (edlib NW over each mapping's region, on the GPU))" << std::endl;
+                 "    --align [--alignMaxLen N, default 100000]: append NM:i and cg:Z (edlib NW over each mapping's region, on the GPU),\n"
+                 "    --indexShards N [default 1]: cut the reference index by contig into N device images (shard i on the i-th device of\n"
+                 "    --devices, round robin), for references whose index does not fit one GPU; the output is the same)" << std::endl;
     exit(0);
   }
   parameters.align = found("align");
@@ -262,6 +265,20 @@ void parseandSave(int argc, char **argv, Parameters &parameters)
     }
     if (parameters.devices.empty()) usage_error("ERROR, --devices needs a list such as 0-7 or 0,2,5");
     parameters.device = parameters.devices[0];
+  }
+  if (found("indexShards")) {
+    const std::string &v = opt["indexShards"];
+    if (v.empty() || v.size() > 9 || v.find_first_not_of("0123456789") != std::string::npos || std::stoll(v) < 1)
+      usage_error("ERROR, --indexShards needs a whole number of shards >= 1, not '" + v + "'");
+    parameters.index_shards = (int)std::stoll(v);
+    if (parameters.index_shards > 1) {
+      if (parameters.host_index || !parameters.saveIndexFilename.empty() || !parameters.loadIndexFilename.empty())
+        usage_error("ERROR, --indexShards builds every shard on its device: it cannot be combined with --hostIndex, --saveIndex or "
+                    "--loadIndex, which keep one index on the host");
+      if (parameters.devices.size() > (size_t)parameters.index_shards)
+        usage_error("ERROR, --indexShards " + v + " with " + std::to_string(parameters.devices.size()) +
+                    " devices: every device must hold a shard (read-parallel copies of a sharded index are not supported)");
+    }
   }
   if (found("batchBases")) parameters.batch_bases = to<uint64_t>(opt["batchBases"]);
   if (found("subBatchBases")) parameters.sub_batch_bases = to<uint64_t>(opt["subBatchBases"]);

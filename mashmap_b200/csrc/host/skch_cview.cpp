@@ -757,4 +757,31 @@ int skch_format_selftest(int64_t n, uint64_t seed)
   return bad;
 }
 
+/* --indexShards for the CPU tests: BatchMapper::planShards (first[n_shards + 1]; returns 0, or -1 with the reason in
+ * skch_last_plan_error()) and the frequent seeds of the union of per-shard key counts (globalFrequentSeeds: writes the
+ * ascending frequent hashes to out[cap], returns their number, or -1 when cap is too small) */
+static thread_local std::string g_plan_error;
+int skch_plan_shards(const uint64_t *len, const int32_t *group, int n_contigs, int by_group, int n_shards, int32_t *first)
+{
+  std::vector<int32_t> f;
+  g_plan_error = BatchMapper::planShards(std::vector<uint64_t>(len, len + n_contigs), std::vector<int>(group, group + n_contigs),
+                                         by_group != 0, n_shards, f);
+  if (!g_plan_error.empty()) return -1;
+  std::copy(f.begin(), f.end(), first);
+  return 0;
+}
+const char *skch_last_plan_error() { return g_plan_error.c_str(); }
+int64_t skch_global_frequent_seeds(int n_shards, const uint64_t *const *keys, const uint32_t *const *counts, const uint64_t *n,
+                                   float kmer_pct_threshold, uint64_t *out, uint64_t cap, int32_t *threshold, uint64_t *n_unique)
+{
+  int t = 0;
+  const std::vector<hash_t> f = globalFrequentSeeds(std::vector<const hash_t *>(keys, keys + n_shards),
+                                                    std::vector<const uint32_t *>(counts, counts + n_shards),
+                                                    std::vector<uint64_t>(n, n + n_shards), kmer_pct_threshold, t, *n_unique);
+  *threshold = t;
+  if (f.size() > cap) return -1;
+  std::copy(f.begin(), f.end(), out);
+  return (int64_t)f.size();
+}
+
 }  // extern "C"

@@ -608,30 +608,8 @@ void Sketch::index()
       for (size_t c = 0; c < ph[p].size(); c++)
         if (ph[p][c]) hist[(int)c] += (int)ph[p][c];
   }
-  std::cerr << "[mashmap-b200::skch::Sketch::computeFreqHist] Frequency histogram of minmer interval points = ("
-            << hist.begin()->first << ", " << hist.begin()->second << ") ... (" << hist.rbegin()->first << ", "
-            << hist.rbegin()->second << ")" << std::endl;
+  freqThreshold = computeFreqThreshold(hist, (int64_t)lookupKeys.size(), param.kmer_pct_threshold);
   phase("histogram");
-  int64_t totalUniqueMinmers = lookupKeys.size();
-  int64_t minmerToIgnore = totalUniqueMinmers * param.kmer_pct_threshold / 100;
-  int64_t sum = 0;
-  for (auto it = hist.rbegin(); it != hist.rend(); it++) {
-    sum += it->second;
-    if (sum < minmerToIgnore) {
-      freqThreshold = it->first;
-    } else if (sum == minmerToIgnore) {
-      freqThreshold = it->first;
-      break;
-    } else {
-      break;
-    }
-  }
-  if (freqThreshold != std::numeric_limits<int>::max())
-    std::cerr << "[mashmap-b200::skch::Sketch::computeFreqHist] With threshold " << param.kmer_pct_threshold
-              << "%, ignore minmers occurring >= " << freqThreshold << " times during lookup." << std::endl;
-  else
-    std::cerr << "[mashmap-b200::skch::Sketch::computeFreqHist] With threshold " << param.kmer_pct_threshold
-              << "%, consider all minmers during lookup." << std::endl;
   /* 5. frequent seeds (:488-504): flag the keys, drop their entries from minmerIndex only */
   if (freqThreshold == std::numeric_limits<int>::max()) return;
   std::vector<std::vector<uint64_t>> dropped(NP); /* index positions to remove (few: 0.001 % of the keys by default) */
@@ -659,6 +637,72 @@ void Sketch::index()
     minmerIndex.resize(w);
   }
   phase("compaction");
+}
+
+int computeFreqThreshold(const std::map<int, int> &hist, int64_t totalUniqueMinmers, float kmer_pct_threshold)
+{  // winSketch.hpp:418-449
+  std::cerr << "[mashmap-b200::skch::Sketch::computeFreqHist] Frequency histogram of minmer interval points = ("
+            << hist.begin()->first << ", " << hist.begin()->second << ") ... (" << hist.rbegin()->first << ", "
+            << hist.rbegin()->second << ")" << std::endl;
+  int freqThreshold = std::numeric_limits<int>::max();
+  int64_t minmerToIgnore = totalUniqueMinmers * kmer_pct_threshold / 100;
+  int64_t sum = 0;
+  for (auto it = hist.rbegin(); it != hist.rend(); it++) {
+    sum += it->second;
+    if (sum < minmerToIgnore) {
+      freqThreshold = it->first;
+    } else if (sum == minmerToIgnore) {
+      freqThreshold = it->first;
+      break;
+    } else {
+      break;
+    }
+  }
+  if (freqThreshold != std::numeric_limits<int>::max())
+    std::cerr << "[mashmap-b200::skch::Sketch::computeFreqHist] With threshold " << kmer_pct_threshold
+              << "%, ignore minmers occurring >= " << freqThreshold << " times during lookup." << std::endl;
+  else
+    std::cerr << "[mashmap-b200::skch::Sketch::computeFreqHist] With threshold " << kmer_pct_threshold
+              << "%, consider all minmers during lookup." << std::endl;
+  return freqThreshold;
+}
+
+std::vector<hash_t> globalFrequentSeeds(const std::vector<const hash_t *> &keys, const std::vector<const uint32_t *> &counts,
+                                        const std::vector<uint64_t> &n, float kmer_pct_threshold, int &threshold, uint64_t &n_unique)
+{
+  /* one pass of an N-way merge (N is small) gives the union's distinct hashes with their summed counts */
+  const size_t N = keys.size();
+  std::vector<uint64_t> at(N, 0);
+  std::vector<std::pair<hash_t, uint32_t>> merged;
+  uint64_t total = 0;
+  for (size_t i = 0; i < N; i++) total += n[i];
+  merged.reserve(total);
+  while (true) {
+    bool any = false;
+    hash_t h = 0;
+    for (size_t i = 0; i < N; i++)
+      if (at[i] < n[i] && (!any || keys[i][at[i]] < h)) { h = keys[i][at[i]]; any = true; }
+    if (!any) break;
+    uint64_t c = 0;
+    for (size_t i = 0; i < N; i++)
+      if (at[i] < n[i] && keys[i][at[i]] == h) c += counts[i][at[i]++];
+    merged.emplace_back(h, (uint32_t)std::min<uint64_t>(c, std::numeric_limits<uint32_t>::max()));
+  }
+  n_unique = merged.size();
+  std::cerr << "[mashmap-b200::skch::Sketch::index] unique minmers = " << n_unique << std::endl;
+  threshold = std::numeric_limits<int>::max();
+  std::vector<hash_t> freq;
+  if (merged.empty()) {
+    std::cerr << "[mashmap-b200::skch::Sketch::computeFreqHist] No minmers." << std::endl;
+    return freq;
+  }
+  std::map<int, int> hist;
+  for (const auto &e : merged) hist[(int)e.second]++;
+  threshold = computeFreqThreshold(hist, (int64_t)merged.size(), kmer_pct_threshold);
+  if (threshold == std::numeric_limits<int>::max()) return freq;
+  for (const auto &e : merged)
+    if ((int64_t)e.second >= (int64_t)threshold) freq.push_back(e.first);  // isFreqSeed: count >= threshold (:488-495)
+  return freq;
 }
 
 void Sketch::saveIndexTSV(const std::string &path) const

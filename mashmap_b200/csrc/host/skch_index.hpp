@@ -16,6 +16,7 @@
 #define SKCH_INDEX_HPP
 
 #include <limits>
+#include <map>
 #include <memory>
 #include <string>
 #include <type_traits>
@@ -48,6 +49,16 @@ int addMinmersChunked(std::vector<MinmerInfo> &out, char *seq, offset_t len, int
 /* commonFunc.hpp:591-603 */
 uint64_t getReferenceSize(const std::vector<std::string> &refSequences);
 }  // namespace CommonFunc
+
+/* computeFreqHist's threshold (winSketch.hpp:418-449) over the histogram {interval points -> keys} of totalUniqueMinmers
+ * keys, with the reference's log lines; INT_MAX = consider all minmers */
+int computeFreqThreshold(const std::map<int, int> &hist, int64_t totalUniqueMinmers, float kmer_pct_threshold);
+/* The frequent seeds of a reference indexed in contig shards: keys[i][0, n[i]) are shard i's distinct hashes (ascending) and
+ * counts[i] their interval points. The histogram is the one of the union (a hash counts the points of every shard; each
+ * distinct hash is one key), so threshold, log lines and the returned hashes (ascending, count >= threshold) are those of
+ * the unsharded index. */
+std::vector<hash_t> globalFrequentSeeds(const std::vector<const hash_t *> &keys, const std::vector<const uint32_t *> &counts,
+                                        const std::vector<uint64_t> &n, float kmer_pct_threshold, int &threshold, uint64_t &n_unique);
 
 class Sketch {
  public:

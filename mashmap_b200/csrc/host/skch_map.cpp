@@ -55,6 +55,35 @@ void BatchMapper::setRefGroups()
   }
 }
 
+std::string BatchMapper::planShards(const std::vector<uint64_t> &len, const std::vector<int> &group, bool byGroup, int n_shards,
+                                    std::vector<int32_t> &first)
+{
+  const size_t C = len.size();
+  std::vector<uint64_t> before(C + 1, 0);  // bases of contigs [0, i)
+  for (size_t i = 0; i < C; i++) before[i + 1] = before[i] + len[i];
+  std::vector<int32_t> cuts;  // a cut at i: a shard begins with contig i
+  for (size_t i = 1; i < C; i++)
+    if (!byGroup || group[i] != group[i - 1]) cuts.push_back((int32_t)i);
+  if (n_shards < 1) return "--indexShards needs at least one shard";
+  if ((size_t)n_shards > cuts.size() + 1)
+    return "--indexShards " + std::to_string(n_shards) + ": the reference can be cut in at most " + std::to_string(cuts.size() + 1) +
+           " shards (" + std::to_string(cuts.size()) + " possible cut points between " +
+           (byGroup ? "runs of contigs in different -Y prefix groups" : "contigs") + ")";
+  first.assign(1, 0);
+  size_t lo = 0;
+  for (int k = 1; k < n_shards; k++) {  // cut k: the allowed point closest to k/N of the bases, leaving one for each later cut
+    const double want = (double)before[C] * k / n_shards;
+    const size_t hi = cuts.size() - (size_t)(n_shards - 1 - k);
+    size_t best = lo;
+    for (size_t j = lo; j < hi; j++)
+      if (std::abs((double)before[(size_t)cuts[j]] - want) < std::abs((double)before[(size_t)cuts[best]] - want)) best = j;
+    first.push_back(cuts[best]);
+    lo = best + 1;
+  }
+  first.push_back((int32_t)C);
+  return "";
+}
+
 int BatchMapper::getRefGroup(const std::string &seqName) const
 {  // computeMap.hpp:164-177
   const auto queryPrefix = prefix(seqName, param.prefix_delim);
@@ -171,48 +200,58 @@ BatchMapper::BatchMapper(const Parameters &p, const Sketch &refsketch) : param(p
   mp.kmer_size = param.kmerSize; mp.seg_length = param.segLength; mp.sketch_size = param.sketchSize;
   mp.stage1_topani_filter = param.stage1_topANI_filter; mp.skip_self = param.skip_self;
   mp.skip_prefix = param.skip_prefix; mp.lower_triangular = param.lower_triangular;
-  int rc = mm_ctx_create(param.device, &mp, &ctx);
-  if (rc != MM_OK) die(std::string("mm_ctx_create: ") + mm_last_error(nullptr));
-  std::vector<int32_t> clen(refSketch.metadata.size());
-  for (size_t i = 0; i < clen.size(); i++) clen[i] = refSketch.metadata[i].len;
-  if (refSketch.deviceBuildPending()) {
-    // skch::Sketch's build / index / computeFreqHist / dropFreqSeedSet on the device (mm_index_build.cu); the log lines
-    // are the reference's (winSketch.hpp:228, :403, :418-449)
-    mm_index_stats st;
-    auto t0 = Clock::now();
-    rc = mm_index_build(ctx, refSketch.deviceText(), 0, refSketch.deviceTextOffsets().data(), (int32_t)clen.size(), contigNameId.data(),
-                        refIdGroup.data(), param.kmer_pct_threshold, 0, &st);
-    if (rc != MM_OK) die(std::string("mm_index_build: ") + mm_last_error(ctx) + " (--hostIndex builds the index on the host)");
-    std::cerr << "[mashmap-b200::skch::Sketch::build] minmer windows picked from reference = " << st.n_minmers_before_filter << std::endl;
-    std::cerr << "[mashmap-b200::skch::Sketch::index] unique minmers = " << st.n_keys << std::endl;
-    if (st.n_keys) {
-      std::cerr << "[mashmap-b200::skch::Sketch::computeFreqHist] Frequency histogram of minmer interval points = (" << st.hist_min_count << ", "
-                << st.hist_min_keys << ") ... (" << st.hist_max_count << ", " << st.hist_max_keys << ")" << std::endl;
-      if (st.freq_threshold != std::numeric_limits<int>::max())
-        std::cerr << "[mashmap-b200::skch::Sketch::computeFreqHist] With threshold " << param.kmer_pct_threshold
-                  << "%, ignore minmers occurring >= " << st.freq_threshold << " times during lookup." << std::endl;
-      else
-        std::cerr << "[mashmap-b200::skch::Sketch::computeFreqHist] With threshold " << param.kmer_pct_threshold
-                  << "%, consider all minmers during lookup." << std::endl;
-    } else {
-      std::cerr << "[mashmap-b200::skch::Sketch::computeFreqHist] No minmers." << std::endl;
-    }
-    std::cerr << "[mashmap-b200::skch::Sketch] index built on the device in " << since(t0) << " s (window scan " << st.ms_scan * 1e-3
-              << " s over " << st.n_chunks << " chunks, " << st.n_fixed_chunks << " re-scanned exactly; records " << st.ms_post * 1e-3
-              << " s; lookup + frequency filter " << st.ms_lookup * 1e-3 << " s)" << std::endl;
-    refSketch.deviceBuildDone(st.freq_threshold);
+  int rc;
+  if (param.index_shards > 1) {
+    buildShards(mp);
   } else {
-    rc = mm_index_upload(ctx, refSketch.minmerIndex.data(), refSketch.minmerIndex.size(), refSketch.lookupKeys.data(),
-                         refSketch.lookupOffsets.data(), refSketch.lookupKeys.size(), refSketch.lookupPoints.data(),
-                         refSketch.lookupPoints.size(), refSketch.lookupKeyIsFreq.data(), clen.data(), contigNameId.data(),
-                         refIdGroup.data(), (int32_t)clen.size());
-    if (rc != MM_OK) die(std::string("mm_index_upload: ") + mm_last_error(ctx));
+    rc = mm_ctx_create(param.device, &mp, &ctx);
+    if (rc != MM_OK) die(std::string("mm_ctx_create: ") + mm_last_error(nullptr));
+    std::vector<int32_t> clen(refSketch.metadata.size());
+    for (size_t i = 0; i < clen.size(); i++) clen[i] = refSketch.metadata[i].len;
+    if (refSketch.deviceBuildPending()) {
+      // skch::Sketch's build / index / computeFreqHist / dropFreqSeedSet on the device (mm_index_build.cu); the log lines
+      // are the reference's (winSketch.hpp:228, :403, :418-449)
+      mm_index_stats st;
+      auto t0 = Clock::now();
+      rc = mm_index_build(ctx, refSketch.deviceText(), 0, refSketch.deviceTextOffsets().data(), (int32_t)clen.size(), contigNameId.data(),
+                          refIdGroup.data(), param.kmer_pct_threshold, 0, &st);
+      if (rc != MM_OK) die(std::string("mm_index_build: ") + mm_last_error(ctx) + " (--hostIndex builds the index on the host)");
+      std::cerr << "[mashmap-b200::skch::Sketch::build] minmer windows picked from reference = " << st.n_minmers_before_filter << std::endl;
+      std::cerr << "[mashmap-b200::skch::Sketch::index] unique minmers = " << st.n_keys << std::endl;
+      if (st.n_keys) {
+        std::cerr << "[mashmap-b200::skch::Sketch::computeFreqHist] Frequency histogram of minmer interval points = (" << st.hist_min_count << ", "
+                  << st.hist_min_keys << ") ... (" << st.hist_max_count << ", " << st.hist_max_keys << ")" << std::endl;
+        if (st.freq_threshold != std::numeric_limits<int>::max())
+          std::cerr << "[mashmap-b200::skch::Sketch::computeFreqHist] With threshold " << param.kmer_pct_threshold
+                    << "%, ignore minmers occurring >= " << st.freq_threshold << " times during lookup." << std::endl;
+        else
+          std::cerr << "[mashmap-b200::skch::Sketch::computeFreqHist] With threshold " << param.kmer_pct_threshold
+                    << "%, consider all minmers during lookup." << std::endl;
+      } else {
+        std::cerr << "[mashmap-b200::skch::Sketch::computeFreqHist] No minmers." << std::endl;
+      }
+      std::cerr << "[mashmap-b200::skch::Sketch] index built on the device in " << since(t0) << " s (window scan " << st.ms_scan * 1e-3
+                << " s over " << st.n_chunks << " chunks, " << st.n_fixed_chunks << " re-scanned exactly; records " << st.ms_post * 1e-3
+                << " s; lookup + frequency filter " << st.ms_lookup * 1e-3 << " s)" << std::endl;
+      refSketch.deviceBuildDone(st.freq_threshold);
+    } else {
+      rc = mm_index_upload(ctx, refSketch.minmerIndex.data(), refSketch.minmerIndex.size(), refSketch.lookupKeys.data(),
+                           refSketch.lookupOffsets.data(), refSketch.lookupKeys.size(), refSketch.lookupPoints.data(),
+                           refSketch.lookupPoints.size(), refSketch.lookupKeyIsFreq.data(), clen.data(), contigNameId.data(),
+                           refIdGroup.data(), (int32_t)clen.size());
+      if (rc != MM_OK) die(std::string("mm_index_upload: ") + mm_last_error(ctx));
+    }
   }
-  rc = mm_tables_upload(ctx, sketchCutoffs.data(), (int32_t)sketchCutoffs.size(), minHits.data(), (int32_t)minHits.size());
-  if (rc != MM_OK) die(std::string("mm_tables_upload: ") + mm_last_error(ctx));
+  for (size_t i = 0; i < std::max<size_t>(1, shards.size()); i++) {
+    mm_ctx *c = shards.empty() ? ctx : shards[i].ctx;
+    rc = mm_tables_upload(c, sketchCutoffs.data(), (int32_t)sketchCutoffs.size(), minHits.data(), (int32_t)minHits.size());
+    if (rc != MM_OK) die(std::string("mm_tables_upload: ") + mm_last_error(c));
+  }
   tail_ = new MapTail(param, refSketch.metadata, refIdGroup);
-  // one group per device; the first one owns the uploaded image, the others receive a copy over NVLink
+  // one group per device; the first one owns the uploaded image, the others receive a copy over NVLink. A sharded index
+  // has one group (the first shard's device): every part runs on all shards
   std::vector<int> devs = param.devices.empty() ? std::vector<int>{param.device} : param.devices;
+  if (!shards.empty()) devs.resize(1);
   std::vector<mm_ctx *> others;
   for (size_t d = 0; d < devs.size(); d++) {
     DeviceGroup *g = new DeviceGroup();
@@ -246,7 +285,7 @@ BatchMapper::BatchMapper(const Parameters &p, const Sketch &refsketch) : param(p
     // further contexts share the device's index image: one lane per pipeline stage in flight (upload / kernels / fetch + tail)
     g->lanes[0].ctx = g->owner;
     g->nLanes = 1;
-    const int max_lanes = getenv("MM_LANES") ? std::max(1, std::min<int>(MAX_LANES, atoi(getenv("MM_LANES")))) : MAX_LANES;  // experiment
+    const int max_lanes = !shards.empty() ? 1 : getenv("MM_LANES") ? std::max(1, std::min<int>(MAX_LANES, atoi(getenv("MM_LANES")))) : MAX_LANES;  // experiment
     for (int l = 1; l < max_lanes; l++) {
       mm_ctx *c2 = nullptr;
       if (mm_ctx_create(g->device, &mp, &c2) != MM_OK) break;
@@ -255,6 +294,7 @@ BatchMapper::BatchMapper(const Parameters &p, const Sketch &refsketch) : param(p
       g->nLanes = l + 1;
     }
     for (int l = 0; l < g->nLanes; l++) mm_ctx_set_wait_mode(g->lanes[l].ctx, g->blockingWaits ? 1 : 0);
+    for (auto &sh : shards) mm_ctx_set_wait_mode(sh.ctx, g->blockingWaits ? 1 : 0);
     if (g->nLanes > 1 && !getenv("MM_NO_GATE")) {
       g->gate = new Gate();
       for (int l = 0; l < g->nLanes; l++) mm_ctx_set_phase_hook(g->lanes[l].ctx, &BatchMapper::phaseHook, g->gate);
@@ -275,7 +315,156 @@ BatchMapper::~BatchMapper()
     delete g;
   }
   delete tail_;
+  for (auto &sh : shards)
+    if (sh.ctx != ctx) mm_ctx_destroy(sh.ctx);
   if (ctx) mm_ctx_destroy(ctx);
+}
+
+/* --indexShards: the plan, pass 1 on every shard (its hashes and their interval-point counts), the frequent seeds of the
+ * whole reference on the host, pass 2 (each shard's image with exactly those dropped). The log lines of the index are the
+ * unsharded build's. */
+void BatchMapper::buildShards(const mm_params &mp)
+{
+  const int N = param.index_shards;
+  const size_t C = refSketch.metadata.size();
+  std::vector<uint64_t> len(C);
+  for (size_t i = 0; i < C; i++) len[i] = (uint64_t)refSketch.metadata[i].len;
+  const std::string why = planShards(len, refIdGroup, param.skip_prefix, N, shardFirst);
+  if (!why.empty()) die(why);
+  if (!refSketch.deviceBuildPending()) die("--indexShards builds the index on the device");
+  const std::vector<int> devs = param.devices.empty() ? std::vector<int>{param.device} : param.devices;
+  std::cerr << "[mashmap-b200::skch::BatchMapper] index cut into " << N << " shards by contig:" << std::endl;
+  for (int i = 0; i < N; i++) {
+    uint64_t bases = 0;
+    for (int32_t c = shardFirst[i]; c < shardFirst[i + 1]; c++) bases += len[(size_t)c];
+    std::cerr << "[mashmap-b200::skch::BatchMapper]   shard " << i << ": contigs " << shardFirst[i] << "-" << shardFirst[i + 1] - 1 << " ("
+              << refSketch.metadata[(size_t)shardFirst[i]].name << " .. " << refSketch.metadata[(size_t)shardFirst[i + 1] - 1].name << "), "
+              << bases << " bases, device " << devs[(size_t)i % devs.size()] << std::endl;
+  }
+  auto t0 = Clock::now();
+  shards.resize((size_t)N);
+  const char *text = refSketch.deviceText();
+  const std::vector<uint64_t> &toff = refSketch.deviceTextOffsets();
+  auto shardOffsets = [&](int i) {  // the shard's contigs relative to its first base
+    std::vector<uint64_t> o;
+    for (int32_t c = shardFirst[i]; c <= shardFirst[i + 1]; c++) o.push_back(toff[(size_t)c] - toff[(size_t)shardFirst[i]]);
+    return o;
+  };
+  std::vector<std::vector<hash_t>> keys((size_t)N);
+  std::vector<std::vector<uint32_t>> counts((size_t)N);
+  uint64_t picked = 0;
+  for (int i = 0; i < N; i++) {
+    Shard &sh = shards[(size_t)i];
+    const int dev = devs[(size_t)i % devs.size()];
+    int rc = mm_ctx_create(dev, &mp, &sh.ctx);
+    if (rc != MM_OK) die("mm_ctx_create (device " + std::to_string(dev) + "): " + mm_last_error(nullptr));
+    const std::vector<uint64_t> o = shardOffsets(i);
+    uint64_t n = 0;
+    mm_index_stats st;
+    rc = mm_index_key_counts(sh.ctx, text + toff[(size_t)shardFirst[i]], 0, o.data(), (int32_t)(o.size() - 1), nullptr, nullptr, 0, &n, &st);
+    if (rc == MM_ECAPACITY) {
+      keys[(size_t)i].resize(n);
+      counts[(size_t)i].resize(n);
+      rc = mm_index_key_counts(sh.ctx, nullptr, 0, nullptr, 0, keys[(size_t)i].data(), counts[(size_t)i].data(), n, &n, nullptr);
+    }
+    if (rc != MM_OK) die(std::string("mm_index_key_counts (shard ") + std::to_string(i) + "): " + mm_last_error(sh.ctx));
+    picked += st.n_minmers_before_filter;
+  }
+  std::cerr << "[mashmap-b200::skch::Sketch::build] minmer windows picked from reference = " << picked << std::endl;
+  std::vector<const hash_t *> kp;
+  std::vector<const uint32_t *> cp;
+  std::vector<uint64_t> np;
+  for (int i = 0; i < N; i++) { kp.push_back(keys[(size_t)i].data()); cp.push_back(counts[(size_t)i].data()); np.push_back(keys[(size_t)i].size()); }
+  int threshold = std::numeric_limits<int>::max();
+  uint64_t unique = 0;
+  const std::vector<hash_t> freq = globalFrequentSeeds(kp, cp, np, param.kmer_pct_threshold, threshold, unique);
+  keys.clear(); counts.clear();
+  std::vector<int32_t> clen(C);
+  for (size_t i = 0; i < C; i++) clen[i] = refSketch.metadata[i].len;
+  for (int i = 0; i < N; i++) {
+    Shard &sh = shards[(size_t)i];
+    const std::vector<uint64_t> o = shardOffsets(i);
+    mm_index_stats st;
+    int rc = mm_index_build_shard(sh.ctx, text + toff[(size_t)shardFirst[i]], 0, o.data(), shardFirst[i], shardFirst[i + 1] - shardFirst[i],
+                                  clen.data(), contigNameId.data(), refIdGroup.data(), (int32_t)C, freq.data(), freq.size(), 0, &st);
+    if (rc != MM_OK) die(std::string("mm_index_build_shard (shard ") + std::to_string(i) + "): " + mm_last_error(sh.ctx) +
+                         " (a device that cannot hold its shard's image wants more shards)");
+    void *blob = nullptr;
+    uint64_t bytes = 0;
+    mm_index_blob(sh.ctx, &blob, &bytes);
+    std::cerr << "[mashmap-b200::skch::BatchMapper]   shard " << i << ": " << st.n_minmers << " minmers, " << st.n_keys << " lookup keys, "
+              << bytes << " index bytes" << std::endl;
+  }
+  std::cerr << "[mashmap-b200::skch::Sketch] index built on the device in " << N << " shards in " << since(t0) << " s" << std::endl;
+  refSketch.deviceBuildDone(threshold);
+  ctx = shards[0].ctx;
+}
+
+/* every shard maps the part. Without -Y one L1 sweep covers all contigs: phase 1 gives each shard's best intersection,
+ * phase 2 maps with their maximum and knows which later shards have points (mm_map_resident_with_best). With -Y each
+ * prefix group is swept on its own and lies in one shard: every shard's L1 is exact alone. */
+void BatchMapper::shardsCompute(Lane &ln)
+{
+  const bool twoPhase = !param.skip_prefix;
+  std::vector<int32_t> best;
+  std::vector<uint8_t> after;
+  if (twoPhase) {
+    best.assign(ln.nseg, 0);
+    for (size_t i = 0; i < shards.size(); i++) {
+      Shard &sh = shards[i];
+      sh.best.resize(ln.nseg);
+      if (mm_map_resident_l1_best(sh.ctx, sh.best.data()) != MM_OK)
+        die(std::string("mm_map_resident_l1_best (shard ") + std::to_string(i) + "): " + mm_last_error(sh.ctx));
+      for (size_t s = 0; s < ln.nseg; s++) best[s] = std::max(best[s], sh.best[s]);
+    }
+    after.assign(ln.nseg, 0);  // shards from the last one down: does a later one have points of the segment?
+  }
+  for (size_t i = shards.size(); i-- > 0;) {
+    Shard &sh = shards[i];
+    const int rc = twoPhase ? mm_map_resident_with_best(sh.ctx, best.data(), after.data(), &sh.nc, &sh.nl) : mm_map_resident(sh.ctx, &sh.nc, &sh.nl);
+    if (twoPhase)
+      for (size_t s = 0; s < ln.nseg; s++) after[s] |= sh.best[s] > 0 ? 1 : 0;
+    if (rc != MM_OK) die(std::string("mm_map_resident (shard ") + std::to_string(i) + "): " + mm_last_error(sh.ctx));
+  }
+  ln.nc = ln.nl = 0;
+  for (const Shard &sh : shards) { ln.nc += sh.nc; ln.nl += sh.nl; }
+}
+
+/* the shards' records of each segment, in shard order (= reference order: shards are ascending contig ranges), as one
+ * unsharded context returns them */
+void BatchMapper::shardsFetch(Lane &ln)
+{
+  for (size_t i = 0; i < shards.size(); i++) {
+    Shard &sh = shards[i];
+    sh.segRes.resize(ln.nseg); sh.cands.resize(sh.nc); sh.loci.resize(sh.nl);
+    if (mm_batch_fetch(sh.ctx, sh.segRes.data(), sh.cands.data(), sh.nc, sh.loci.data(), sh.nl) != MM_OK)
+      die(std::string("mm_batch_fetch (shard ") + std::to_string(i) + "): " + mm_last_error(sh.ctx));
+  }
+  uint64_t nc = 0, nl = 0;
+  for (size_t s = 0; s < ln.nseg; s++) {
+    mm_segment_result r = shards[0].segRes[s];
+    r.first_candidate = (uint32_t)nc; r.n_candidates = 0; r.n_points = 0; r.best_intersection = 0;
+    bool mhTaken = false;
+    for (size_t i = 0; i < shards.size(); i++) {
+      const mm_segment_result &q = shards[i].segRes[s];
+      if (q.sketch_max_hash != r.sketch_max_hash || q.sketch_raw_count != r.sketch_raw_count || q.sketch_size != r.sketch_size)
+        die("index shards disagree on the sketch of fragment " + std::to_string(ln.s0 + s) + " (shard " + std::to_string(i) + ")");
+      r.n_points += q.n_points;
+      r.best_intersection = std::max(r.best_intersection, q.best_intersection);
+      // the first reference group in point order decides minimumHits: the first shard with points holds it
+      if (!mhTaken && q.n_points > 0) { r.minimum_hits = q.minimum_hits; mhTaken = true; }
+      for (uint32_t c = q.first_candidate; c < q.first_candidate + q.n_candidates; c++) {
+        mm_l1_candidate cd = shards[i].cands[c];
+        memcpy(ln.loci.data() + nl, shards[i].loci.data() + cd.first_locus, (size_t)cd.n_loci * sizeof(mm_l2_locus));
+        cd.first_locus = (uint32_t)nl;
+        nl += cd.n_loci;
+        ln.cands.data()[nc++] = cd;
+        r.n_candidates++;
+      }
+    }
+    if (!mhTaken) r.minimum_hits = 0;
+    ln.segRes.data()[s] = r;
+  }
 }
 
 char *BatchMapper::allocBases(uint64_t n_bases)
@@ -377,8 +566,11 @@ void BatchMapper::laneUpload(Lane &ln, const ReadBatch &b, size_t r0, size_t r1)
     segp = ln.segs.data();
   }
   ln.nseg = s1 - ln.s0;
-  int rc = mm_batch_upload_packed(ln.ctx, b.nibbles(b0), b1 - b0, segp, ln.nseg);
-  if (rc != MM_OK) die(std::string("mm_batch_upload_packed: ") + mm_last_error(ln.ctx));
+  for (size_t i = 0; i < std::max<size_t>(1, shards.size()); i++) {  // a sharded index: the part goes to every shard
+    mm_ctx *c = shards.empty() ? ln.ctx : shards[i].ctx;
+    const int rc = mm_batch_upload_packed(c, b.nibbles(b0), b1 - b0, segp, ln.nseg);
+    if (rc != MM_OK) die(std::string("mm_batch_upload_packed: ") + mm_last_error(c));
+  }
   ln.msUpload = since(t0) * 1e3;
   ln.secDevice += since(t0);
 }
@@ -386,8 +578,12 @@ void BatchMapper::laneUpload(Lane &ln, const ReadBatch &b, size_t r0, size_t r1)
 void BatchMapper::laneCompute(Lane &ln)
 {
   auto t0 = Clock::now();
-  int rc = mm_map_resident(ln.ctx, &ln.nc, &ln.nl);
-  if (rc != MM_OK) die(std::string("mm_map_resident: ") + mm_last_error(ln.ctx));
+  if (!shards.empty()) {
+    shardsCompute(ln);
+  } else {
+    int rc = mm_map_resident(ln.ctx, &ln.nc, &ln.nl);
+    if (rc != MM_OK) die(std::string("mm_map_resident: ") + mm_last_error(ln.ctx));
+  }
   ln.msCompute = since(t0) * 1e3;
   ln.secDevice += since(t0);
 }
@@ -401,8 +597,12 @@ void BatchMapper::laneFinish(DeviceGroup &g, Lane &ln, const ReadBatch &b, std::
   if (ln.segRes.size() < ln.nseg) ln.segRes.reserve(ln.nseg + ln.nseg / 8 + 1024);
   if (ln.cands.size() < ln.nc) ln.cands.reserve(ln.nc + ln.nc / 8 + 1024);
   if (ln.loci.size() < ln.nl) ln.loci.reserve(ln.nl + ln.nl / 8 + 1024);
-  int rc = mm_batch_fetch(ln.ctx, ln.segRes.data(), ln.cands.data(), ln.cands.size(), ln.loci.data(), ln.loci.size());
-  if (rc != MM_OK) die(std::string("mm_batch_fetch: ") + mm_last_error(ln.ctx));
+  if (!shards.empty()) {
+    shardsFetch(ln);
+  } else {
+    int rc = mm_batch_fetch(ln.ctx, ln.segRes.data(), ln.cands.data(), ln.cands.size(), ln.loci.data(), ln.loci.size());
+    if (rc != MM_OK) die(std::string("mm_batch_fetch: ") + mm_last_error(ln.ctx));
+  }
   mm_last_stage_ms(ln.ctx, ln.stageMs);
   const double msFetch = since(t0) * 1e3;
   ln.secDevice += since(t0);

@@ -79,6 +79,11 @@ class BatchMapper {
   void alignOneToOne(const MappingResultsVector_t &maps, const std::function<const uint8_t *(seqno_t)> &query, std::string &paf);
   void reportAlignment() const;  // --align: totals of the run to stderr
 
+  /* --indexShards: cuts contigs [0, len.size()) into n_shards contiguous ranges balanced by bases; with byGroup (-Y) a cut
+   * only falls where group[] changes, so that no prefix group spans two shards. first[i] = first contig of shard i
+   * (first[n_shards] = the number of contigs). Returns "" or why the reference cannot be cut so. */
+  static std::string planShards(const std::vector<uint64_t> &len, const std::vector<int> &group, bool byGroup, int n_shards,
+                                std::vector<int32_t> &first);
   int getRefGroup(const std::string &seqName) const;  // computeMap.hpp:164-177
   const std::vector<int> &refGroups() const { return refIdGroup; }
   const MapTail &tail() const { return *tail_; }
@@ -150,6 +155,21 @@ class BatchMapper {
     int tailThreads = 1;
   };
   std::vector<DeviceGroup *> groups;
+  /* --indexShards N > 1: shard i (contigs [shardFirst[i], shardFirst[i + 1])) is the index image of shards[i].ctx, on
+   * devices[i % D]; every part of a batch runs on all of them (one lane) and their records are merged per segment */
+  struct Shard {
+    mm_ctx *ctx = nullptr;
+    std::vector<mm_segment_result> segRes;
+    std::vector<mm_l1_candidate> cands;
+    std::vector<mm_l2_locus> loci;
+    std::vector<int32_t> best;
+    uint64_t nc = 0, nl = 0;
+  };
+  std::vector<Shard> shards;
+  std::vector<int32_t> shardFirst;
+  void buildShards(const mm_params &mp);
+  void shardsCompute(Lane &ln);
+  void shardsFetch(Lane &ln);
   void setRefGroups();
   void laneUpload(Lane &ln, const ReadBatch &b, size_t r0, size_t r1);
   void laneCompute(Lane &ln);

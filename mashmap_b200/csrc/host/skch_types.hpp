@@ -110,6 +110,7 @@ struct Parameters {
   bool host_index = false;        // --hostIndex: build the reference index on the host (implied by --saveIndex / --loadIndex)
   int device = 0;                 // CUDA device ordinal (--device)
   std::vector<int> devices;       // --devices 0-7 / 0,2,5: several GPUs driven by this process (empty = {device})
+  int index_shards = 1;           // --indexShards N: the index cut by contig into N images, shard i on devices[i % D]
   uint64_t batch_bases = 1ULL << 30;  // query bases per device batch
   uint64_t sub_batch_bases = 640ULL << 20;  // a batch is mapped as sub-batches of this size on two pipelined lanes
   bool align = false;             // --align: NM:i / cg:Z tags from edlib NW over each printed mapping's region (on the device)

@@ -90,6 +90,13 @@ struct mm_ctx {
   mm_devbuf<unsigned char> d_scan_tmp, d_l2_order;
   mm_devbuf<uint2> d_l2_recs;
   mm_devbuf<uint32_t> d_l1_slow;
+  /* --indexShards: each segment's sweep-#1 best over this shard (mm_map_resident_l1_best), then the one over all shards
+   * (mm_map_resident_with_best); l1_best_ready: the resident batch has been sketched and its bests written */
+  mm_devbuf<int32_t> d_l1_best;
+  mm_devbuf<uint8_t> d_l1_after;
+  bool l1_best_ready = false;
+  /* mm_index_key_counts: a shard's distinct hashes and their interval-point counts, kept until the caller takes them */
+  mm_devbuf<uint64_t> kc_keys; mm_devbuf<uint32_t> kc_counts; uint64_t kc_n = 0; bool kc_ready = false;
   int l1_warp = 1; /* 1 = warp-per-segment fast path + CTA path for big segments; 0 = CTA path only (MM_L1_CTA=1) */
   int l2_mode = 1; /* 1 = stream kernels (mm_l2_stream.cu), 0 = general kernel only (MM_L2_GENERAL=1) */
   bool batch_mapped = false;
@@ -372,6 +379,7 @@ int upload_batch(mm_ctx *c, const void *bases, uint64_t n_bases, const mm_segmen
   c->n_segs = c->n_work = 0;
   c->n_long = 0;
   c->batch_mapped = false;
+  c->l1_best_ready = false;
   const uint64_t S = (uint64_t)c->params.sketch_size;
   const int L = c->params.seg_length, step = L - c->params.kmer_size + 1;
   std::vector<mm_segment> work;
@@ -480,6 +488,9 @@ mm_dev_batch make_batch(mm_ctx *c)
   b.l2_ranges = c->d_l2_ranges.get(); b.l2_rec_off = c->d_l2_rec_off.get();
   b.l2_recs = c->d_l2_recs.get(); b.l2_recs_cap = c->d_l2_recs.capacity();
   b.l2_loci_per_cand = 2;
+  b.l1_best = c->d_l1_best.get();
+  b.l1_after = c->d_l1_after.get();
+  b.l1_mode = MM_L1_FULL;
   return b;
 }
 
@@ -664,13 +675,16 @@ int run_l2_general(mm_ctx *c)
   });
 }
 
-/* K1 -> K2 -> K3 on the resident batch, growing output buffers and retrying on overflow */
-int run_pipeline(mm_ctx *c)
+/* K1 -> K2 -> K3 on the resident batch, growing output buffers and retrying on overflow. l1_mode (mm_internal.h):
+ * MM_L1_BEST_ONLY stops after K2 with each segment's best in d_l1_best; MM_L1_GIVEN_BEST takes the bests from there and
+ * skips K1 on its first attempt (the sketches of the best-only run are still in place: it did not compact them) */
+int run_pipeline(mm_ctx *c, int l1_mode = MM_L1_FULL)
 {
   int rc = check_ready(c);
   if (rc) return rc;
   CU(c, cudaSetDevice(c->device));
   c->batch_mapped = false;
+  c->l1_best_ready = false;
   const uint64_t n_segs = c->n_segs;
   CU(c, c->d_cands.reserve(2 * n_segs + 1024));
   CU(c, c->d_loci.reserve(2 * c->d_cands.capacity()));
@@ -681,11 +695,13 @@ int run_pipeline(mm_ctx *c)
 
   for (int attempt = 0; attempt < 6; attempt++) {
     mm_dev_batch b = make_batch(c);
+    b.l1_mode = l1_mode;
     ZERO_WORDS(c, c->d_counters.get(), sizeof(mm_counters) / 4);
     CU(c, cudaEventRecord(c->ev[EV_MAP_START], c->stream));
-    if ((rc = launch_pack_if_ascii(c))) return rc;
+    const bool sketch = l1_mode != MM_L1_GIVEN_BEST || attempt > 0;
+    if (sketch && (rc = launch_pack_if_ascii(c))) return rc;
     CU(c, cudaEventRecord(c->ev[EV_K1_START], c->stream));
-    if ((rc = launch_sketch_all(c, true))) return rc;
+    if (sketch && (rc = launch_sketch_all(c, true))) return rc;
     CU(c, cudaEventRecord(c->ev[EV_K1_END], c->stream));
     int l1_launches = 0;
     CU(c, mm_launch_l1(c->params, c->ix, b, c->stream, c->sm_count, c->d_l1_slow.get(), c->l1_warp, &l1_launches));
@@ -712,6 +728,10 @@ int run_pipeline(mm_ctx *c)
       retry = true;
     }
     if (retry) continue;
+    if (l1_mode == MM_L1_BEST_ONLY) {
+      c->l1_best_ready = true;
+      return MM_OK;
+    }
     c->n_cands = need_cands;
     /* K3: the stream kernels, or the general kernel where they are off or their own work areas do not fit */
     c->stage_ms[ST_L2_PREP] = c->stage_ms[ST_L2_SCAN] = 0; /* timed by the stream path only */
@@ -973,6 +993,38 @@ int mm_map_resident(mm_ctx *c, uint64_t *n_candidates, uint64_t *n_loci)
   return MM_OK;
 }
 
+int mm_map_resident_l1_best(mm_ctx *c, int32_t *best)
+{
+  if (!c || !best) return fail(c, MM_EINVAL, "null argument");
+  if (c->params.skip_prefix)
+    return fail(c, MM_EINVAL, "with skip_prefix every reference group has its own best: mm_map_resident is exact on a shard");
+  CU(c, cudaSetDevice(c->device));
+  if (c->d_l1_best.capacity() < c->n_segs + 1) {
+    CU(c, c->d_l1_best.reserve(c->n_segs + c->n_segs / 8 + 1024));
+    CU(c, c->d_l1_after.reserve(c->d_l1_best.capacity()));
+  }
+  int rc = run_pipeline(c, MM_L1_BEST_ONLY);
+  if (rc) return rc;
+  CU(c, cudaMemcpyAsync(best, c->d_l1_best.get(), c->n_segs * 4, cudaMemcpyDeviceToHost, c->stream));
+  CU(c, wait_stream(c));
+  return MM_OK;
+}
+
+int mm_map_resident_with_best(mm_ctx *c, const int32_t *best, const uint8_t *points_after, uint64_t *n_candidates, uint64_t *n_loci)
+{
+  if (!c || !best || !points_after) return fail(c, MM_EINVAL, "null argument");
+  if (!c->l1_best_ready) return fail(c, MM_ESTATE, "mm_map_resident_l1_best has not run on the resident batch");
+  CU(c, cudaSetDevice(c->device));
+  CU(c, cudaMemcpyAsync(c->d_l1_best.get(), best, c->n_segs * 4, cudaMemcpyHostToDevice, c->stream));
+  CU(c, cudaMemcpyAsync(c->d_l1_after.get(), points_after, c->n_segs, cudaMemcpyHostToDevice, c->stream));
+  c->l1_best_ready = false; /* the sketches are compacted from here on */
+  int rc = run_pipeline(c, MM_L1_GIVEN_BEST);
+  if (rc) return rc;
+  if (n_candidates) *n_candidates = c->n_cands;
+  if (n_loci) *n_loci = c->n_loci;
+  return MM_OK;
+}
+
 int mm_batch_fetch(mm_ctx *c, mm_segment_result *seg_results, mm_l1_candidate *cands, uint64_t cand_cap,
                    mm_l2_locus *loci, uint64_t loci_cap)
 {
@@ -1107,32 +1159,30 @@ int mm_host_alloc(void **ptr, uint64_t bytes)
 }
 int mm_host_free(void *ptr) { return cudaFreeHost(ptr) == cudaSuccess ? MM_OK : MM_ECUDA; }
 
-/* skch::Sketch's build + index + computeFreqHist + dropFreqSeedSet on the device (mm_index_build.cu) */
-int mm_index_build(mm_ctx *c, const char *seqs, int seqs_on_device, const uint64_t *contig_offsets, int32_t n_contigs,
-                   const int32_t *contig_name_id, const int32_t *contig_group, float kmer_pct_threshold, int keep_lookup,
-                   mm_index_stats *stats)
+namespace {
+/* the device builder over contigs [0, n_contigs) of contig_offsets (text at seqs, host or device) */
+int run_builder(mm_ctx *c, const char *seqs, int seqs_on_device, const uint64_t *contig_offsets, int32_t n_contigs,
+                float kmer_pct_threshold, const mm_shard_freq *shard, mm_built_index &B)
 {
-  if (!c) return MM_EINVAL;
-  if (n_contigs < 1 || !contig_offsets || !seqs) return fail(c, MM_EINVAL, "no contigs");
-  CU(c, cudaSetDevice(c->device));
-  const auto t0 = std::chrono::steady_clock::now();
-  drop_index(c);
-  image_guard guard{c};
-  c->built = mm_built_index{};
-  c->built_kept = false;
   const uint64_t total = contig_offsets[n_contigs];
   mm_devbuf<uint8_t> staged;
   if (!seqs_on_device) {
     CU(c, staged.reserve(total + 64));
     CU(c, cudaMemcpyAsync(staged.get(), seqs, total, cudaMemcpyHostToDevice, c->stream));
   }
-  mm_built_index B;
   std::string err;
   int rc = mm_build_index_device(c->params, seqs_on_device ? (const uint8_t *)seqs : staged.get(), contig_offsets, n_contigs,
-                                 kmer_pct_threshold, c->stream, c->sm_count, &B, err);
-  staged.reset();
+                                 kmer_pct_threshold, shard, c->stream, c->sm_count, &B, err);
   if (rc != MM_OK) return fail(c, rc, "index build: %s", err.c_str());
   c->launches += 12;
+  return MM_OK;
+}
+
+/* the image of what run_builder left in B (contig tables of n_contigs entries) */
+int image_from_build(mm_ctx *c, mm_built_index &B, int32_t n_contigs, const int32_t *clen, const int32_t *contig_name_id,
+                     const int32_t *contig_group, int keep_lookup, mm_index_stats *stats, std::chrono::steady_clock::time_point t0)
+{
+  int rc = MM_OK;
 
   const uint64_t n_mi = B.n_minmers, n_keys = B.n_keys, n_points = B.n_points;
   if (n_mi >= (1ULL << 32)) return fail(c, MM_EINVAL, "more than 2^32 minmers");
@@ -1162,9 +1212,7 @@ int mm_index_build(mm_ctx *c, const char *seqs, int seqs_on_device, const uint64
   mm_devbuf<uint32_t> d_err;
   CU(c, d_err.reserve(1));
   CU(c, cudaMemsetAsync(d_err.get(), 0, 4, c->stream));
-  std::vector<int32_t> clen((size_t)n_contigs);
-  for (int32_t q = 0; q < n_contigs; q++) clen[(size_t)q] = (int32_t)(contig_offsets[q + 1] - contig_offsets[q]);
-  rc = finish_image(c, cstart, B.keys.get(), B.offs.get(), B.is_freq.get(), d_err.get(), clen.data(), contig_name_id, contig_group);
+  rc = finish_image(c, cstart, B.keys.get(), B.offs.get(), B.is_freq.get(), d_err.get(), clen, contig_name_id, contig_group);
   if (!c->blob_ready) return rc; /* else rc is write_tables': the index stands either way */
   if (stats) {
     memset(stats, 0, sizeof *stats);
@@ -1176,6 +1224,96 @@ int mm_index_build(mm_ctx *c, const char *seqs, int seqs_on_device, const uint64
   }
   if (keep_lookup) { c->built = std::move(B); c->built_kept = true; }
   return rc;
+}
+} // namespace
+
+/* skch::Sketch's build + index + computeFreqHist + dropFreqSeedSet on the device (mm_index_build.cu) */
+int mm_index_build(mm_ctx *c, const char *seqs, int seqs_on_device, const uint64_t *contig_offsets, int32_t n_contigs,
+                   const int32_t *contig_name_id, const int32_t *contig_group, float kmer_pct_threshold, int keep_lookup,
+                   mm_index_stats *stats)
+{
+  if (!c) return MM_EINVAL;
+  if (n_contigs < 1 || !contig_offsets || !seqs) return fail(c, MM_EINVAL, "no contigs");
+  CU(c, cudaSetDevice(c->device));
+  const auto t0 = std::chrono::steady_clock::now();
+  drop_index(c);
+  image_guard guard{c};
+  c->built = mm_built_index{};
+  c->built_kept = false;
+  mm_built_index B;
+  int rc = run_builder(c, seqs, seqs_on_device, contig_offsets, n_contigs, kmer_pct_threshold, nullptr, B);
+  if (rc) return rc;
+  std::vector<int32_t> clen((size_t)n_contigs);
+  for (int32_t q = 0; q < n_contigs; q++) clen[(size_t)q] = (int32_t)(contig_offsets[q + 1] - contig_offsets[q]);
+  return image_from_build(c, B, n_contigs, clen.data(), contig_name_id, contig_group, keep_lookup, stats, t0);
+}
+
+int mm_index_key_counts(mm_ctx *c, const char *seqs, int seqs_on_device, const uint64_t *contig_offsets, int32_t n_contigs,
+                        uint64_t *keys, uint32_t *counts, uint64_t cap, uint64_t *n_keys, mm_index_stats *stats)
+{
+  if (!c || !n_keys) return MM_EINVAL;
+  CU(c, cudaSetDevice(c->device));
+  if (seqs) {
+    if (n_contigs < 1 || !contig_offsets) return fail(c, MM_EINVAL, "no contigs");
+    c->kc_keys.reset(); c->kc_counts.reset(); c->kc_n = 0; c->kc_ready = false;
+    const auto t0 = std::chrono::steady_clock::now();
+    mm_built_index B;
+    const mm_shard_freq count_only{1, nullptr, 0};
+    int rc = run_builder(c, seqs, seqs_on_device, contig_offsets, n_contigs, 0.f, &count_only, B);
+    if (rc) return rc;
+    c->kc_keys = std::move(B.keys); c->kc_counts = std::move(B.counts); c->kc_n = B.n_keys; c->kc_ready = true;
+    if (stats) {
+      memset(stats, 0, sizeof *stats);
+      stats->n_minmers_before_filter = B.n_minmers_before_filter; stats->n_keys = B.n_keys; stats->n_points = B.n_points;
+      stats->freq_threshold = 0x7fffffff; stats->n_chunks = B.n_chunks; stats->n_fixed_chunks = B.n_fixed_chunks;
+      stats->fix_rounds = B.fix_rounds; stats->ms_scan = B.ms_scan; stats->ms_post = B.ms_post;
+      stats->ms_total = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    }
+  } else if (!c->kc_ready) {
+    return fail(c, MM_ESTATE, "no key counts kept: call with the shard's contigs first");
+  }
+  *n_keys = c->kc_n;
+  if (cap < c->kc_n) return fail(c, MM_ECAPACITY, "need room for %llu keys", (unsigned long long)c->kc_n);
+  if (c->kc_n && (!keys || !counts)) return fail(c, MM_EINVAL, "null output");
+  if (c->kc_n) {
+    CU(c, cudaMemcpyAsync(keys, c->kc_keys.get(), c->kc_n * 8, cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaMemcpyAsync(counts, c->kc_counts.get(), c->kc_n * 4, cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+  }
+  c->kc_keys.reset(); c->kc_counts.reset(); c->kc_n = 0; c->kc_ready = false;
+  return MM_OK;
+}
+
+int mm_index_build_shard(mm_ctx *c, const char *seqs, int seqs_on_device, const uint64_t *contig_offsets, int32_t first_contig,
+                         int32_t n_shard_contigs, const int32_t *contig_len, const int32_t *contig_name_id,
+                         const int32_t *contig_group, int32_t n_contigs, const uint64_t *freq_hashes, uint64_t n_freq,
+                         int keep_lookup, mm_index_stats *stats)
+{
+  if (!c) return MM_EINVAL;
+  if (n_shard_contigs < 1 || !contig_offsets || !seqs || !contig_len) return fail(c, MM_EINVAL, "no contigs");
+  if (first_contig < 0 || n_contigs < first_contig + n_shard_contigs) return fail(c, MM_EINVAL, "the shard's contigs are out of range");
+  if (n_freq && !freq_hashes) return fail(c, MM_EINVAL, "null frequent-hash list");
+  for (uint64_t j = 1; j < n_freq; j++)
+    if (freq_hashes[j] <= freq_hashes[j - 1]) return fail(c, MM_EINVAL, "the frequent hashes are not strictly ascending");
+  CU(c, cudaSetDevice(c->device));
+  const auto t0 = std::chrono::steady_clock::now();
+  drop_index(c);
+  image_guard guard{c};
+  c->built = mm_built_index{};
+  c->built_kept = false;
+  /* every contig of the reference, those outside the shard empty: the builder then writes global seqIds */
+  std::vector<uint64_t> off((size_t)n_contigs + 1);
+  for (int32_t q = 0; q <= n_contigs; q++)
+    off[(size_t)q] = contig_offsets[std::min(std::max(q - first_contig, 0), n_shard_contigs)];
+  mm_devbuf<uint64_t> d_freq;
+  CU(c, d_freq.reserve(n_freq + 1));
+  if (n_freq) CU(c, cudaMemcpyAsync(d_freq.get(), freq_hashes, n_freq * 8, cudaMemcpyHostToDevice, c->stream));
+  mm_built_index B;
+  const mm_shard_freq listed{0, d_freq.get(), n_freq};
+  int rc = run_builder(c, seqs, seqs_on_device, off.data(), n_contigs, 0.f, &listed, B);
+  d_freq.reset();
+  if (rc) return rc;
+  return image_from_build(c, B, n_contigs, contig_len, contig_name_id, contig_group, keep_lookup, stats, t0);
 }
 
 /* host copies of what mm_index_build left on the device (needs keep_lookup); any output may be NULL */

@@ -393,6 +393,39 @@ __global__ void k_mark_freq(uint64_t n_keys, const uint32_t *__restrict__ cnt, u
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n_keys) is_freq[i] = cnt[i] >= threshold ? 1 : 0;
 }
+/* a shard of a contig-sharded index: the frequent seeds are the listed ones (ascending), not those above a local threshold */
+__device__ __forceinline__ bool in_sorted(const uint64_t *__restrict__ a, uint64_t n, uint64_t h)
+{
+  uint64_t lo = 0, hi = n;
+  while (lo < hi) {
+    const uint64_t mid = (lo + hi) >> 1;
+    if (a[mid] < h) lo = mid + 1; else hi = mid;
+  }
+  return lo < n && a[lo] == h;
+}
+__global__ void k_mark_listed(uint64_t n_keys, const uint64_t *__restrict__ keys, const uint64_t *__restrict__ freq, uint64_t n_freq,
+                              uint8_t *is_freq)
+{
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n_keys) is_freq[i] = in_sorted(freq, n_freq, keys[i]) ? 1 : 0;
+}
+__global__ void k_flag_absent(uint64_t n_freq, const uint64_t *__restrict__ freq, const uint64_t *__restrict__ keys, uint64_t n_keys,
+                              uint32_t *absent)
+{
+  const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j < n_freq) absent[j] = in_sorted(keys, n_keys, freq[j]) ? 0u : 1u;
+}
+/* the listed hashes the shard lacks: frequent keys with no points after its own keys, so that every shard drops them */
+__global__ void k_append_absent(uint64_t n_freq, const uint64_t *__restrict__ freq, const uint32_t *__restrict__ absent,
+                                const uint64_t *__restrict__ at, uint64_t n_keys, uint64_t n_points, uint64_t *keys, uint64_t *offs,
+                                uint8_t *is_freq)
+{
+  const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n_freq || !absent[j]) return;
+  const uint64_t d = n_keys + at[j];
+  keys[d] = freq[j]; offs[d] = n_points; is_freq[d] = 1;
+}
+
 /* keep[index position] = the record's hash is not a frequent seed (dropFreqSeedSet :497-504) */
 __global__ void k_keep_not_freq(uint64_t n, const uint32_t *__restrict__ perm, const uint64_t *__restrict__ rec_key, const uint8_t *__restrict__ is_freq,
                                 uint32_t *keep)
@@ -511,7 +544,7 @@ __global__ void k_build_table(const uint64_t *keys, const uint64_t *offs, const 
   if (i >= n_keys) return;
   uint64_t cnt = offs[i + 1] - offs[i];
   if (is_freq[i] && cnt > MM_VAL_CNT_MASK) cnt = MM_VAL_CNT_MASK; /* a frequent seed's list is never gathered: only the flag is read */
-  if (cnt == 0 || cnt > MM_VAL_CNT_MASK || offs[i] >= (1ULL << (64 - MM_VAL_OFF_SHIFT))) { atomicOr(err, 2u); return; }
+  if ((cnt == 0 && !is_freq[i]) || cnt > MM_VAL_CNT_MASK || offs[i] >= (1ULL << (64 - MM_VAL_OFF_SHIFT))) { atomicOr(err, 2u); return; }
   const uint64_t val = (offs[i] << MM_VAL_OFF_SHIFT) | (cnt << 1) | (is_freq[i] ? 1ULL : 0ULL);
   const uint32_t mask = (1u << tab_log2) - 1u;
   uint32_t slot = mm_tab_slot_of(keys[i], tab_log2);
@@ -562,7 +595,8 @@ __global__ void k_unpack_points(uint64_t n, const uint64_t *__restrict__ pts, co
   X(28) X(29) X(30) X(31) X(32)
 
 int mm_build_index_device(const mm_params &p, const uint8_t *d_seq, const uint64_t *h_contig_off, int32_t n_contigs,
-                          float kmer_pct_threshold, cudaStream_t st, int sm_count, mm_built_index *out, std::string &err)
+                          float kmer_pct_threshold, const mm_shard_freq *shard, cudaStream_t st, int sm_count,
+                          mm_built_index *out, std::string &err)
 {
   *out = mm_built_index{};
   const int K = p.kmer_size, w = p.seg_length, s = p.sketch_size;
@@ -853,48 +887,59 @@ int mm_build_index_device(const mm_params &p, const uint8_t *d_seq, const uint64
     CE(cudaStreamSynchronize(st));
     dv.free_now(key_start); dv.free_now(run_start); dv.free_now(key_idx); dv.free_now(run_idx); dv.free_now(hs);
     /* histogram of interval points per key (winSketch.hpp:415-417) */
-    uint32_t *cnt = nullptr;
-    CE(dv.alloc(cnt, n_keys));
+    CE(out->counts.reserve(n_keys));
+    uint32_t *cnt = out->counts.get();
     k_key_counts<<<blocks(n_keys), 256, 0, st>>>(n_keys, offs, n_points, cnt);
-    uint32_t max_cnt = 0;
-    {
-      uint32_t *d_max = nullptr;
-      CE(dv.alloc(d_max, 1));
-      void *tmp = nullptr; size_t bytes = 0;
-      cub::DeviceReduce::Max(nullptr, bytes, cnt, d_max, (int64_t)n_keys, st);
-      CE(cudaMalloc(&tmp, bytes + 16));
-      cub::DeviceReduce::Max(tmp, bytes, cnt, d_max, (int64_t)n_keys, st);
-      CE(cudaMemcpyAsync(&max_cnt, d_max, 4, cudaMemcpyDeviceToHost, st));
+    if (shard && shard->count_only) {
       CE(cudaStreamSynchronize(st));
-      cudaFree(tmp);
-      dv.free_now(d_max);
+      out->offs.reset(); out->pts.reset(); out->is_freq.reset();
+      for (auto &e : ev) cudaEventDestroy(e);
+      out->n_keys = n_keys; out->n_points = n_points; out->n_minmers_before_filter = n_mi;
+      return MM_OK;
     }
-    const uint32_t hist_n = max_cnt + 2;
-    unsigned long long *d_hist = nullptr;
-    CE(dv.alloc(d_hist, hist_n));
-    CE(cudaMemsetAsync(d_hist, 0, (size_t)hist_n * 8, st));
-    k_histogram<<<blocks(n_keys), 256, 0, st>>>(n_keys, cnt, d_hist, hist_n);
-    std::vector<unsigned long long> hist(hist_n);
-    CE(cudaMemcpyAsync(hist.data(), d_hist, (size_t)hist_n * 8, cudaMemcpyDeviceToHost, st));
-    CE(cudaStreamSynchronize(st));
-    dv.free_now(d_hist);
-    { /* computeFreqHist :431-441, the same arithmetic (int64 * float / 100 -> int64; walk from the most frequent) */
-      const int64_t totalUniqueMinmers = (int64_t)n_keys;
-      const int64_t minmerToIgnore = totalUniqueMinmers * kmer_pct_threshold / 100;
-      int64_t sum = 0;
-      for (int64_t f = (int64_t)hist_n - 1; f >= 0; f--) {
-        if (!hist[(size_t)f]) continue;
-        sum += (int64_t)hist[(size_t)f];
-        if (sum < minmerToIgnore) threshold = (int32_t)f;
-        else if (sum == minmerToIgnore) { threshold = (int32_t)f; break; }
-        else break;
+    if (!shard) { /* the frequency threshold over this index alone */
+      uint32_t max_cnt = 0;
+      {
+        uint32_t *d_max = nullptr;
+        CE(dv.alloc(d_max, 1));
+        void *tmp = nullptr; size_t bytes = 0;
+        cub::DeviceReduce::Max(nullptr, bytes, cnt, d_max, (int64_t)n_keys, st);
+        CE(cudaMalloc(&tmp, bytes + 16));
+        cub::DeviceReduce::Max(tmp, bytes, cnt, d_max, (int64_t)n_keys, st);
+        CE(cudaMemcpyAsync(&max_cnt, d_max, 4, cudaMemcpyDeviceToHost, st));
+        CE(cudaStreamSynchronize(st));
+        cudaFree(tmp);
+        dv.free_now(d_max);
       }
-      out->hist_min_count = 0; out->hist_max_count = max_cnt;
-      for (uint32_t f = 0; f < hist_n; f++) if (hist[f]) { out->hist_min_count = f; out->hist_min_keys = hist[f]; break; }
-      out->hist_max_keys = hist[max_cnt];
+      const uint32_t hist_n = max_cnt + 2;
+      unsigned long long *d_hist = nullptr;
+      CE(dv.alloc(d_hist, hist_n));
+      CE(cudaMemsetAsync(d_hist, 0, (size_t)hist_n * 8, st));
+      k_histogram<<<blocks(n_keys), 256, 0, st>>>(n_keys, cnt, d_hist, hist_n);
+      std::vector<unsigned long long> hist(hist_n);
+      CE(cudaMemcpyAsync(hist.data(), d_hist, (size_t)hist_n * 8, cudaMemcpyDeviceToHost, st));
+      CE(cudaStreamSynchronize(st));
+      dv.free_now(d_hist);
+      { /* computeFreqHist :431-441, the same arithmetic (int64 * float / 100 -> int64; walk from the most frequent) */
+        const int64_t totalUniqueMinmers = (int64_t)n_keys;
+        const int64_t minmerToIgnore = totalUniqueMinmers * kmer_pct_threshold / 100;
+        int64_t sum = 0;
+        for (int64_t f = (int64_t)hist_n - 1; f >= 0; f--) {
+          if (!hist[(size_t)f]) continue;
+          sum += (int64_t)hist[(size_t)f];
+          if (sum < minmerToIgnore) threshold = (int32_t)f;
+          else if (sum == minmerToIgnore) { threshold = (int32_t)f; break; }
+          else break;
+        }
+        out->hist_min_count = 0; out->hist_max_count = max_cnt;
+        for (uint32_t f = 0; f < hist_n; f++) if (hist[f]) { out->hist_min_count = f; out->hist_min_keys = hist[f]; break; }
+        out->hist_max_keys = hist[max_cnt];
+      }
     }
-    k_mark_freq<<<blocks(n_keys), 256, 0, st>>>(n_keys, cnt, (uint32_t)threshold, is_freq);
-    dv.free_now(cnt);
+    if (shard) k_mark_listed<<<blocks(n_keys), 256, 0, st>>>(n_keys, keys, shard->d_freq, shard->n_freq, is_freq);
+    else k_mark_freq<<<blocks(n_keys), 256, 0, st>>>(n_keys, cnt, (uint32_t)threshold, is_freq);
+    CE(cudaStreamSynchronize(st));
+    out->counts.reset();
     /* dropFreqSeedSet: the frequent hashes leave minmerIndex (not the lookup) */
     uint32_t *keep = nullptr; uint64_t *koff = nullptr;
     CE(dv.alloc(keep, n_mi)); CE(dv.alloc(koff, n_mi + 1));
@@ -912,6 +957,27 @@ int mm_build_index_device(const mm_params &p, const uint8_t *d_seq, const uint64
     CE(cudaStreamSynchronize(st));
     dv.free_now(keep); dv.free_now(koff);
     dv.free_now(m_hash); dv.free_now(m_wpos); dv.free_now(m_wend); dv.free_now(m_seq); dv.free_now(m_strand);
+  }
+  if (shard && shard->n_freq) { /* global frequent hashes this shard does not contain */
+    const uint64_t nf = shard->n_freq;
+    uint32_t *absent = nullptr; uint64_t *at = nullptr;
+    CE(dv.alloc(absent, nf)); CE(dv.alloc(at, nf + 1));
+    k_flag_absent<<<blocks(nf), 256, 0, st>>>(nf, shard->d_freq, keys, n_keys, absent);
+    CE(exclusive_sum_u32_to_u64(absent, at, nf, st, dv));
+    uint64_t lo = 0; uint32_t lu = 0;
+    CE(cudaMemcpy(&lo, at + nf - 1, 8, cudaMemcpyDeviceToHost)); CE(cudaMemcpy(&lu, absent + nf - 1, 4, cudaMemcpyDeviceToHost));
+    const uint64_t n_abs = lo + lu;
+    if (n_abs) {
+      CE(out->keys.reserve_keep(n_keys + n_abs, n_keys, st)); CE(out->offs.reserve_keep(n_keys + n_abs + 1, n_keys, st));
+      CE(out->is_freq.reserve_keep(n_keys + n_abs, n_keys, st));
+      if (!out->pts) CE(out->pts.reserve(1));
+      keys = out->keys.get(); offs = out->offs.get(); is_freq = out->is_freq.get();
+      k_append_absent<<<blocks(nf), 256, 0, st>>>(nf, shard->d_freq, absent, at, n_keys, n_points, keys, offs, is_freq);
+      CE(cudaGetLastError());
+      n_keys += n_abs;
+      CE(cudaMemcpyAsync(offs + n_keys, &n_points, 8, cudaMemcpyHostToDevice, st));
+      CE(cudaStreamSynchronize(st));
+    }
   }
   cudaEventRecord(ev[3], st);
   CE(cudaStreamSynchronize(st));

@@ -16,6 +16,7 @@ struct mm_built_index {
   mm_devbuf<uint64_t> hash; mm_devbuf<int32_t> wpos, wend, seq; mm_devbuf<int8_t> strand;
   /* minmerPosLookupIndex, keys ascending: keys[n_keys], offs[n_keys + 1], pts[n_points] (packed, mm_pack_point), is_freq[n_keys] */
   mm_devbuf<uint64_t> keys, offs, pts; mm_devbuf<uint8_t> is_freq;
+  mm_devbuf<uint32_t> counts; /* mm_shard_freq::count_only: the interval points of every key */
   int32_t freq_threshold = 0x7fffffff;
   /* statistics */
   uint64_t n_minmers_before_filter = 0;
@@ -24,8 +25,21 @@ struct mm_built_index {
   unsigned long long hist_min_keys = 0, hist_max_keys = 0;
   float ms_scan = 0, ms_post = 0, ms_lookup = 0;
 };
-/* d_seq: the contigs as text, back to back, on the device (readable up to h_contig_off[n_contigs]); returns MM_OK or MM_E* */
+/* One shard of a contig-sharded index (--indexShards, DESIGN.md). count_only: stop after Sketch::index and leave every
+ * distinct hash (ascending) in out->keys and its interval-point count in out->counts. Otherwise d_freq[n_freq] (device,
+ * ascending) are the frequent hashes of the WHOLE reference: exactly those are flagged and dropped, in place of the
+ * builder's own threshold, and the listed hashes this shard does not contain are appended after its keys as frequent keys
+ * with no points. */
+struct mm_shard_freq {
+  int count_only;
+  const uint64_t *d_freq;
+  uint64_t n_freq;
+};
+/* d_seq: the contigs as text, back to back, on the device (readable up to h_contig_off[n_contigs]); a contig of length 0
+ * gets no records (so a shard keeps the global seqIds of its contigs). shard: nullptr = the frequency threshold of
+ * kmer_pct_threshold over these contigs. Returns MM_OK or MM_E* */
 int mm_build_index_device(const mm_params &p, const uint8_t *d_seq, const uint64_t *h_contig_off, int32_t n_contigs,
-                          float kmer_pct_threshold, cudaStream_t st, int sm_count, mm_built_index *out, std::string &err);
+                          float kmer_pct_threshold, const mm_shard_freq *shard, cudaStream_t st, int sm_count,
+                          mm_built_index *out, std::string &err);
 
 #endif

@@ -124,7 +124,18 @@ struct mm_dev_batch {
   uint64_t l2_recs_cap;
   const uint32_t *l2_perm;       /* order in which k_l2_scan takes the candidates (nullptr = identity)        */
   uint32_t l2_loci_per_cand;     /* fixed locus slots per candidate in `loci`; overflow -> general kernel  */
+  /* K2 of a contig-sharded index (--indexShards): MM_L1_BEST_ONLY writes each segment's sweep-#1 best to l1_best[seg]
+   * and nothing else (no candidates, the sketch is not compacted); MM_L1_GIVEN_BEST takes the early return and the HG
+   * raise from l1_best[seg] (the best over all shards) instead of its own sweep */
+  int32_t *l1_best;
+  /* MM_L1_GIVEN_BEST, fragments longer than seg_length: l1_after[seg] != 0 = a later shard has points of the segment. The
+   * reference then tests this shard's last position group when its sweep moves on to that contig (:1026-1027) */
+  const uint8_t *l1_after;
+  int32_t l1_mode;
 };
+#define MM_L1_FULL 0
+#define MM_L1_BEST_ONLY 1
+#define MM_L1_GIVEN_BEST 2
 
 /* insert stream = index entries [it0, it0+nI) (by wpos); delete stream = death-order entries [d0, d0+nD) */
 struct mm_l2_range {

@@ -265,7 +265,7 @@ struct l1_shared {
 template <int NT, int LOCAL>
 __device__ int l1_process_range(const mm_params &prm, const mm_dev_index &ix, const uint64_t *keys, uint32_t *copn,
                                 uint32_t *head, uint32_t *ginfo, uint32_t n, int qs, l1_shared<NT, LOCAL> &sh, l1_out_list &o,
-                                int &mh_out)
+                                int &mh_out, const mm_dev_batch &b, uint32_t seg)
 {
   const int tid = grp<NT>::tid();
   const uint32_t chunk = (n + NT - 1) / NT;
@@ -335,12 +335,13 @@ __device__ int l1_process_range(const mm_params &prm, const mm_dev_index &ix, co
   }
   /* minimumHits (computeMap.hpp:1144, host table by Q.sketchSize) and the HG raise (:987-998) */
   int mh = ix.min_hits[min(qs, ix.n_min_hits - 1)];
-  bool go = true;
+  bool go = b.l1_mode != MM_L1_BEST_ONLY;
+  const int tb = b.l1_mode == MM_L1_GIVEN_BEST ? b.l1_best[seg] : best;
   if (prm.stage1_topani_filter) {
-    if (best < mh) go = false;
+    if (tb < mh) go = false;
     else {
       const double denom = fmax(1.0, (double)prm.sketch_size / 1000.0);
-      int ci = (int)((double)min(best, qs) / denom);
+      int ci = (int)((double)min(tb, qs) / denom);
       ci = min(ci, ix.n_cutoffs - 1);
       mh = max(ix.cutoffs[ci], mh);
     }
@@ -357,7 +358,8 @@ __device__ int l1_process_range(const mm_params &prm, const mm_dev_index &ix, co
  * l1_close_run). Returns bestIntersectionSize of sweep #1 (uncapped); mh_out = minimumHits after the HG raise, 0 on the
  * early return (:987-990). */
 __device__ int l1_window_range(const mm_params &prm, const mm_dev_index &ix, const uint64_t *keys, const uint32_t *hid,
-                               uint32_t n, int qs, int window_len, int *freq, uint32_t n_hits, l1_out_list &o, int &mh_out)
+                               uint32_t n, int qs, int window_len, int *freq, uint32_t n_hits, l1_out_list &o, int &mh_out,
+                               const mm_dev_batch &b, uint32_t seg)
 {
   auto seq = [&](uint32_t i) { return mm_point_seq(keys[i]); };
   auto pos = [&](uint32_t i) { return mm_point_pos(keys[i]); };
@@ -386,10 +388,12 @@ __device__ int l1_window_range(const mm_params &prm, const mm_dev_index &ix, con
   }
   int mh = ix.min_hits[min(qs, ix.n_min_hits - 1)];
   mh_out = 0;
+  if (b.l1_mode == MM_L1_BEST_ONLY) return best;
+  const int tb = b.l1_mode == MM_L1_GIVEN_BEST ? b.l1_best[seg] : best;
   if (prm.stage1_topani_filter) {
-    if (best < mh) return best; /* :987-990 */
+    if (tb < mh) return best; /* :987-990 */
     const double denom = fmax(1.0, (double)prm.sketch_size / 1000.0);
-    const int ci = min((int)((double)min(best, qs) / denom), ix.n_cutoffs - 1);
+    const int ci = min((int)((double)min(tb, qs) / denom), ix.n_cutoffs - 1);
     mh = max(ix.cutoffs[ci], mh); /* :992-997 */
   }
   mh_out = mh;
@@ -433,6 +437,26 @@ __device__ int l1_window_range(const mm_params &prm, const mm_dev_index &ix, con
       }
     } else {
       if (in_cand) push_local();
+      in_cand = false;
+    }
+  }
+  if (b.l1_mode == MM_L1_GIVEN_BEST && b.l1_after[seg]) { /* the next group is a later shard's: this shard's last one is tested */
+    if (overlap >= mh) {
+      if (c_seq != cur_seq && in_cand) {
+        push_local();
+        in_cand = false;
+      }
+      if (!in_cand) {
+        c_start = c_end = cur_pos - window_len;
+        c_seq = cur_seq;
+        c_isz = overlap;
+        in_cand = true;
+      } else {
+        c_isz = max(c_isz, overlap);
+        c_end = cur_pos - window_len;
+      }
+    } else if (in_cand) {
+      push_local();
       in_cand = false;
     }
   }
@@ -496,7 +520,7 @@ __device__ bool l1_segment(const mm_params &prm, const mm_dev_index &ix, const m
     const uint32_t pk = group_exclusive_scan<NT>(keep ? 1u : 0u, sh.warp_sums, tot_k);
     const uint32_t ph = group_exclusive_scan<NT>(hit ? 1u : 0u, sh.warp_sums, tot_h);
     const uint32_t pm = group_exclusive_scan<NT>(cnt, sh.warp_sums, tot_m);
-    if (keep) { /* destination index <= j: never overtakes the reads of a later chunk */
+    if (keep && b.l1_mode != MM_L1_BEST_ONLY) { /* destination index <= j: never overtakes the reads of a later chunk */
       b.sk_hash[sbase + kept_total + pk] = h;
       b.sk_pos[sbase + kept_total + pk] = ps;
       b.sk_strand[sbase + kept_total + pk] = st;
@@ -622,10 +646,10 @@ __device__ bool l1_segment(const mm_params &prm, const mm_dev_index &ix, const m
       if (WIN) { /* only thread 0's best / mh are read (the segment result below) */
         if (tid == 0)
           best = l1_window_range(prm, ix, keys + start, copn + start, end - start, (int)kept_total, sg.length - prm.seg_length,
-                                 (int *)hits, hit_total, out, mh); /* the hit list is dead: its space holds hash_to_freq */
+                                 (int *)hits, hit_total, out, mh, b, seg); /* the hit list is dead: its space holds hash_to_freq */
         grp<NT>::sync();
       } else {
-        best = l1_process_range<NT, LOCAL>(prm, ix, keys + start, copn, head, ginfo, end - start, (int)kept_total, sh, out, mh);
+        best = l1_process_range<NT, LOCAL>(prm, ix, keys + start, copn, head, ginfo, end - start, (int)kept_total, sh, out, mh, b, seg);
       }
       if (pass == 0) {
         best_all = max(best_all, best);
@@ -672,6 +696,7 @@ __device__ bool l1_segment(const mm_params &prm, const mm_dev_index &ix, const m
     r.n_candidates = sh.out_n;
     r._pad = 0;
     b.seg_res[seg] = r;
+    if (b.l1_mode == MM_L1_BEST_ONLY) b.l1_best[seg] = best_all;
   }
   grp<NT>::sync();
   return true;

@@ -102,6 +102,11 @@ def lib():
         L.skch_bm_paf.restype = vp
         L.skch_bm_results.argtypes = [vp, vp, C.c_uint64]
         L.skch_bm_results.restype = C.c_uint64
+        L.skch_plan_shards.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp]
+        L.skch_last_plan_error.restype = C.c_char_p
+        L.skch_global_frequent_seeds.argtypes = [C.c_int, vp, vp, vp, C.c_float, vp, C.c_uint64, C.POINTER(C.c_int32),
+                                                 C.POINTER(C.c_uint64)]
+        L.skch_global_frequent_seeds.restype = C.c_int64
         _lib = L
     return _lib
 
@@ -361,3 +366,30 @@ class HostTail:
         if self.h:
             lib().skch_tail_destroy(self.h)
             self.h = None
+
+
+def plan_shards(contig_len, groups, by_group, n_shards):
+    """--indexShards' plan (skch::BatchMapper::planShards): the first contig of every shard plus the contig count, or
+    ValueError with the reason the reference cannot be cut so"""
+    ln = np.ascontiguousarray(contig_len, dtype=np.uint64)
+    gr = np.ascontiguousarray(groups, dtype=np.int32)
+    first = np.zeros(max(n_shards, 0) + 1, dtype=np.int32)
+    if lib().skch_plan_shards(ln.ctypes.data, gr.ctypes.data, len(ln), int(by_group), n_shards, first.ctypes.data) != 0:
+        raise ValueError(lib().skch_last_plan_error().decode())
+    return first
+
+
+def global_frequent_seeds(shard_keys, shard_counts, kmer_pct_threshold):
+    """the frequent seeds of a reference indexed in shards, from each shard's distinct hashes (ascending) and their
+    interval-point counts: (threshold, number of distinct hashes, frequent hashes ascending)"""
+    ks = [np.ascontiguousarray(k, dtype=np.uint64) for k in shard_keys]
+    cs = [np.ascontiguousarray(c, dtype=np.uint32) for c in shard_counts]
+    kp = (C.c_void_p * len(ks))(*[k.ctypes.data for k in ks])
+    cp = (C.c_void_p * len(cs))(*[c.ctypes.data for c in cs])
+    n = np.array([len(k) for k in ks], dtype=np.uint64)
+    out = np.zeros(max(1, int(n.sum())), dtype=np.uint64)
+    thr, uniq = C.c_int32(0), C.c_uint64(0)
+    m = lib().skch_global_frequent_seeds(len(ks), C.cast(kp, C.c_void_p), C.cast(cp, C.c_void_p), n.ctypes.data,
+                                         kmer_pct_threshold, out.ctypes.data, len(out), C.byref(thr), C.byref(uniq))
+    assert m >= 0
+    return int(thr.value), int(uniq.value), out[:m].copy()
