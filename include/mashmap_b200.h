@@ -312,6 +312,25 @@ int mm_last_pack_ms(const mm_ctx *ctx, float *ms);
 int mm_host_alloc(void **ptr, uint64_t bytes);
 int mm_host_free(void *ptr);
 
+/* ---- BGZF / raw DEFLATE inflation on the device (mm_inflate.cu) -------------------------------------
+ * A handle of its own: inflating needs none of mm_ctx's mapping parameters. Block i is the raw DEFLATE stream
+ * comp[comp_off[i], comp_off[i+1]) (a BGZF member's data, without its gzip header and trailer); it must inflate to
+ * exactly out[out_off[i], out_off[i+1]) (ISIZE bytes) with CRC-32 crc[i]. comp_off and out_off have n_blocks + 1
+ * entries, both non-decreasing. Host pointers in and out (pinned ones copy faster, mm_host_alloc); the blocks go
+ * through the device in slices that fit the handle's device buffers. On a block that does not inflate, does not fill its
+ * range exactly, or has another CRC: MM_EINVAL, *bad_block = its index (else -1), mm_inflater_error() says why.
+ * The decoder never reads or writes outside a block's ranges, whatever the input. The handle stays usable after any
+ * error. */
+typedef struct mm_inflater mm_inflater;
+int mm_inflater_create(int device, mm_inflater **out);
+int mm_inflater_destroy(mm_inflater *inf);
+const char *mm_inflater_error(const mm_inflater *inf); /* NULL handle: the last mm_inflater_create error */
+int mm_inflate_blocks(mm_inflater *inf, const uint8_t *comp, const uint64_t *comp_off, const uint64_t *out_off,
+                      const uint32_t *crc, uint64_t n_blocks, uint8_t *out, int64_t *bad_block);
+/* CUDA-event time of the last successful mm_inflate_blocks, in milliseconds: [0] the inflate kernels, [1] the whole
+ * call (uploads, kernels, downloads) */
+int mm_inflater_last_ms(const mm_inflater *inf, float ms[2]);
+
 #ifdef __cplusplus
 }
 #endif

@@ -114,6 +114,12 @@ def lib():
         L.mm_last_stage_ms.argtypes = [vp, C.POINTER(C.c_float * 8)]
         L.mm_host_alloc.argtypes = [C.POINTER(vp), u64]
         L.mm_host_free.argtypes = [vp]
+        L.mm_inflater_create.argtypes = [C.c_int, C.POINTER(vp)]
+        L.mm_inflater_destroy.argtypes = [vp]
+        L.mm_inflater_error.argtypes = [vp]
+        L.mm_inflater_error.restype = C.c_char_p
+        L.mm_inflate_blocks.argtypes = [vp, vp, vp, vp, vp, u64, vp, C.POINTER(C.c_int64)]
+        L.mm_inflater_last_ms.argtypes = [vp, C.POINTER(C.c_float * 2)]
         _lib = L
     return _lib
 
@@ -124,6 +130,7 @@ EXPORTED_SYMBOLS = [
     "mm_map_segments", "mm_map_segments_packed", "mm_batch_upload", "mm_batch_upload_packed", "mm_last_pack_ms", "mm_map_resident", "mm_batch_fetch", "mm_batch_fetch_sketch",
     "mm_last_stage_ms", "mm_ctx_set_phase_hook", "mm_ctx_set_wait_mode", "mm_params_check", "mm_host_alloc", "mm_host_free",
     "mm_index_key_counts", "mm_index_build_shard", "mm_map_resident_l1_best", "mm_map_resident_with_best",
+    "mm_inflater_create", "mm_inflater_destroy", "mm_inflater_error", "mm_inflate_blocks", "mm_inflater_last_ms",
 ]
 
 
@@ -180,6 +187,43 @@ class PinnedBuffer:
     def __del__(self):
         try:
             self.free()
+        except Exception:
+            pass
+
+
+class Inflater:
+    """mm_inflater: raw DEFLATE blocks inflated on the device"""
+
+    def __init__(self, device=0):
+        self._h = C.c_void_p()
+        rc = lib().mm_inflater_create(device, C.byref(self._h))
+        if rc != MM_OK:
+            raise MashmapError(rc, lib().mm_inflater_error(None).decode())
+
+    def inflate(self, comp, comp_off, out_off, crc, out=None):
+        """(rc, bad_block, out, error): comp uint8, comp_off / out_off uint64 [n+1], crc uint32 [n]"""
+        comp = _c(comp, np.uint8)
+        comp_off, out_off, crc = _c(comp_off, np.uint64), _c(out_off, np.uint64), _c(crc, np.uint32)
+        n = len(crc)
+        if out is None:
+            out = np.zeros(max(int(out_off[-1]) if n else 0, 1), dtype=np.uint8)
+        bad = C.c_int64()
+        rc = lib().mm_inflate_blocks(self._h, _ptr(comp), _ptr(comp_off), _ptr(out_off), _ptr(crc), n, _ptr(out), C.byref(bad))
+        return rc, bad.value, out, lib().mm_inflater_error(self._h).decode()
+
+    def last_ms(self):
+        a = (C.c_float * 2)()
+        lib().mm_inflater_last_ms(self._h, C.byref(a))
+        return a[0], a[1]
+
+    def close(self):
+        if self._h:
+            lib().mm_inflater_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
         except Exception:
             pass
 

@@ -4,6 +4,7 @@
  * Not part of the drop-in boundary (that is include/mashmap_b200.h + the skch:: classes).
  */
 #include <algorithm>
+#include <memory>
 #include <atomic>
 #include <chrono>
 #include <thread>
@@ -22,6 +23,9 @@
 #include "skch_stats.hpp"
 #include "skch_filter.hpp"
 #include "skch_tail.hpp"
+#include "../mm_inflate.h"
+
+#include <zlib.h>
 
 using namespace skch;
 
@@ -459,6 +463,143 @@ int64_t skch_fasta_readers_diff(const char *path, int threads, uint64_t *n_recor
     if (a != b) bad++;
   }
   return bad;
+}
+
+/* ---- BGZF input (tests) ---- */
+
+/* the host build of mm_inflate.h on one raw DEFLATE stream of exactly out_len inflated bytes: its mmi_status; *crc gets
+ * the CRC-32 of the text when it inflated */
+int skch_mmi_inflate(const uint8_t *comp, uint64_t comp_len, uint8_t *out, uint64_t out_len, uint32_t *crc)
+{
+  std::unique_ptr<mmi_tables> t(new mmi_tables());
+  const int rc = mmi_inflate(comp, comp_len, out, out_len, *t, 0, 1);
+  if (rc == MMI_OK && crc) {
+    uint32_t tab[256];
+    mmi_crc_table(tab, 0, 1);
+    *crc = mmi_crc_finish(mmi_crc_share(tab, out, out_len, 0, 1), out_len);
+  }
+  return rc;
+}
+
+namespace {
+/* the host inflater, made to report block `fail_at` of the whole file (counted across calls) as bad */
+struct FailingInflater : seqio::HostInflater {
+  int64_t fail_at, seen = 0;
+  uint64_t calls = 0;
+  explicit FailingInflater(int64_t f) : fail_at(f) {}
+  int inflate(const uint8_t *comp, const uint64_t *comp_off, const uint64_t *out_off, const uint32_t *crc, uint64_t n,
+              uint8_t *out, int64_t *bad_block, std::string &error) override
+  {
+    calls++;
+    const int64_t first = seen;
+    seen += (int64_t)n;
+    if (fail_at >= first && fail_at < seen) {
+      *bad_block = fail_at - first;
+      error = "rejected by the test";
+      return 1;
+    }
+    return HostInflater::inflate(comp, comp_off, out_off, crc, n, out, bad_block, error);
+  }
+};
+thread_local std::string g_bgzf_error;
+}  // namespace
+
+const char *skch_bgzf_error() { return g_bgzf_error.c_str(); }
+
+/* the text of a BGZF FASTA file as the windowed reader hands it over (windows of window_bytes, host inflater; block
+ * fail_block reported bad, -1 = none): its length (the first cap bytes go to buf), -1 if the reader declines the file,
+ * -3 on an error (skch_bgzf_error). *n_windows / *n_calls: windows handed over, inflater calls made. */
+int64_t skch_bgzf_text(const char *path, uint64_t window_bytes, int threads, int64_t fail_block, uint8_t *buf, uint64_t cap,
+                       uint64_t *n_windows, uint64_t *n_calls)
+{
+  seqio::BgzfFasta bz;
+  if (!bz.open(path)) return -1;
+  FailingInflater inf(fail_block);
+  uint64_t n = 0, w = 0;
+  const int rc = bz.for_each_window(inf, window_bytes, threads, [&](const seqio::FastaText &t) {
+    if (n < cap) memcpy(buf + n, t.data(), std::min<uint64_t>(cap - n, t.size()));
+    n += t.size();
+    w++;
+  });
+  if (n_windows) *n_windows = w;
+  if (n_calls) *n_calls = inf.calls;
+  if (rc < 0) { g_bgzf_error = bz.error(); return -3; }
+  return rc == 1 ? -1 : (int64_t)n;
+}
+
+/* everything gzread gives for a file (what the line reader reads): its length, the first cap bytes to buf */
+int64_t skch_gzread_text(const char *path, uint8_t *buf, uint64_t cap)
+{
+  gzFile f = gzopen(path, "rb");
+  if (!f) return -1;
+  std::vector<char> b(1 << 20);
+  uint64_t n = 0;
+  int got;
+  while ((got = gzread(f, b.data(), (unsigned)b.size())) > 0) {
+    if (n < cap) memcpy(buf + n, b.data(), std::min<uint64_t>(cap - n, (uint64_t)got));
+    n += (uint64_t)got;
+  }
+  gzclose(f);
+  return (int64_t)n;
+}
+
+/* records of a BGZF FASTA file through the windowed reader (host inflater) against the line reader: -1 if the reader
+ * declines the file, -3 on an error, else the number of records that differ in name, bases or nibbles */
+int64_t skch_bgzf_readers_diff(const char *path, uint64_t window_bytes, int threads, uint64_t *n_records, uint64_t *n_bases)
+{
+  std::vector<std::pair<std::string, std::string>> ref;
+  uint64_t bases = 0;
+  if (!seqio::for_each_seq_in_file(path, {}, "", [&](const std::string &name, const std::string &seq) {
+        ref.emplace_back(name, seq);
+        bases += seq.size();
+      }))
+    return -2;
+  if (n_records) *n_records = ref.size();
+  if (n_bases) *n_bases = bases;
+  seqio::BgzfFasta bz;
+  if (!bz.open(path)) return -1;
+  seqio::HostInflater inf;
+  size_t i = 0;
+  int64_t bad = 0;
+  const int rc = bz.for_each_window(inf, window_bytes, threads, [&](const seqio::FastaText &t) {
+    for (const seqio::FastaRecord &r : t.records()) {
+      if (i >= ref.size()) { bad++; continue; }
+      std::string seq(r.seq_len, '\0');
+      t.copy_bases(r, &seq[0]);
+      std::vector<uint8_t> a((r.seq_len + 1) / 2 + 1, 0), b((r.seq_len + 1) / 2 + 1, 0);
+      t.pack_bases(r, a.data());
+      seqio::pack_bases(seq.data(), seq.size(), b.data());
+      if (r.seq_len & 1) { a[r.seq_len / 2] |= 0xF0; b[r.seq_len / 2] |= 0xF0; }
+      if (t.name(r) != ref[i].first || seq != ref[i].second || a != b) bad++;
+      i++;
+    }
+  });
+  if (rc < 0) { g_bgzf_error = bz.error(); return -3; }
+  if (rc == 1) return -1;
+  return bad + (int64_t)(ref.size() - std::min(ref.size(), i));
+}
+
+/* skch_read_file_digest's digest through the windowed BGZF reader (host inflater); -1 if it declines the file */
+int skch_bgzf_read_digest(const char *path, uint64_t window_bytes, int threads, uint64_t *n_records, uint64_t *n_bases, uint64_t *digest)
+{
+  uint64_t h = 1469598103934665603ULL, nr = 0, nb = 0;
+  auto eat = [&h](const std::string &s) {
+    for (unsigned char c : s) { h ^= c; h *= 1099511628211ULL; }
+    h ^= 0xFF; h *= 1099511628211ULL;
+  };
+  seqio::BgzfFasta bz;
+  if (!bz.open(path)) return -1;
+  seqio::HostInflater inf;
+  const int rc = bz.for_each_window(inf, window_bytes, threads, [&](const seqio::FastaText &t) {
+    for (const auto &r : t.records()) {
+      std::string seq(r.seq_len, '\0');
+      t.copy_bases(r, &seq[0]);
+      eat(t.name(r)); eat(seq); nr++; nb += seq.size();
+    }
+  });
+  if (rc != 0) return rc == 1 ? -1 : -3;
+  *n_records = nr; *n_bases = nb; *digest = h;
+  return 0;
 }
 
 /* records, bases and an FNV-1a digest of every (name, sequence) pair of a file in order, through the line reader (bulk = 0)

@@ -395,27 +395,54 @@ void Sketch::build()
   seqno_t seqCounter = 0;
   uint64_t textBytes = 0, textCap = 0;
   if (on_device) deviceTextOffsets_.push_back(0);
+  auto onSequence = [&](const std::string &name, const std::string &seq) {
+    offset_t len = seq.length();
+    metadata.push_back(ContigInfo{name, len});
+    if (param.align) keepForAlign(seq.data(), seq.size());
+    if (on_device) {  // every contig, also the short ones: seqId = position in metadata
+      if (textBytes + seq.size() + 64 > textCap) {
+        textCap = std::max<uint64_t>(textCap * 2, textBytes + seq.size() + (64ULL << 20));
+        deviceText_ = (char *)realloc(deviceText_, textCap);
+        if (!deviceText_) { std::cerr << "[mashmap-b200] ERROR: out of memory reading the reference" << std::endl; exit(1); }
+      }
+      memcpy(deviceText_ + textBytes, seq.data(), seq.size());
+      textBytes += seq.size();
+      deviceTextOffsets_.push_back(textBytes);
+    } else if (len >= param.kmerSize && param.loadIndexFilename.empty()) {
+      tasks.emplace_back(new Task{seq, seqCounter});
+    }
+    seqCounter++;
+  };
+  std::unique_ptr<seqio::DeviceInflater> inflater;  // BGZF references of an index built on the device
   for (const auto &fileName : param.refSequences) {
-    bool ok = seqio::for_each_seq_in_file(fileName, allowed, param.target_prefix,
-                                          [&](const std::string &name, const std::string &seq) {
-                                            offset_t len = seq.length();
-                                            metadata.push_back(ContigInfo{name, len});
-                                            if (param.align) keepForAlign(seq.data(), seq.size());
-                                            if (on_device) {  // every contig, also the short ones: seqId = position in metadata
-                                              if (textBytes + seq.size() + 64 > textCap) {
-                                                textCap = std::max<uint64_t>(textCap * 2, textBytes + seq.size() + (64ULL << 20));
-                                                deviceText_ = (char *)realloc(deviceText_, textCap);
-                                                if (!deviceText_) { std::cerr << "[mashmap-b200] ERROR: out of memory reading the reference" << std::endl; exit(1); }
-                                              }
-                                              memcpy(deviceText_ + textBytes, seq.data(), seq.size());
-                                              textBytes += seq.size();
-                                              deviceTextOffsets_.push_back(textBytes);
-                                            } else if (len >= param.kmerSize && param.loadIndexFilename.empty()) {
-                                              tasks.emplace_back(new Task{seq, seqCounter});
-                                            }
-                                            seqCounter++;
-                                          });
-    if (!ok) exit(1);
+    seqio::BgzfFasta bz;
+    int rc = 1;
+    if (on_device && !getenv("MM_SERIAL_INPUT") && bz.open(fileName)) {
+      const int dev = param.devices.empty() ? param.device : param.devices[0];
+      if (!inflater) inflater.reset(new seqio::DeviceInflater(dev));
+      std::string seq;
+      uint64_t windows = 0;
+      // the line reader's semantics: a record outside --targetPrefix / --targetList comes with an empty sequence
+      rc = bz.for_each_window(*inflater, seqio::bgzf_window_bytes(param.batch_bases), param.threads, [&](const seqio::FastaText &t) {
+        for (const seqio::FastaRecord &r : t.records()) {
+          const std::string name = t.name(r);
+          const bool keep = (param.target_prefix.empty() || name.compare(0, param.target_prefix.length(), param.target_prefix) == 0) &&
+                            (allowed.empty() || allowed.count(name));
+          seq.resize(keep ? r.seq_len : 0);
+          if (keep) t.copy_bases(r, &seq[0]);
+          onSequence(name, seq);
+        }
+        windows++;
+      });
+      if (rc < 0) {
+        std::cerr << bz.error() << std::endl;
+        exit(1);
+      }
+      if (rc == 0)
+        std::cerr << "[mashmap-b200::skch::Sketch::build] " << fileName << ": BGZF, inflated on device " << dev << " in "
+                  << windows << " windows" << std::endl;
+    }
+    if (rc == 1 && !seqio::for_each_seq_in_file(fileName, allowed, param.target_prefix, onSequence)) exit(1);
     sequencesByFileInfo.push_back(seqCounter);
   }
   if (seqCounter == 0) {

@@ -803,6 +803,7 @@ struct Map::Impl {
   bool workerActive = false;
   std::vector<MappingResultsVector_t> results;
   std::vector<std::string> text;
+  std::unique_ptr<seqio::DeviceInflater> inflater;  // BGZF queries, on the run's first device
 
   Impl(const Parameters &p, const Sketch &s, PostProcessResultsFn_t f, Map &m, Clock::time_point tCtor = Clock::now())
       : param(p), refSketch(s), processMappingResults(f), self(m), bm(p, s)
@@ -900,8 +901,8 @@ struct Map::Impl {
   }
 
   /* onSequence for every record of a mapped FASTA file; the bases go from the file mapping straight into the pinned
-   * batch buffer, copied by all host threads just before the batch is mapped */
-  void ingestMapped(const seqio::FastaFile &ff)
+   * batch buffer, copied by all host threads just before the batch is mapped (a BGZF window: from the inflated text) */
+  void ingestMapped(const seqio::FastaText &ff)
   {
     struct CopyJob { size_t rec; uint64_t dst; };
     std::vector<CopyJob> jobs;
@@ -966,6 +967,23 @@ struct Map::Impl {
       if (!getenv("MM_SERIAL_INPUT") && ff.open(fileName, param.threads)) {  // plain FASTA: bulk path
         ingestMapped(ff);
         continue;
+      }
+      seqio::BgzfFasta bz;
+      if (!getenv("MM_SERIAL_INPUT") && bz.open(fileName)) {  // BGZF FASTA: inflated on the device, window by window
+        const int dev = param.devices.empty() ? param.device : param.devices[0];
+        if (!inflater) inflater.reset(new seqio::DeviceInflater(dev));
+        uint64_t windows = 0;
+        const int rc = bz.for_each_window(*inflater, seqio::bgzf_window_bytes(param.batch_bases), param.threads,
+                                          [&](const seqio::FastaText &t) { ingestMapped(t); windows++; });
+        if (rc < 0) {
+          std::cerr << bz.error() << std::endl;
+          exit(1);
+        }
+        if (rc == 0) {
+          std::cerr << "[mashmap-b200::skch::Map::mapQuery] " << fileName << ": BGZF, inflated on device " << dev << " in "
+                    << windows << " windows" << std::endl;
+          continue;
+        }
       }
       bool ok = seqio::for_each_seq_in_file(fileName, {}, "", [&](const std::string &name, const std::string &seq) { onSequence(name, seq); });
       if (!ok) exit(1);

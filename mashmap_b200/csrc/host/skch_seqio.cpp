@@ -5,6 +5,9 @@
 #include <sys/stat.h>
 #include <unistd.h>
 #include <zlib.h>
+
+#include "../../../include/mashmap_b200.h"
+#include "../mm_inflate.h"
 #if defined(__x86_64__)
 #include <immintrin.h>
 #endif
@@ -13,6 +16,7 @@
 #include <atomic>
 #include <cstring>
 #include <iostream>
+#include <memory>
 #include <thread>
 #include <vector>
 
@@ -135,6 +139,14 @@ bool FastaFile::open(const std::string &filename, int threads)
   data_ = (const char *)m;
   if (data_[0] != '>') return false; /* gzip magic, FASTQ, anything else: the line reader handles those */
   madvise(m, size_, MADV_SEQUENTIAL);
+  parse(data_, size_, threads);
+  return true;
+}
+
+void FastaText::parse(const char *text, uint64_t size, int threads)
+{
+  data_ = text;
+  size_ = size;
   const int T = (int)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)std::max(1, threads), size_ / (1 << 20) + 1));
   /* 1. record starts: '>' at the beginning of a line, found independently in T byte ranges */
   std::vector<std::vector<uint64_t>> starts((size_t)T);
@@ -158,7 +170,7 @@ bool FastaFile::open(const std::string &filename, int threads)
   std::vector<uint64_t> all;
   for (auto &v : starts) all.insert(all.end(), v.begin(), v.end());
   /* 2. per record: header, sequence region, base count */
-  recs_.resize(all.size());
+  recs_.assign(all.size(), FastaRecord{});
   {
     std::atomic<size_t> next{0};
     std::vector<std::thread> pool;
@@ -192,10 +204,9 @@ bool FastaFile::open(const std::string &filename, int threads)
     }
     for (auto &th : pool) th.join();
   }
-  return true;
 }
 
-void FastaFile::copy_bases(const FastaRecord &r, char *dst) const
+void FastaText::copy_bases(const FastaRecord &r, char *dst) const
 {
   const char *c = data_ + r.seq_off, *ce = c + r.raw_len;
   while (c < ce) {
@@ -264,7 +275,7 @@ void pack_bases(const char *src, uint64_t n, uint8_t *dst)
   pack_scalar((const uint8_t *)src, n, dst);
 }
 
-void FastaFile::pack_bases(const FastaRecord &r, uint8_t *dst) const
+void FastaText::pack_bases(const FastaRecord &r, uint8_t *dst) const
 {
   /* lines are gathered into an even-sized stretch of text first (a line may have an odd length; nibble pairs must not
    * straddle two pack calls), then packed: the stretch stays in the L1/L2 cache */
@@ -284,6 +295,260 @@ void FastaFile::pack_bases(const FastaRecord &r, uint8_t *dst) const
     c = next;
   }
   if (fill) seqio::pack_bases(buf, fill, dst);
+}
+
+/* ---- BGZF ---- */
+
+void *BlockInflater::alloc(uint64_t bytes) { return malloc(bytes); }
+void BlockInflater::release(void *p) { free(p); }
+
+int HostInflater::inflate(const uint8_t *comp, const uint64_t *comp_off, const uint64_t *out_off, const uint32_t *crc,
+                          uint64_t n_blocks, uint8_t *out, int64_t *bad_block, std::string &error)
+{
+  static const struct CrcTab {
+    uint32_t t[256];
+    CrcTab() { mmi_crc_table(t, 0, 1); }
+  } tab;
+  std::unique_ptr<mmi_tables> t(new mmi_tables());
+  *bad_block = -1;
+  for (uint64_t i = 0; i < n_blocks; i++) {
+    const uint64_t on = out_off[i + 1] - out_off[i];
+    int rc = mmi_inflate(comp + comp_off[i], comp_off[i + 1] - comp_off[i], out + out_off[i], on, *t, 0, 1);
+    if (rc == MMI_OK && mmi_crc_finish(mmi_crc_share(tab.t, out + out_off[i], on, 0, 1), on) != crc[i]) rc = MMI_E_CRC;
+    if (rc != MMI_OK) {
+      *bad_block = (int64_t)i;
+      error = "inflate status " + std::to_string(rc);
+      return rc;
+    }
+  }
+  return 0;
+}
+
+DeviceInflater::DeviceInflater(int device)
+{
+  mm_inflater *h = nullptr;
+  if (mm_inflater_create(device, &h) != MM_OK) {
+    std::cerr << "[mashmap-b200] ERROR: mm_inflater_create: " << mm_inflater_error(nullptr) << std::endl;
+    exit(1);
+  }
+  inf_ = h;
+}
+
+DeviceInflater::~DeviceInflater() { mm_inflater_destroy((mm_inflater *)inf_); }
+
+int DeviceInflater::inflate(const uint8_t *comp, const uint64_t *comp_off, const uint64_t *out_off, const uint32_t *crc,
+                            uint64_t n_blocks, uint8_t *out, int64_t *bad_block, std::string &error)
+{
+  const int rc = mm_inflate_blocks((mm_inflater *)inf_, comp, comp_off, out_off, crc, n_blocks, out, bad_block);
+  if (rc != MM_OK) error = mm_inflater_error((mm_inflater *)inf_);
+  return rc;
+}
+
+void *DeviceInflater::alloc(uint64_t bytes)
+{
+  void *p = nullptr;
+  return mm_host_alloc(&p, bytes) == MM_OK ? p : nullptr;
+}
+
+void DeviceInflater::release(void *p) { mm_host_free(p); }
+
+uint64_t bgzf_window_bytes(uint64_t batch_bases) { return std::min<uint64_t>(std::max<uint64_t>(batch_bases, 1 << 16), 1ULL << 28); }
+
+namespace {
+
+inline uint32_t le16(const uint8_t *p) { return p[0] | ((uint32_t)p[1] << 8); }
+inline uint32_t le32(const uint8_t *p) { return le16(p) | (le16(p + 2) << 16); }
+
+struct Member {
+  uint64_t data_off, data_len, next;
+  uint32_t crc, isize;
+};
+
+/* 1: a complete BGZF member at p; 0: a gzip member for zlib (not BGZF, unusual header, or cut short); -1: no member
+ * starts at p (end of file, or trailing bytes that gzread ignores) */
+int scan_member(const uint8_t *d, uint64_t size, uint64_t p, Member &m)
+{
+  if (size - p < 2 || d[p] != 0x1F || d[p + 1] != 0x8B) return -1;
+  if (size - p < 12 || d[p + 2] != 8 || d[p + 3] != 4) return 0; /* FEXTRA alone: BGZF sets no other flag */
+  const uint64_t xlen = le16(d + p + 10), x0 = p + 12, x1 = x0 + xlen;
+  if (x1 > size) return 0;
+  uint64_t bsize = 0;
+  bool bc = false;
+  for (uint64_t q = x0; q + 4 <= x1;) {
+    const uint64_t slen = le16(d + q + 2);
+    if (d[q] == 'B' && d[q + 1] == 'C' && slen == 2 && q + 6 <= x1) { bsize = le16(d + q + 4); bc = true; }
+    q += 4 + slen;
+  }
+  const uint64_t total = bsize + 1;
+  if (!bc || total < 12 + xlen + 8 || p + total > size) return 0;
+  m.data_off = x1;
+  m.data_len = p + total - 8 - x1;
+  m.crc = le32(d + p + total - 8);
+  m.isize = le32(d + p + total - 4);
+  m.next = p + total;
+  return m.isize <= 65536 ? 1 : 0; /* BGZF blocks hold at most 64 KiB of text; zlib takes anything else */
+}
+
+}  // namespace
+
+BgzfFasta::~BgzfFasta()
+{
+  if (d_) munmap((void *)d_, size_);
+  if (fd_ >= 0) close(fd_);
+}
+
+bool BgzfFasta::open(const std::string &filename)
+{
+  path_ = filename;
+  fd_ = ::open(filename.c_str(), O_RDONLY);
+  if (fd_ < 0) return false;
+  struct stat st;
+  if (fstat(fd_, &st) != 0 || !S_ISREG(st.st_mode) || st.st_size < 18) return false;
+  size_ = (uint64_t)st.st_size;
+  void *m = mmap(nullptr, size_, PROT_READ, MAP_PRIVATE, fd_, 0);
+  if (m == MAP_FAILED) { size_ = 0; return false; }
+  d_ = (const uint8_t *)m;
+  madvise(m, size_, MADV_SEQUENTIAL);
+  Member mb;
+  return scan_member(d_, size_, 0, mb) == 1;
+}
+
+bool BgzfFasta::corrupt(uint64_t off, const std::string &why)
+{
+  error_ = "[mashmap-b200] ERROR: " + path_ + ": corrupt gzip/BGZF block at byte offset " + std::to_string(off) + ": " + why;
+  return false;
+}
+
+bool BgzfFasta::grow(BlockInflater &inf, Buf &b, uint64_t need)
+{
+  if (need <= b.cap) return true;
+  const uint64_t cap = std::max<uint64_t>(need, b.cap + b.cap / 2);
+  char *q = (char *)inf.alloc(cap);
+  if (!q) {
+    error_ = "[mashmap-b200] ERROR: cannot allocate " + std::to_string(cap) + " bytes of host memory to read " + path_;
+    return false;
+  }
+  if (b.used) memcpy(q, b.p, b.used);
+  if (b.p) inf.release(b.p);
+  b.p = q;
+  b.cap = cap;
+  return true;
+}
+
+/* appends text to b until it holds `target` bytes or the members end */
+bool BgzfFasta::fill(BlockInflater &inf, Buf &b, uint64_t target)
+{
+  while (b.used < target && !eof_) {
+    Member m;
+    const int kind = scan_member(d_, size_, pos_, m);
+    if (kind < 0) { eof_ = true; break; }
+    if (kind == 0) { /* one gzip member through zlib, as gzread would inflate it */
+      z_stream zs;
+      memset(&zs, 0, sizeof zs);
+      if (inflateInit2(&zs, 15 + 16) != Z_OK) return corrupt(pos_, "zlib cannot start");
+      const uint64_t start = pos_;
+      uint64_t in_left = size_ - pos_;
+      const uint8_t *in = d_ + pos_;
+      int rc = Z_OK;
+      while (true) {
+        if (!grow(inf, b, b.used + (1 << 20))) { inflateEnd(&zs); return false; }
+        zs.next_out = (Bytef *)b.p + b.used;
+        zs.avail_out = (uInt)std::min<uint64_t>(b.cap - b.used, 1u << 30);
+        const uInt feed = (uInt)std::min<uint64_t>(in_left, 1u << 30);
+        zs.next_in = (Bytef *)in;
+        zs.avail_in = feed;
+        const uInt out0 = zs.avail_out;
+        rc = inflate(&zs, Z_NO_FLUSH);
+        b.used += out0 - zs.avail_out;
+        in += feed - zs.avail_in;
+        in_left -= feed - zs.avail_in;
+        if (rc == Z_STREAM_END) break;
+        if (rc == Z_BUF_ERROR && in_left == 0) break; /* cut short: gzread hands over what inflated, then ends */
+        if (rc != Z_OK && rc != Z_BUF_ERROR) break;
+        if (in_left == 0 && zs.avail_out != 0) { rc = Z_BUF_ERROR; break; }
+      }
+      const char *msg = zs.msg;
+      inflateEnd(&zs);
+      if (rc == Z_STREAM_END) pos_ = (uint64_t)(in - d_);
+      else if (rc == Z_BUF_ERROR) eof_ = true;
+      else return corrupt(start, msg ? msg : "zlib error");
+      continue;
+    }
+    /* consecutive BGZF members up to the target, at least one: one call of the inflater */
+    coff_.assign(1, 0);
+    ooff_.assign(1, 0);
+    moff_.clear();
+    crc_.clear();
+    uint64_t p = pos_, out = 0;
+    while (true) {
+      moff_.push_back(p);
+      crc_.push_back(m.crc);
+      coff_.push_back(coff_.back() + m.data_len);
+      out += m.isize;
+      ooff_.push_back(out);
+      p = m.next;
+      if (b.used + out >= target || scan_member(d_, size_, p, m) != 1) break;
+    }
+    stage_.resize(coff_.back());
+    for (size_t i = 0; i < moff_.size(); i++) {
+      Member mi;
+      scan_member(d_, size_, moff_[i], mi);
+      memcpy(stage_.data() + coff_[i], d_ + mi.data_off, mi.data_len);
+    }
+    if (!grow(inf, b, b.used + out + 1)) return false;
+    int64_t bad = -1;
+    std::string why;
+    if (inf.inflate(stage_.data(), coff_.data(), ooff_.data(), crc_.data(), moff_.size(), (uint8_t *)b.p + b.used, &bad, why) != 0)
+      return corrupt(bad >= 0 && (size_t)bad < moff_.size() ? moff_[(size_t)bad] : pos_, why);
+    b.used += out;
+    pos_ = p;
+  }
+  return true;
+}
+
+int BgzfFasta::for_each_window(BlockInflater &inf, uint64_t window_bytes, int threads, const std::function<void(const FastaText &)> &fn)
+{
+  Buf cur, nxt;
+  struct Release {
+    BlockInflater &inf;
+    Buf &a, &b;
+    ~Release() { if (a.p) inf.release(a.p); if (b.p) inf.release(b.p); }
+  } release{inf, cur, nxt};
+  window_bytes = std::max<uint64_t>(window_bytes, 1);
+  if (!fill(inf, cur, window_bytes)) return -1;
+  if (cur.used == 0 || cur.p[0] != '>') return 1;
+  FastaText text;
+  while (cur.used) {
+    /* cut after the last record start that is not the window's first byte; a record longer than the window grows it */
+    uint64_t cut = cur.used;
+    if (!eof_) {
+      cut = 0;
+      for (uint64_t q = cur.used; q > 1;) {
+        const char *g = (const char *)memrchr(cur.p + 1, '>', q - 1);
+        if (!g) break;
+        if (g[-1] == '\n') { cut = (uint64_t)(g - cur.p); break; }
+        q = (uint64_t)(g - cur.p);
+      }
+      if (cut == 0) {
+        if (!fill(inf, cur, cur.used + window_bytes)) return -1;
+        continue;
+      }
+    }
+    const uint64_t carry = cur.used - cut;
+    if (!grow(inf, nxt, carry + window_bytes + 1)) return -1;
+    memcpy(nxt.p, cur.p + cut, carry);
+    nxt.used = carry;
+    bool ok = true;
+    std::thread next;
+    if (!eof_) next = std::thread([&]() { ok = fill(inf, nxt, carry + window_bytes); });
+    text.parse(cur.p, cut, threads);
+    fn(text);
+    if (next.joinable()) next.join();
+    if (!ok) return -1;
+    std::swap(cur, nxt);
+    nxt.used = 0;
+  }
+  return 0;
 }
 
 }  // namespace seqio

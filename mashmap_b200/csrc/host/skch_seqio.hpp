@@ -39,27 +39,115 @@ struct FastaRecord {
   uint64_t seq_len;   /* bases = raw_len minus the newlines */
 };
 
-class FastaFile {
+/* the records of a FASTA text held in memory (a mapped file, or one window of an inflated BGZF file) */
+class FastaText {
  public:
-  FastaFile() = default;
-  ~FastaFile();
-  FastaFile(const FastaFile &) = delete;
-  /* false if the file is not a plain FASTA file that can be mapped (gzip, FASTQ, pipe ...): use for_each_seq_in_file */
-  bool open(const std::string &filename, int threads);
+  /* cuts text[0, size) into records with up to `threads` host threads; text[0] is '>' and stays valid while in use */
+  void parse(const char *text, uint64_t size, int threads);
   const std::vector<FastaRecord> &records() const { return recs_; }
   const char *data() const { return data_; }
+  uint64_t size() const { return size_; }
   std::string name(const FastaRecord &r) const { return std::string(data_ + r.name_off, r.name_len); }
   /* copies the record's bases to dst (seq_len bytes) */
   void copy_bases(const FastaRecord &r, char *dst) const;
   /* the record's bases as nibbles (pack_bases below) to dst ((seq_len + 1) / 2 bytes), newlines dropped on the way */
   void pack_bases(const FastaRecord &r, uint8_t *dst) const;
 
- private:
+ protected:
   const char *data_ = nullptr;
   uint64_t size_ = 0;
-  int fd_ = -1;
   std::vector<FastaRecord> recs_;
 };
+
+class FastaFile : public FastaText {
+ public:
+  FastaFile() = default;
+  ~FastaFile();
+  FastaFile(const FastaFile &) = delete;
+  /* false if the file is not a plain FASTA file that can be mapped (gzip, FASTQ, pipe ...): use for_each_seq_in_file */
+  bool open(const std::string &filename, int threads);
+
+ private:
+  int fd_ = -1;
+};
+
+/*
+ * The one step of the BGZF reader that a caller chooses: inflate raw DEFLATE blocks, with mm_inflate_blocks' contract
+ * (include/mashmap_b200.h). The program passes DeviceInflater; the tests pass HostInflater (the host build of
+ * mm_inflate.h) or a fake. alloc / release give the reader's text buffers (pinned ones for the device).
+ */
+class BlockInflater {
+ public:
+  virtual ~BlockInflater() = default;
+  /* 0, or nonzero with *bad_block = the failing block's index (or -1) and `error` saying why */
+  virtual int inflate(const uint8_t *comp, const uint64_t *comp_off, const uint64_t *out_off, const uint32_t *crc,
+                      uint64_t n_blocks, uint8_t *out, int64_t *bad_block, std::string &error) = 0;
+  virtual void *alloc(uint64_t bytes);
+  virtual void release(void *p);
+};
+
+class HostInflater : public BlockInflater {
+ public:
+  int inflate(const uint8_t *comp, const uint64_t *comp_off, const uint64_t *out_off, const uint32_t *crc,
+              uint64_t n_blocks, uint8_t *out, int64_t *bad_block, std::string &error) override;
+};
+
+class DeviceInflater : public BlockInflater {
+ public:
+  /* exits the program (status 1) if the device cannot be used */
+  explicit DeviceInflater(int device);
+  ~DeviceInflater() override;
+  int inflate(const uint8_t *comp, const uint64_t *comp_off, const uint64_t *out_off, const uint32_t *crc,
+              uint64_t n_blocks, uint8_t *out, int64_t *bad_block, std::string &error) override;
+  void *alloc(uint64_t bytes) override;
+  void release(void *p) override;
+
+ private:
+  void *inf_ = nullptr;
+};
+
+/*
+ * FASTA in BGZF (bgzip) members, read window by window. A member is BGZF when its gzip header has FEXTRA with a 'BC'
+ * subfield of length 2; its BSIZE, CRC32 and ISIZE place its data and its text before anything is inflated, so a
+ * window's members go to the BlockInflater in one call. A member that is not BGZF, or one cut short by the end of the
+ * file, is inflated on the host by zlib, in order, and bytes after the last member are ignored: the text is the one
+ * gzread gives the line reader. A corrupt member is an error, where gzread would end the text early.
+ */
+class BgzfFasta {
+ public:
+  BgzfFasta() = default;
+  ~BgzfFasta();
+  BgzfFasta(const BgzfFasta &) = delete;
+  /* false if the file cannot be mapped or its first member is not BGZF: the line reader handles it */
+  bool open(const std::string &filename);
+  /*
+   * Inflates the text in windows of about window_bytes (grown while one record does not fit), cuts each window at its
+   * last record start, carries the rest into the next window, and hands each window's records, parsed by `threads`
+   * threads, to fn. Window i+1 is inflated while fn runs on window i. Returns 0; 1 if the text does not start with '>'
+   * (nothing was handed over: the line reader handles the file); -1 on a corrupt member (error() names the file and the
+   * member's byte offset).
+   */
+  int for_each_window(BlockInflater &inf, uint64_t window_bytes, int threads, const std::function<void(const FastaText &)> &fn);
+  const std::string &error() const { return error_; }
+
+ private:
+  struct Buf { char *p = nullptr; uint64_t cap = 0, used = 0; };
+  bool grow(BlockInflater &inf, Buf &b, uint64_t need);
+  bool fill(BlockInflater &inf, Buf &b, uint64_t target);
+  bool corrupt(uint64_t off, const std::string &why);
+
+  std::string path_, error_;
+  const uint8_t *d_ = nullptr;
+  uint64_t size_ = 0, pos_ = 0;
+  bool eof_ = false;
+  int fd_ = -1;
+  std::vector<uint8_t> stage_;
+  std::vector<uint64_t> coff_, ooff_, moff_;
+  std::vector<uint32_t> crc_;
+};
+
+/* text bytes per BGZF window for a run of --batchBases b: b, kept within [64 KiB, 256 MiB] */
+uint64_t bgzf_window_bytes(uint64_t batch_bases);
 
 /*
  * The device's input format (include/mashmap_b200.h, mm_map_segments_packed): one nibble per base, base i of the

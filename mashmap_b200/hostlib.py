@@ -54,6 +54,17 @@ def lib():
         L.skch_tail_map_read.restype = C.c_char_p
         L.skch_fasta_readers_diff.argtypes = [C.c_char_p, C.c_int, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
         L.skch_fasta_readers_diff.restype = C.c_int64
+        L.skch_mmi_inflate.argtypes = [C.c_char_p, C.c_uint64, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint32)]
+        L.skch_bgzf_error.restype = C.c_char_p
+        L.skch_bgzf_text.argtypes = [C.c_char_p, C.c_uint64, C.c_int, C.c_int64, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64),
+                                     C.POINTER(C.c_uint64)]
+        L.skch_bgzf_text.restype = C.c_int64
+        L.skch_gzread_text.argtypes = [C.c_char_p, C.c_void_p, C.c_uint64]
+        L.skch_gzread_text.restype = C.c_int64
+        L.skch_bgzf_readers_diff.argtypes = [C.c_char_p, C.c_uint64, C.c_int, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
+        L.skch_bgzf_readers_diff.restype = C.c_int64
+        L.skch_bgzf_read_digest.argtypes = [C.c_char_p, C.c_uint64, C.c_int, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64),
+                                            C.POINTER(C.c_uint64)]
         L.skch_index_from_minmers.argtypes = [C.c_void_p, C.c_uint64, C.c_int, C.c_float]
         L.skch_index_from_minmers.restype = C.c_void_p
         L.skch_index_build.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float]
@@ -289,6 +300,46 @@ def fasta_readers_diff(path, threads=4):
     reader declines the file (gzip, FASTQ ...)"""
     nr, nb = C.c_uint64(), C.c_uint64()
     d = lib().skch_fasta_readers_diff(path.encode(), threads, C.byref(nr), C.byref(nb))
+    return d, nr.value, nb.value
+
+
+def mmi_inflate(comp, out_len):
+    """the host build of mm_inflate.h on one raw DEFLATE stream that must inflate to exactly out_len bytes:
+    (mmi_status, text, CRC-32)"""
+    comp = bytes(comp)
+    out = np.zeros(max(int(out_len), 1), dtype=np.uint8)
+    crc = C.c_uint32()
+    rc = lib().skch_mmi_inflate(comp, len(comp), out.ctypes.data_as(C.c_void_p), int(out_len), C.byref(crc))
+    return rc, out[: int(out_len)].tobytes(), crc.value
+
+
+def bgzf_text(path, window_bytes=1 << 20, threads=2, fail_block=-1):
+    """(text, windows, inflater calls) as the windowed BGZF reader hands the text over (host inflater); text is None if
+    the reader declines the file; raises RuntimeError with the reader's message on an error"""
+    nw, nc = C.c_uint64(), C.c_uint64()
+    n = lib().skch_bgzf_text(path.encode(), window_bytes, threads, fail_block, None, 0, C.byref(nw), C.byref(nc))
+    if n == -1:
+        return None, 0, 0
+    if n < 0:
+        raise RuntimeError(lib().skch_bgzf_error().decode())
+    buf = np.zeros(max(n, 1), dtype=np.uint8)
+    lib().skch_bgzf_text(path.encode(), window_bytes, threads, fail_block, buf.ctypes.data_as(C.c_void_p), n, C.byref(nw), C.byref(nc))
+    return buf[:n].tobytes(), nw.value, nc.value
+
+
+def gzread_text(path):
+    """everything zlib's gzread gives for the file: the text the line reader reads"""
+    n = lib().skch_gzread_text(path.encode(), None, 0)
+    buf = np.zeros(max(n, 1), dtype=np.uint8)
+    lib().skch_gzread_text(path.encode(), buf.ctypes.data_as(C.c_void_p), n)
+    return buf[:n].tobytes()
+
+
+def bgzf_readers_diff(path, window_bytes, threads=2):
+    """(differences, records, bases): the windowed BGZF reader (host inflater) against the line reader; -1 if it
+    declines the file"""
+    nr, nb = C.c_uint64(), C.c_uint64()
+    d = lib().skch_bgzf_readers_diff(path.encode(), window_bytes, threads, C.byref(nr), C.byref(nb))
     return d, nr.value, nb.value
 
 
