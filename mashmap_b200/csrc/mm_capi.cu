@@ -530,6 +530,15 @@ int read_back(mm_ctx *c, const void *dev, void *out, size_t bytes) /* bytes: who
 }
 #define RD(c, dev, out) do { int rc__ = read_back((c), (dev), (out), sizeof *(out)); if (rc__) return rc__; } while (0)
 
+/* tests: MM_CAND_ELEMS / MM_LOCI_ELEMS set the room a fresh candidate / locus buffer starts with (the locus buffer: room
+ * beyond the stream kernel's fixed slots), so that a small batch takes the regrow paths. Read on every call; a buffer that
+ * has grown is never shrunk. -1 when unset. */
+int64_t test_elems(const char *name, int64_t lo)
+{
+  const char *e = getenv(name);
+  return e ? std::max<int64_t>(lo, strtoll(e, nullptr, 10)) : -1;
+}
+
 /* returned by run_l2_stream when its own work areas cannot be allocated: the general kernel maps the batch instead */
 constexpr int L2_STREAM_NO_ROOM = 1;
 constexpr int L2_NONE_APPENDED = 2; /* see run_l2_loci */
@@ -589,7 +598,9 @@ int run_l2_stream(mm_ctx *c)
       return L2_STREAM_NO_ROOM;
     }
   }
-  if (c->d_loci.capacity() < nc * LPC + 1024) CU(c, c->d_loci.reserve(nc * LPC + nc / 8 + 4096));
+  const int64_t loci0 = test_elems("MM_LOCI_ELEMS", 0);
+  if (loci0 >= 0) CU(c, c->d_loci.reserve(nc * LPC + (uint64_t)loci0));
+  else if (c->d_loci.capacity() < nc * LPC + 1024) CU(c, c->d_loci.reserve(nc * LPC + nc / 8 + 4096));
   ZERO_WORDS(c, c->d_l2_rec_off.get() + nc, 2);
   CU(c, mm_launch_l2_ranges(c->params, c->ix, make_batch(c), (uint32_t)nc, c->d_scan_tmp.get(), c->d_scan_tmp.capacity(),
                             c->stream));
@@ -686,8 +697,9 @@ int run_pipeline(mm_ctx *c, int l1_mode = MM_L1_FULL)
   c->batch_mapped = false;
   c->l1_best_ready = false;
   const uint64_t n_segs = c->n_segs;
-  CU(c, c->d_cands.reserve(2 * n_segs + 1024));
-  CU(c, c->d_loci.reserve(2 * c->d_cands.capacity()));
+  const int64_t cand0 = test_elems("MM_CAND_ELEMS", 1), loci0 = test_elems("MM_LOCI_ELEMS", 0);
+  CU(c, c->d_cands.reserve(cand0 >= 0 ? (uint64_t)cand0 : 2 * n_segs + 1024));
+  CU(c, c->d_loci.reserve(loci0 >= 0 ? (uint64_t)loci0 : 2 * c->d_cands.capacity()));
   uint64_t pool0 = 32ULL << 20; /* interval points the bump pool holds at first (grown on demand below) */
   if (const char *e = getenv("MM_L1_POOL_ELEMS")) pool0 = std::max<uint64_t>(1024, strtoull(e, nullptr, 10)); /* tests: force the regrow path */
   if ((rc = ensure_scratch(c, c->d_scratch ? c->d_scratch.capacity() - c->scratch_pool : pool0))) return rc;

@@ -647,6 +647,10 @@ int mm_build_index_device(const mm_params &p, const uint8_t *d_seq, const uint64
       const uint64_t fit = room / L.bytes / 128 * 128;
       if (fit < threads) threads = (uint32_t)std::max<uint64_t>(fit, 128);
     }
+    if (const char *e = getenv("MM_INDEX_MACHINES")) { /* tests: a small grid, so that each machine scans many chunks */
+      const uint32_t cap = (uint32_t)std::max<long>(128, (strtol(e, nullptr, 10) + 127) / 128 * 128);
+      threads = std::min(threads, cap);
+    }
     const uint32_t grid = threads / 128;
     unsigned char *slabs = nullptr;
     CE(dv.alloc(slabs, (uint64_t)threads * L.bytes));
@@ -683,49 +687,81 @@ int mm_build_index_device(const mm_params &p, const uint8_t *d_seq, const uint64
       return cudaGetLastError();
     };
 
-    /* ---- acceptance chain, fix-up rounds ----
+    /* ---- acceptance, fix-up rounds ----
      * A chunk is good if it starts a contig and ran clean, or if its predecessor is good, it ran clean (no failure, no
-     * expired heap entry taken) and its state digest at its start equals its predecessor's at its end. Runs of chunks that
-     * are not good form chains; a chain always starts right after a chunk that was accepted on its pass-1 (warm-up) run, is
-     * re-scanned by one thread from that chunk's exact end state, and is extended and re-scanned as a whole if the chunk
-     * that follows it does not match the chain's new end state. */
-    std::vector<uint8_t> ok(n_chunks, 0);
+     * expired heap entry taken) and its state digest at its start equals its predecessor's at its end. A chunk that is not
+     * good starts a chain of rejected chunks, or joins the chain right before it; a chain starts right after a good chunk
+     * and is re-scanned by one thread from that chunk's exact end state.
+     * A chunk right after a chain that is not re-scanned yet is decided in a later round, against the chain's exact end
+     * state (it is pending, and so is every chunk after it), unless it failed on its own, which rejects it whatever came
+     * before it: then it joins the chain at once. A chain whose next chunk does not match its new end state is extended by
+     * that chunk and re-scanned as a whole. So each contig has at most one dirty chain per round, and all of the contig
+     * before that chain is good: the chain's start state (chunk first-1 and the resolved exports of first-2) depends on
+     * nothing that is rewritten in the same round. The export resolution stops at the dirty chain too, since the exports of
+     * pending chunks inherit record starts from the chunks the chain is about to rewrite; what it resolved is final, so
+     * the next round resolves from there on. A round decides at least the chunk after each chain it re-scanned, so there
+     * are at most as many rounds as chunks; a contig with r separate runs of rejected chunks takes about r rounds. */
+    enum : uint8_t { CH_GOOD, CH_DIRTY, CH_PENDING };
+    std::vector<uint8_t> state(n_chunks, CH_PENDING);
     std::vector<int32_t> in_chain(n_chunks, -1);
     struct HostChain { uint32_t first, n; bool dirty; };
     std::vector<HostChain> hchains;
+    std::vector<uint32_t> resolve_n(cf.size()); /* per contig: the chunks whose exports the next resolution may touch */
+    std::vector<uint32_t> resolved(cf.size(), 0); /* per contig: its chunks up to this one have resolved exports */
+    std::vector<uint32_t> res_first(cf.size()), res_n(cf.size());
+    auto resolve_upto = [&](const std::vector<uint32_t> &limit) { /* resolve chunks (resolved, limit) of each contig */
+      for (size_t g = 0; g < cf.size(); g++) {
+        res_first[g] = cf[g] + resolved[g];
+        res_n[g] = limit[g] > resolved[g] ? limit[g] - resolved[g] : 0;
+        if (limit[g] > resolved[g]) resolved[g] = limit[g] - 1;
+      }
+      cudaError_t e = cudaMemcpyAsync(d_cf, res_first.data(), cf.size() * 4, cudaMemcpyHostToDevice, st);
+      if (e == cudaSuccess) e = cudaMemcpyAsync(d_cn, res_n.data(), cf.size() * 4, cudaMemcpyHostToDevice, st);
+      return e == cudaSuccess ? resolve() : e;
+    };
     wm_record *fix = nullptr;
     std::vector<uint64_t> fix_off(n_chunks, 0);
-    uint64_t fix_used = 0, fix_capacity = 0;
+    uint64_t fix_used = 0, fix_capacity = 0, decided_before = 0;
     const uint32_t fix_cap = (uint32_t)(3 * chunk_len + s + 64); /* at most three records per position */
-    for (int round = 0; round < 256; round++) {
-      for (uint32_t c = 0; c < n_chunks; c++) {
-        const bool first = chunks[c].a == 0;
-        bool good;
-        if (in_chain[c] >= 0) {
-          if (outs[c].flags & 3u) { err = "window machine capacity exceeded while re-scanning a chunk"; return MM_ECAPACITY; }
-          good = !hchains[(size_t)in_chain[c]].dirty;
-        } else if (first) {
-          good = !(outs[c].flags & 3u);
-        } else {
-          good = ok[c - 1] && !(outs[c].flags & 7u) && outs[c].d_start == outs[c - 1].d_end;
-        }
-        ok[c] = good ? 1 : 0;
-        if (!good && in_chain[c] < 0) {
-          if (!first && in_chain[c - 1] >= 0) { /* the chain before it grows by this chunk and is re-scanned as a whole */
-            HostChain &hc = hchains[(size_t)in_chain[c - 1]];
-            hc.n++; hc.dirty = true;
-            in_chain[c] = in_chain[c - 1];
+    for (uint32_t round = 0;; round++) {
+      uint64_t decided = 0;
+      for (size_t g = 0; g < cf.size(); g++) {
+        resolve_n[g] = cnn[g];
+        for (uint32_t c = cf[g]; c < cf[g] + cnn[g]; c++) {
+          const bool first = c == cf[g];
+          if (in_chain[c] >= 0) { /* re-scanned in an earlier round: exact (a chain is only dirty from the chunk that made it so on) */
+            if (outs[c].flags & 3u) { err = "window machine capacity exceeded while re-scanning a chunk"; return MM_ECAPACITY; }
+            state[c] = CH_GOOD;
           } else {
-            in_chain[c] = (int32_t)hchains.size();
-            hchains.push_back(HostChain{c, 1, true});
+            const uint8_t prev = first ? CH_GOOD : state[c - 1];
+            const bool own_fail = (outs[c].flags & (first ? 3u : 7u)) != 0;
+            if (prev == CH_GOOD && !own_fail && (first || outs[c].d_start == outs[c - 1].d_end)) {
+              state[c] = CH_GOOD;
+            } else if (prev == CH_PENDING || (prev == CH_DIRTY && !own_fail)) {
+              state[c] = CH_PENDING;
+            } else {
+              if (!first && in_chain[c - 1] >= 0) { /* the chain before it grows by this chunk and is re-scanned as a whole */
+                HostChain &hc = hchains[(size_t)in_chain[c - 1]];
+                hc.n++; hc.dirty = true;
+                in_chain[c] = in_chain[c - 1];
+              } else {
+                in_chain[c] = (int32_t)hchains.size();
+                hchains.push_back(HostChain{c, 1, true});
+              }
+              state[c] = CH_DIRTY;
+              resolve_n[g] = std::min(resolve_n[g], hchains[(size_t)in_chain[c]].first - cf[g]);
+            }
           }
+          if (state[c] != CH_PENDING) decided++;
         }
       }
       std::vector<wb_chain> chains;
       for (auto &hc : hchains)
         if (hc.dirty) chains.push_back(wb_chain{hc.first, hc.n, 0});
       if (chains.empty()) break;
-      out->fix_rounds = (uint32_t)round + 1;
+      if (round > 0 && decided <= decided_before) { err = "chunk stitching made no progress"; return MM_ECUDA; }
+      decided_before = decided;
+      out->fix_rounds = round + 1;
       uint64_t need = 0;
       for (auto &cn : chains) { cn.out_offset = fix_used + need; need += (uint64_t)cn.n * fix_cap; }
       if ((fix_used + need) * sizeof(wm_record) > (48ULL << 30)) { err = "too many chunks need an exact re-scan (N-rich / low-complexity reference): use the host builder"; return MM_ECAPACITY; }
@@ -741,7 +777,7 @@ int mm_build_index_device(const mm_params &p, const uint8_t *d_seq, const uint64
       for (auto &cn : chains)
         for (uint32_t q = 0; q < cn.n; q++) fix_off[cn.first + q] = cn.out_offset + (uint64_t)q * fix_cap;
       fix_used += need;
-      CE(resolve()); /* the re-scan takes record starts from the exports of the chunks before the chain */
+      CE(resolve_upto(resolve_n)); /* the re-scan takes record starts from the exports of the chunks before the chain */
       wb_chain *d_chains = nullptr;
       CE(dv.alloc(d_chains, chains.size()));
       CE(cudaMemcpyAsync(d_chains, chains.data(), chains.size() * sizeof(wb_chain), cudaMemcpyHostToDevice, st));
@@ -762,10 +798,10 @@ int mm_build_index_device(const mm_params &p, const uint8_t *d_seq, const uint64
     out->n_fixed_chunks = 0;
     for (auto &hc : hchains) out->n_fixed_chunks += hc.n;
     for (uint32_t c = 0; c < n_chunks; c++)
-      if (!ok[c]) { err = "chunk stitching did not converge"; return MM_ECUDA; }
+      if (state[c] != CH_GOOD) { err = "chunk stitching did not converge"; return MM_ECUDA; }
     dv.free_now(slabs);
 
-    CE(resolve());
+    CE(resolve_upto(cnn));
     k_patch_starts<<<n_chunks, 128, 0, st>>>(d_chunks, d_outs, n_chunks, rec, rec_cap, d_ex, stride, d_err);
     CE(cudaGetLastError());
     uint32_t h_err = 0;

@@ -180,3 +180,136 @@ def test_index_degenerate_contigs(workdir, monkeypatch, w, s, k):
     # this is reported, not asserted)
     print(f"device {len(mi)} records / reference {len(exact)}; outside tie groups {len(a)} / {len(b)}, identical: {same}")
     ctx.close()
+
+
+# ---- small grids, many chains, rejected blocks ------------------------------------------------------------------------
+# MM_INDEX_MACHINES caps the window-scan grid, so that each machine scans many chunks one after another in its own slab.
+# A low-complexity block makes about two records per position, more than a chunk's record buffer (chunk/4 + s + 64)
+# holds: every chunk with enough of it is rejected and re-scanned exactly.
+LOW_COMPLEXITY = b"ACACACACACGTGTGTGTGT"
+
+
+def _low_block(n):
+    return np.frombuffer(LOW_COMPLEXITY * (n // len(LOW_COMPLEXITY)), np.uint8)
+
+
+def _device_minmers(genome, k, w, s, monkeypatch, chunk, machines=None):
+    from mashmap_b200 import capi
+
+    monkeypatch.setenv("MM_INDEX_CHUNK", str(chunk))
+    if machines is not None:
+        monkeypatch.setenv("MM_INDEX_MACHINES", str(machines))
+    ctx = capi.Context(kmer_size=k, seg_length=w, sketch_size=s)
+    try:
+        seqs = np.concatenate(genome).astype(np.uint8)
+        offs = np.zeros(len(genome) + 1, dtype=np.uint64)
+        offs[1:] = np.cumsum([len(c) for c in genome])
+        st = ctx.index_build(seqs, offs, kmer_pct_threshold=0.0, keep_lookup=True)
+        return st, ctx.index_download()[0]
+    finally:
+        ctx.close()
+
+
+def _assert_host_minmers(mi, genome, k, w, s):
+    """the device index against the host builder with the device's tie rule (see test_index_degenerate_contigs)"""
+    from mashmap_b200 import hostlib
+
+    want = np.concatenate([hostlib.add_minmers(g, k, w, s, seq_id=i, stable_ties=True) for i, g in enumerate(genome)])
+    assert len(mi) == len(want), (len(mi), len(want))
+    for f in ("hash", "wpos", "wpos_end", "seqId", "strand"):
+        assert np.array_equal(mi[f], want[f]), f
+
+
+def _touched_chunks(begin, end, k, chunk):
+    """the chunks (of k-mer positions) whose k-mers read a base of [begin, end)"""
+    return set(range(max(0, begin - k + 1) // chunk, (end - 1) // chunk + 1))
+
+
+@pytest.mark.parametrize("case", ["random", "panel", "big"])
+def test_index_many_chunks_per_machine(workdir, monkeypatch, case):
+    """a grid of 128 machines over 1,024-position chunks: every machine scans many chunks in turn, reusing its slab"""
+    monkeypatch.setenv("MM_INDEX_MACHINES", "128")
+    if case == "random":
+        d = datasets.make_random_set(workdir, tag="ixr")
+        args = ["-r", d["ref"], "-q", d["qry"], "-s", "5000", "--pi", "85", "-t", "4"]
+    elif case == "panel":
+        d = datasets.make_panel_set(workdir, tag="ixp")
+        args = ["-r", d["ref"], "-q", d["qry"], "-s", "5000", "--pi", "85", "--kmerThreshold", "5", "-t", "4"]
+    else:
+        d = datasets.make_big_random_set(workdir, tag="ixb", n_contigs=4, contig_len=1_000_000, n_reads=2)
+        args = ["-r", d["ref"], "-q", d["qry"], "-s", "5000", "--pi", "95", "--dense", "-t", "8"]
+    st = build_and_compare(d, args, chunk=1024, monkeypatch=monkeypatch, expect_fixed=False if case != "panel" else None)
+    assert st["n_chunks"] >= 8 * 128, st  # at least eight chunks per machine (about thirty on the big set)
+
+
+def test_index_more_chains_than_machines(monkeypatch):
+    """240 contigs, each with a low-complexity block, on a grid of 128 machines. The first rejected chunk of a contig is
+    decided in round 0 (all of the contig before it is good), so round 0 re-scans one chain per contig: 240 chains, more
+    than the grid's slabs"""
+    k, w, s, chunk = 16, 500, 10, 1024
+    rng = np.random.default_rng(23)
+    low = _low_block(800)
+    genome = []
+    for i in range(240):
+        g = synth.random_sequence(4000 + 37 * (i % 50), rng)
+        at = 1100 + 7 * (i % 100)
+        g[at : at + len(low)] = low
+        genome.append(g)
+    st, mi = _device_minmers(genome, k, w, s, monkeypatch, chunk, machines=128)
+    print("device index:", st)
+    assert st["n_fixed_chunks"] >= len(genome), st
+    _assert_host_minmers(mi, genome, k, w, s)
+
+
+def test_index_one_rejected_block_rescans_only_its_chunks(monkeypatch):
+    """a 1.1 Mbp contig of random sequence with one low-complexity block whose end sweeps the offsets 0 .. warm before a
+    chunk boundary: only the chunks the block touches (and at most two after them) are re-scanned, not the rest of the
+    contig, and the index is the host builder's"""
+    k, w, s, chunk = 19, 1000, 20, 4096
+    warm = w + 2 * k + 64  # the warm-up of mm_index_build.cu
+    rng = np.random.default_rng(29)
+    base = synth.random_sequence(1_100_000, rng)
+    low = _low_block(3000)
+    boundary = 40 * chunk
+    n_chunks = (len(base) - k + 1 + chunk - 1) // chunk
+    rounds = {}
+    for end in sorted({0, 1, k - 1, k, w // 2, w - 1, w, w + 1, w + k, warm - 64, warm - 1, warm}):
+        g = base.copy()
+        e = boundary - end
+        g[e - len(low) : e] = low
+        st, mi = _device_minmers([g], k, w, s, monkeypatch, chunk)
+        touched = _touched_chunks(e - len(low), e, k, chunk)
+        print(f"block end {end} before a boundary: {len(touched)} chunks touched, {st['n_fixed_chunks']} re-scanned in "
+              f"{st['fix_rounds']} rounds, of {n_chunks}")
+        assert st["n_chunks"] == n_chunks
+        assert 1 <= st["n_fixed_chunks"] <= len(touched) + 2, (end, st)
+        _assert_host_minmers(mi, [g], k, w, s)
+        rounds[end] = st["fix_rounds"]
+    # One round at every offset: the chunk after the re-scanned block always matched the block's exact end state, so the
+    # branch that extends a re-scanned chain is not reached here. It stays, since a chunk that does not match can only be
+    # re-scanned as part of that chain: a new chain would have to start from a rejected chunk's untrusted warm-up state.
+    # fix_rounds >= 2 is reached by separate rejected runs (test_index_many_rejected_blocks_in_one_contig).
+    print("rounds by offset:", rounds)
+
+
+def test_index_many_rejected_blocks_in_one_contig(monkeypatch):
+    """300 low-complexity blocks 1, 2 and 3 chunks apart in one contig: one round per separate run of rejected chunks, each
+    chain bounded by the chunks its block touches, and the index is the host builder's"""
+    k, w, s, chunk = 19, 1000, 20, 4096
+    rng = np.random.default_rng(31)
+    low = _low_block(3000)
+    starts, c = [], 2
+    for i in range(300):
+        starts.append(c * chunk + 200)
+        c += 1 + i % 3
+    g = synth.random_sequence((c + 2) * chunk, rng)
+    allowed = set()
+    for a in starts:
+        g[a : a + len(low)] = low
+        t = _touched_chunks(a, a + len(low), k, chunk)
+        allowed |= t | {max(t) + 1}
+    st, mi = _device_minmers([g], k, w, s, monkeypatch, chunk, machines=128)
+    print("device index:", st, f"{len(allowed)} chunks touched or right after a block")
+    assert len(starts) <= st["n_fixed_chunks"] <= len(allowed), st
+    assert st["fix_rounds"] >= 2, st
+    _assert_host_minmers(mi, [g], k, w, s)

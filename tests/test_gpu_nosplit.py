@@ -141,8 +141,9 @@ def reference_fragment_digests(R, d, ridx, lens):
     return ND.get("fragments", R.key)
 
 
-def map_whole_queries(R, bases, segs):
-    """(digests per fragment, seg_res, ctx diag) through mm_map_segments, checked equal to the resident path"""
+def map_whole_queries(R, bases, segs, fetched=None):
+    """(digests per fragment, seg_res, ctx diag) through mm_map_segments, checked equal to the resident path; the resident
+    path's candidates and loci are appended to `fetched` when it is a list"""
     from mashmap_b200 import capi
 
     ctx = capi.Context(kmer_size=R.p.kmerSize, seg_length=R.p.segLength, sketch_size=R.p.sketchSize,
@@ -159,6 +160,8 @@ def map_whole_queries(R, bases, segs):
     print("stage ms", ctx.stage_ms(), "diag", ctx.diag(), "candidates", len(cands2), "loci", len(loci2))
     dg = ctx.diag()
     ctx.close()
+    if fetched is not None:
+        fetched += [cands2, loci2]
     return got, seg_res2, dg
 
 

@@ -164,6 +164,11 @@ STAGE_CASES = [(w, hg, whole, n) for w, hg, whole in (("random", True, False), (
 
 @pytest.mark.parametrize("which,hg,whole,n", STAGE_CASES)
 def test_merged_stages_equal_unsharded(workdir, kernel_paths, which, hg, whole, n):
+    compare_sharded(workdir, which, hg, whole, n)
+
+
+def compare_sharded(workdir, which, hg, whole, n):
+    """the merged stages of n shards against the unsharded context's; returns each shard context's diag counters"""
     make = {"random": lambda: datasets.make_big_random_set(workdir, tag="shbig"),
             "repeat": lambda: datasets.make_repeat_set(workdir, tag="clir"),
             "panel": lambda: datasets.make_panel_set(workdir, tag="clip")}[which]
@@ -193,14 +198,16 @@ def test_merged_stages_equal_unsharded(workdir, kernel_paths, which, hg, whole, 
             after |= (later > 0).astype(np.uint8)
         c.map_resident_with_best(best, after)
     got = merge([c.batch_fetch() for c in ctxs], len(sg))
+    diags = [c.diag() for c in ctxs]
     if whole:
-        assert any(c.diag()["long_fragments"] > 0 for c in ctxs)
+        assert any(dg["long_fragments"] > 0 for dg in diags)
     for c in ctxs:
         c.close()
     w, g = per_segment(*want), per_segment(*got)
     bad = [i for i in range(len(sg)) if w[i] != g[i]]
     assert not bad, (len(bad), w[bad[0]], g[bad[0]]) if bad else None
     assert want[0]["n_candidates"].sum() > 0
+    return diags
 
 
 def test_given_best_needs_its_first_phase():

@@ -212,9 +212,10 @@ def kernel_paths(request, monkeypatch):
     return request.param
 
 
-def run_stage_parity(d, args, seg_length, expect_diag=(), expect_freq_seeds=False, **ctx_kw):
+def run_stage_parity(d, args, seg_length, expect_diag=(), expect_freq_seeds=False, check=None, **ctx_kw):
     """expect_diag: names of mm_ctx_diag counters that must be non-zero afterwards (the rare path really ran);
-    expect_freq_seeds: the reference must have flagged frequent seeds and some query sketch must have lost hashes to them"""
+    expect_freq_seeds: the reference must have flagged frequent seeds and some query sketch must have lost hashes to them;
+    check: called with the device's (segment results, candidates, loci)"""
     from mashmap_b200 import capi
 
     R = open_session(args, d)
@@ -229,7 +230,11 @@ def run_stage_parity(d, args, seg_length, expect_diag=(), expect_freq_seeds=Fals
         ctx.map_resident()
         seg_res2, cands2, loci2 = ctx.batch_fetch()
         dev_sketch, dev_count = ctx.batch_fetch_sketch()
-        assert np.array_equal(seg_res["n_candidates"], seg_res2["n_candidates"])
+        # the first call is the one a fresh context's small buffers make regrow: its candidates and loci, fragment by
+        # fragment, must be the resident call's, which is compared with the reference below
+        first = [device_fragment_digest(i, seg_res, cands, loci, dev_sketch, dev_count) for i in range(len(segs))]
+        assert first == [device_fragment_digest(i, seg_res2, cands2, loci2, dev_sketch, dev_count) for i in range(len(segs))], \
+            "mm_map_segments and the resident path differ"
         print("stage ms", ctx.stage_ms(), "launches", ctx.kernel_launches)
         def diag(i, seg, full_len, counter, o):
             import oracle_py
@@ -248,6 +253,8 @@ def run_stage_parity(d, args, seg_length, expect_diag=(), expect_freq_seeds=Fals
                 O.close()
 
         bad = compare_stages(ctx, R, d, ridx, start, length, seg_res2, cands2, loci2, dev_sketch, dev_count, diag=diag)
+        if check is not None:
+            check(seg_res2, cands2, loci2)
         dg = ctx.diag()
         print("rare paths taken:", dg)
         for name in expect_diag:
