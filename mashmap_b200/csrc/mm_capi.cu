@@ -193,6 +193,16 @@ struct image_guard {
   ~image_guard() { if (!c->blob_ready) drop_index(c); }
 };
 
+/* a device build replaces the context's index: the old image and kept lookup arrays go first, and the returned guard
+ * leaves the context with no index if the build does not complete */
+image_guard start_build(mm_ctx *c)
+{
+  drop_index(c);
+  c->built = mm_built_index{};
+  c->built_kept = false;
+  return image_guard{c};
+}
+
 /* lays out the index image for these counts (mm_internal.h) and allocates it as the context's own */
 int begin_image(mm_ctx *c, uint64_t n_mi, uint64_t n_keys, uint64_t n_points, int32_t n_contigs)
 {
@@ -1174,7 +1184,7 @@ int mm_host_free(void *ptr) { return cudaFreeHost(ptr) == cudaSuccess ? MM_OK : 
 namespace {
 /* the device builder over contigs [0, n_contigs) of contig_offsets (text at seqs, host or device) */
 int run_builder(mm_ctx *c, const char *seqs, int seqs_on_device, const uint64_t *contig_offsets, int32_t n_contigs,
-                float kmer_pct_threshold, const mm_shard_freq *shard, mm_built_index &B)
+                const mm_freq_rule &rule, mm_built_index &B)
 {
   const uint64_t total = contig_offsets[n_contigs];
   mm_devbuf<uint8_t> staged;
@@ -1183,11 +1193,23 @@ int run_builder(mm_ctx *c, const char *seqs, int seqs_on_device, const uint64_t 
     CU(c, cudaMemcpyAsync(staged.get(), seqs, total, cudaMemcpyHostToDevice, c->stream));
   }
   std::string err;
-  int rc = mm_build_index_device(c->params, seqs_on_device ? (const uint8_t *)seqs : staged.get(), contig_offsets, n_contigs,
-                                 kmer_pct_threshold, shard, c->stream, c->sm_count, &B, err);
+  int rc = mm_build_index_device(c->params, seqs_on_device ? (const uint8_t *)seqs : staged.get(), contig_offsets, n_contigs, rule,
+                                 c->stream, c->sm_count, &B, err);
   if (rc != MM_OK) return fail(c, rc, "index build: %s", err.c_str());
   c->launches += 12;
   return MM_OK;
+}
+
+/* the statistics of the build that left B (mm_freq_rule::COUNT_ONLY leaves the filter's fields at their defaults) */
+void fill_stats(mm_index_stats *stats, const mm_built_index &B, std::chrono::steady_clock::time_point t0)
+{
+  if (!stats) return;
+  memset(stats, 0, sizeof *stats);
+  stats->n_minmers = B.n_minmers; stats->n_minmers_before_filter = B.n_minmers_before_filter; stats->n_keys = B.n_keys; stats->n_points = B.n_points;
+  stats->freq_threshold = B.freq_threshold; stats->n_chunks = B.n_chunks; stats->n_fixed_chunks = B.n_fixed_chunks; stats->fix_rounds = B.fix_rounds;
+  stats->hist_min_count = B.hist_min_count; stats->hist_max_count = B.hist_max_count; stats->hist_min_keys = B.hist_min_keys;
+  stats->hist_max_keys = B.hist_max_keys; stats->ms_scan = B.ms_scan; stats->ms_post = B.ms_post; stats->ms_lookup = B.ms_lookup;
+  stats->ms_total = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
 }
 
 /* the image of what run_builder left in B (contig tables of n_contigs entries) */
@@ -1204,7 +1226,7 @@ int image_from_build(mm_ctx *c, mm_built_index &B, int32_t n_contigs, const int3
     mm_devbuf<unsigned long long> d_cnt;
     CU(c, d_cnt.reserve((size_t)n_contigs + 1));
     CU(c, cudaMemsetAsync(d_cnt.get(), 0, ((size_t)n_contigs + 1) * 8, c->stream));
-    CU(c, mm_index_count_seq(n_mi, B.seq.get(), d_cnt.get(), c->stream));
+    CU(c, mm_index_count_seq(n_mi, B.mi.seq.get(), d_cnt.get(), c->stream));
     std::vector<unsigned long long> cnt((size_t)n_contigs + 1);
     CU(c, cudaMemcpyAsync(cnt.data(), d_cnt.get(), ((size_t)n_contigs + 1) * 8, cudaMemcpyDeviceToHost, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
@@ -1213,27 +1235,20 @@ int image_from_build(mm_ctx *c, mm_built_index &B, int32_t n_contigs, const int3
   if ((rc = begin_image(c, n_mi, n_keys, n_points, n_contigs))) return rc;
   const mm_blob_header &h = c->hdr;
   if (n_mi) {
-    CU(c, cudaMemcpyAsync(c->blob + h.off_idx_hash, B.hash.get(), n_mi * 8, cudaMemcpyDeviceToDevice, c->stream));
-    CU(c, cudaMemcpyAsync(c->blob + h.off_idx_wpos, B.wpos.get(), n_mi * 4, cudaMemcpyDeviceToDevice, c->stream));
-    CU(c, cudaMemcpyAsync(c->blob + h.off_idx_wend, B.wend.get(), n_mi * 4, cudaMemcpyDeviceToDevice, c->stream));
-    CU(c, cudaMemcpyAsync(c->blob + h.off_idx_strand, B.strand.get(), n_mi, cudaMemcpyDeviceToDevice, c->stream));
+    CU(c, cudaMemcpyAsync(c->blob + h.off_idx_hash, B.mi.hash.get(), n_mi * 8, cudaMemcpyDeviceToDevice, c->stream));
+    CU(c, cudaMemcpyAsync(c->blob + h.off_idx_wpos, B.mi.wpos.get(), n_mi * 4, cudaMemcpyDeviceToDevice, c->stream));
+    CU(c, cudaMemcpyAsync(c->blob + h.off_idx_wend, B.mi.wend.get(), n_mi * 4, cudaMemcpyDeviceToDevice, c->stream));
+    CU(c, cudaMemcpyAsync(c->blob + h.off_idx_strand, B.mi.strand.get(), n_mi, cudaMemcpyDeviceToDevice, c->stream));
   }
   if (n_points) CU(c, cudaMemcpyAsync(c->blob + h.off_pts, B.pts.get(), n_points * 8, cudaMemcpyDeviceToDevice, c->stream));
   CU(c, cudaStreamSynchronize(c->stream));
-  B.hash.reset(); B.wpos.reset(); B.wend.reset(); B.seq.reset(); B.strand.reset(); /* before the death order's sort */
+  B.mi.reset(); /* before the death order's sort */
   mm_devbuf<uint32_t> d_err;
   CU(c, d_err.reserve(1));
   CU(c, cudaMemsetAsync(d_err.get(), 0, 4, c->stream));
   rc = finish_image(c, cstart, B.keys.get(), B.offs.get(), B.is_freq.get(), d_err.get(), clen, contig_name_id, contig_group);
   if (!c->blob_ready) return rc; /* else rc is write_tables': the index stands either way */
-  if (stats) {
-    memset(stats, 0, sizeof *stats);
-    stats->n_minmers = n_mi; stats->n_minmers_before_filter = B.n_minmers_before_filter; stats->n_keys = n_keys; stats->n_points = n_points;
-    stats->freq_threshold = B.freq_threshold; stats->n_chunks = B.n_chunks; stats->n_fixed_chunks = B.n_fixed_chunks; stats->fix_rounds = B.fix_rounds;
-    stats->hist_min_count = B.hist_min_count; stats->hist_max_count = B.hist_max_count; stats->hist_min_keys = B.hist_min_keys;
-    stats->hist_max_keys = B.hist_max_keys; stats->ms_scan = B.ms_scan; stats->ms_post = B.ms_post; stats->ms_lookup = B.ms_lookup;
-    stats->ms_total = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
-  }
+  fill_stats(stats, B, t0);
   if (keep_lookup) { c->built = std::move(B); c->built_kept = true; }
   return rc;
 }
@@ -1248,12 +1263,9 @@ int mm_index_build(mm_ctx *c, const char *seqs, int seqs_on_device, const uint64
   if (n_contigs < 1 || !contig_offsets || !seqs) return fail(c, MM_EINVAL, "no contigs");
   CU(c, cudaSetDevice(c->device));
   const auto t0 = std::chrono::steady_clock::now();
-  drop_index(c);
-  image_guard guard{c};
-  c->built = mm_built_index{};
-  c->built_kept = false;
+  const image_guard guard = start_build(c);
   mm_built_index B;
-  int rc = run_builder(c, seqs, seqs_on_device, contig_offsets, n_contigs, kmer_pct_threshold, nullptr, B);
+  int rc = run_builder(c, seqs, seqs_on_device, contig_offsets, n_contigs, mm_freq_rule::own_threshold(kmer_pct_threshold), B);
   if (rc) return rc;
   std::vector<int32_t> clen((size_t)n_contigs);
   for (int32_t q = 0; q < n_contigs; q++) clen[(size_t)q] = (int32_t)(contig_offsets[q + 1] - contig_offsets[q]);
@@ -1270,17 +1282,10 @@ int mm_index_key_counts(mm_ctx *c, const char *seqs, int seqs_on_device, const u
     c->kc_keys.reset(); c->kc_counts.reset(); c->kc_n = 0; c->kc_ready = false;
     const auto t0 = std::chrono::steady_clock::now();
     mm_built_index B;
-    const mm_shard_freq count_only{1, nullptr, 0};
-    int rc = run_builder(c, seqs, seqs_on_device, contig_offsets, n_contigs, 0.f, &count_only, B);
+    int rc = run_builder(c, seqs, seqs_on_device, contig_offsets, n_contigs, mm_freq_rule::count_only(), B);
     if (rc) return rc;
     c->kc_keys = std::move(B.keys); c->kc_counts = std::move(B.counts); c->kc_n = B.n_keys; c->kc_ready = true;
-    if (stats) {
-      memset(stats, 0, sizeof *stats);
-      stats->n_minmers_before_filter = B.n_minmers_before_filter; stats->n_keys = B.n_keys; stats->n_points = B.n_points;
-      stats->freq_threshold = 0x7fffffff; stats->n_chunks = B.n_chunks; stats->n_fixed_chunks = B.n_fixed_chunks;
-      stats->fix_rounds = B.fix_rounds; stats->ms_scan = B.ms_scan; stats->ms_post = B.ms_post;
-      stats->ms_total = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
-    }
+    fill_stats(stats, B, t0);
   } else if (!c->kc_ready) {
     return fail(c, MM_ESTATE, "no key counts kept: call with the shard's contigs first");
   }
@@ -1309,10 +1314,7 @@ int mm_index_build_shard(mm_ctx *c, const char *seqs, int seqs_on_device, const 
     if (freq_hashes[j] <= freq_hashes[j - 1]) return fail(c, MM_EINVAL, "the frequent hashes are not strictly ascending");
   CU(c, cudaSetDevice(c->device));
   const auto t0 = std::chrono::steady_clock::now();
-  drop_index(c);
-  image_guard guard{c};
-  c->built = mm_built_index{};
-  c->built_kept = false;
+  const image_guard guard = start_build(c);
   /* every contig of the reference, those outside the shard empty: the builder then writes global seqIds */
   std::vector<uint64_t> off((size_t)n_contigs + 1);
   for (int32_t q = 0; q <= n_contigs; q++)
@@ -1321,8 +1323,7 @@ int mm_index_build_shard(mm_ctx *c, const char *seqs, int seqs_on_device, const 
   CU(c, d_freq.reserve(n_freq + 1));
   if (n_freq) CU(c, cudaMemcpyAsync(d_freq.get(), freq_hashes, n_freq * 8, cudaMemcpyHostToDevice, c->stream));
   mm_built_index B;
-  const mm_shard_freq listed{0, d_freq.get(), n_freq};
-  int rc = run_builder(c, seqs, seqs_on_device, off.data(), n_contigs, 0.f, &listed, B);
+  int rc = run_builder(c, seqs, seqs_on_device, off.data(), n_contigs, mm_freq_rule::listed(d_freq.get(), n_freq), B);
   d_freq.reset();
   if (rc) return rc;
   return image_from_build(c, B, n_contigs, contig_len, contig_name_id, contig_group, keep_lookup, stats, t0);

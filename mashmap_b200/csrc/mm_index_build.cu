@@ -29,6 +29,7 @@
 #include <cmath>
 #include <cstdio>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "mm_index_build.h"
@@ -242,13 +243,14 @@ __global__ void k_patch_starts(const wb_chunk *__restrict__ chunks, const wb_chu
   }
 }
 
-/* ---- post-processing of addMinmers (:522-568) ---------------------------------------------------------------------- */
+/* ---- post-processing of addMinmers (:522-568) ----------------------------------------------------------------------
+ * Record columns come in mm_rec_views. The compiler ignores __restrict__ on struct members but keeps it on locals, so the
+ * columns a kernel only reads are named as restricted locals: their loads stay independent of its stores. */
 
 /* chunk buffers -> one raw array in emission order; per record: kept as it is (1) / number of pieces it is cut into */
 __global__ void k_gather_raw(const wb_chunk *__restrict__ chunks, const wb_chunk_out *__restrict__ outs, uint32_t n_chunks,
                              const uint64_t *__restrict__ raw_off, const wm_record *__restrict__ rec_buf, uint32_t rec_cap,
-                             const wm_record *__restrict__ fix_buf, const uint64_t *__restrict__ fix_off, int w,
-                             uint64_t *r_hash, int32_t *r_wpos, int32_t *r_wend, int32_t *r_seq, int8_t *r_strand,
+                             const wm_record *__restrict__ fix_buf, const uint64_t *__restrict__ fix_off, int w, mm_rec_view raw,
                              uint32_t *keep, uint32_t *pieces)
 {
   const uint32_t c = blockIdx.x;
@@ -260,8 +262,8 @@ __global__ void k_gather_raw(const wb_chunk *__restrict__ chunks, const wb_chunk
   for (uint32_t i = threadIdx.x; i < o.n_rec; i += blockDim.x) {
     const wm_record r = src[i];
     const uint64_t d = at + i;
-    r_hash[d] = r.hash; r_wpos[d] = r.wpos; r_wend[d] = r.wpos_end; r_seq[d] = seqId;
-    r_strand[d] = (int8_t)(r.votes < 0 ? -1 : 1); /* :534 */
+    raw.hash[d] = r.hash; raw.wpos[d] = r.wpos; raw.wend[d] = r.wpos_end; raw.seq[d] = seqId;
+    raw.strand[d] = (int8_t)(r.votes < 0 ? -1 : 1); /* :534 */
     const bool bad = r.wpos < 0 || r.wpos_end < 0 || r.wpos == r.wpos_end; /* :523-528 */
     const int64_t len = (int64_t)r.wpos_end - (int64_t)r.wpos;
     uint32_t k = 0, p = 0;
@@ -274,17 +276,17 @@ __global__ void k_gather_raw(const wb_chunk *__restrict__ chunks, const wb_chunk
   }
 }
 /* kept records first (emission order), then all pieces (parent's emission order, piece index): the vector the reference sorts */
-__global__ void k_scatter_records(uint64_t n_raw, const uint64_t *__restrict__ r_hash, const int32_t *__restrict__ r_wpos,
-                                  const int32_t *__restrict__ r_wend, const int32_t *__restrict__ r_seq, const int8_t *__restrict__ r_strand,
-                                  const uint32_t *__restrict__ keep, const uint32_t *__restrict__ pieces,
+__global__ void k_scatter_records(uint64_t n_raw, mm_rec_view raw, const uint32_t *__restrict__ keep, const uint32_t *__restrict__ pieces,
                                   const uint64_t *__restrict__ keep_off, const uint64_t *__restrict__ piece_off, uint64_t n_keep, int w,
-                                  uint64_t *o_hash, int32_t *o_wpos, int32_t *o_wend, int32_t *o_seq, int8_t *o_strand)
+                                  mm_rec_view o)
 {
+  const uint64_t *__restrict__ r_hash = raw.hash; const int32_t *__restrict__ r_wpos = raw.wpos, *__restrict__ r_wend = raw.wend;
+  const int32_t *__restrict__ r_seq = raw.seq; const int8_t *__restrict__ r_strand = raw.strand;
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_raw) return;
   if (keep[i]) {
     const uint64_t d = keep_off[i];
-    o_hash[d] = r_hash[i]; o_wpos[d] = r_wpos[i]; o_wend[d] = r_wend[i]; o_seq[d] = r_seq[i]; o_strand[d] = r_strand[i];
+    o.hash[d] = r_hash[i]; o.wpos[d] = r_wpos[i]; o.wend[d] = r_wend[i]; o.seq[d] = r_seq[i]; o.strand[d] = r_strand[i];
   }
   const uint32_t p = pieces[i];
   if (p) {
@@ -292,10 +294,10 @@ __global__ void k_scatter_records(uint64_t n_raw, const uint64_t *__restrict__ r
     const int32_t a = r_wpos[i], e = r_wend[i];
     for (uint32_t c = 0; c < p; c++) { /* :538-553 */
       const uint64_t d = d0 + c;
-      o_hash[d] = r_hash[i]; o_seq[d] = r_seq[i]; o_strand[d] = r_strand[i];
-      o_wpos[d] = a + (int32_t)c * w;
+      o.hash[d] = r_hash[i]; o.seq[d] = r_seq[i]; o.strand[d] = r_strand[i];
+      o.wpos[d] = a + (int32_t)c * w;
       const int32_t hi = a + (int32_t)c * w + w;
-      o_wend[d] = hi < e ? hi : e;
+      o.wend[d] = hi < e ? hi : e;
     }
   }
 }
@@ -311,15 +313,14 @@ __global__ void k_keys_seq_wpos(uint64_t n, const uint32_t *__restrict__ perm, c
   if (i < n) { const uint32_t j = perm[i]; keys[i] = ((uint64_t)(uint32_t)seq[j] << 32) | (uint64_t)(uint32_t)wpos[j]; }
 }
 /* gather in sorted order and flag the records std::unique keeps (:563-568: same wpos and hash as the one before, per contig) */
-__global__ void k_gather_sorted(uint64_t n, const uint32_t *__restrict__ perm, const uint64_t *__restrict__ i_hash,
-                                const int32_t *__restrict__ i_wpos, const int32_t *__restrict__ i_wend, const int32_t *__restrict__ i_seq,
-                                const int8_t *__restrict__ i_strand, uint64_t *o_hash, int32_t *o_wpos, int32_t *o_wend, int32_t *o_seq,
-                                int8_t *o_strand, uint32_t *uniq)
+__global__ void k_gather_sorted(uint64_t n, const uint32_t *__restrict__ perm, mm_rec_view in, mm_rec_view o, uint32_t *uniq)
 {
+  const uint64_t *__restrict__ i_hash = in.hash; const int32_t *__restrict__ i_wpos = in.wpos, *__restrict__ i_wend = in.wend;
+  const int32_t *__restrict__ i_seq = in.seq; const int8_t *__restrict__ i_strand = in.strand;
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const uint32_t j = perm[i];
-  o_hash[i] = i_hash[j]; o_wpos[i] = i_wpos[j]; o_wend[i] = i_wend[j]; o_seq[i] = i_seq[j]; o_strand[i] = i_strand[j];
+  o.hash[i] = i_hash[j]; o.wpos[i] = i_wpos[j]; o.wend[i] = i_wend[j]; o.seq[i] = i_seq[j]; o.strand[i] = i_strand[j];
   uint32_t u = 1;
   if (i > 0) {
     const uint32_t p = perm[i - 1];
@@ -327,15 +328,14 @@ __global__ void k_gather_sorted(uint64_t n, const uint32_t *__restrict__ perm, c
   }
   uniq[i] = u;
 }
-__global__ void k_compact5(uint64_t n, const uint32_t *__restrict__ flag, const uint64_t *__restrict__ off, const uint64_t *__restrict__ i_hash,
-                           const int32_t *__restrict__ i_wpos, const int32_t *__restrict__ i_wend, const int32_t *__restrict__ i_seq,
-                           const int8_t *__restrict__ i_strand, uint64_t *o_hash, int32_t *o_wpos, int32_t *o_wend, int32_t *o_seq,
-                           int8_t *o_strand)
+__global__ void k_compact5(uint64_t n, const uint32_t *__restrict__ flag, const uint64_t *__restrict__ off, mm_rec_view in, mm_rec_view o)
 {
+  const uint64_t *__restrict__ i_hash = in.hash; const int32_t *__restrict__ i_wpos = in.wpos, *__restrict__ i_wend = in.wend;
+  const int32_t *__restrict__ i_seq = in.seq; const int8_t *__restrict__ i_strand = in.strand;
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n || !flag[i]) return;
   const uint64_t d = off[i];
-  o_hash[d] = i_hash[i]; o_wpos[d] = i_wpos[i]; o_wend[d] = i_wend[i]; o_seq[d] = i_seq[i]; o_strand[d] = i_strand[i];
+  o.hash[d] = i_hash[i]; o.wpos[d] = i_wpos[i]; o.wend[d] = i_wend[i]; o.seq[d] = i_seq[i]; o.strand[d] = i_strand[i];
 }
 
 /* ---- Sketch::index (:379-404) ------------------------------------------------------------------------------------------
@@ -434,20 +434,6 @@ __global__ void k_keep_not_freq(uint64_t n, const uint32_t *__restrict__ perm, c
   if (i < n) keep[perm[i]] = is_freq[rec_key[i]] ? 0u : 1u;
 }
 
-struct Dev { /* frees what it allocated when it goes out of scope */
-  std::vector<void *> p;
-  ~Dev() { for (void *x : p) cudaFree(x); }
-  template <typename T> cudaError_t alloc(T *&ptr, uint64_t n)
-  {
-    ptr = nullptr;
-    cudaError_t e = cudaMalloc((void **)&ptr, std::max<uint64_t>(n, 1) * sizeof(T));
-    if (e == cudaSuccess) p.push_back(ptr);
-    return e;
-  }
-  void release(void *x) { p.erase(std::remove(p.begin(), p.end(), x), p.end()); }
-  void free_now(void *x) { if (x) { cudaFree(x); release(x); } }
-};
-
 #define CE(call)                                                                                        \
   do {                                                                                                  \
     cudaError_t e_ = (call);                                                                            \
@@ -456,46 +442,486 @@ struct Dev { /* frees what it allocated when it goes out of scope */
 
 inline uint32_t blocks(uint64_t n, uint32_t per = 256) { return (uint32_t)((n + per - 1) / per); }
 
-cudaError_t exclusive_sum_u32_to_u64(const uint32_t *in, uint64_t *out, uint64_t n, cudaStream_t st, Dev &dv)
+#define MM_FOR_EACH_K(X) \
+  X(8) X(9) X(10) X(11) X(12) X(13) X(14) X(15) X(16) X(17) X(18) X(19) X(20) X(21) X(22) X(23) X(24) X(25) X(26) X(27) \
+  X(28) X(29) X(30) X(31) X(32)
+
+/* f(std::integral_constant<int, K>()) for a k-mer size K that is compiled in (mm_sketch_kmer_supported) */
+template <typename F>
+void for_kmer(int K, F &&f)
 {
-  void *tmp = nullptr;
+  switch (K) {
+#define X(KK) case KK: f(std::integral_constant<int, KK>()); break;
+    MM_FOR_EACH_K(X)
+#undef X
+  }
+}
+
+/* cub's two-call convention: call(nullptr, bytes) sizes the temporary storage, which is then held in tmp for the real call */
+template <typename Call>
+cudaError_t cub_run(mm_devbuf<uint8_t> &tmp, Call &&call)
+{
   size_t bytes = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, bytes, cub::TransformInputIterator<uint64_t, cub::CastOp<uint64_t>, const uint32_t *>(in, cub::CastOp<uint64_t>()), out, (int64_t)n, st);
-  cudaError_t e = cudaMalloc(&tmp, bytes + 16);
-  if (e != cudaSuccess) return e;
-  e = cub::DeviceScan::ExclusiveSum(tmp, bytes, cub::TransformInputIterator<uint64_t, cub::CastOp<uint64_t>, const uint32_t *>(in, cub::CastOp<uint64_t>()), out, (int64_t)n, st);
-  cudaStreamSynchronize(st);
-  cudaFree(tmp);
-  (void)dv;
-  return e;
+  cudaError_t e = call(nullptr, bytes);
+  if (e == cudaSuccess) e = tmp.reserve(bytes + 16);
+  return e == cudaSuccess ? call(tmp.get(), bytes) : e;
+}
+
+/* off[i] = flag[0] + ... + flag[i - 1] (n > 0), and total = the sum of all n flags; `st` is synchronised once */
+cudaError_t count_flags(const uint32_t *flag, uint64_t *off, uint64_t n, cudaStream_t st, uint64_t &total)
+{
+  const cub::TransformInputIterator<uint64_t, cub::CastOp<uint64_t>, const uint32_t *> in(flag, cub::CastOp<uint64_t>());
+  mm_devbuf<uint8_t> tmp;
+  cudaError_t e = cub_run(tmp, [&](void *t, size_t &bytes) { return cub::DeviceScan::ExclusiveSum(t, bytes, in, off, (int64_t)n, st); });
+  uint64_t last_off = 0; uint32_t last_flag = 0;
+  if (e == cudaSuccess) e = cudaMemcpyAsync(&last_off, off + n - 1, 8, cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(&last_flag, flag + n - 1, 4, cudaMemcpyDeviceToHost, st);
+  const cudaError_t s = cudaStreamSynchronize(st); /* before the temporary goes and the last values are read */
+  total = last_off + last_flag;
+  return e != cudaSuccess ? e : s;
 }
 template <typename KeyT>
 cudaError_t sort_pairs(KeyT *k_in, KeyT *k_out, uint32_t *v_in, uint32_t *v_out, uint64_t n, int end_bit, cudaStream_t st)
 {
-  void *tmp = nullptr;
-  size_t bytes = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, bytes, k_in, k_out, v_in, v_out, (int64_t)n, 0, end_bit, st);
-  cudaError_t e = cudaMalloc(&tmp, bytes + 16);
-  if (e != cudaSuccess) return e;
-  e = cub::DeviceRadixSort::SortPairs(tmp, bytes, k_in, k_out, v_in, v_out, (int64_t)n, 0, end_bit, st);
-  cudaStreamSynchronize(st);
-  cudaFree(tmp);
-  return e;
+  mm_devbuf<uint8_t> tmp;
+  const cudaError_t e = cub_run(tmp, [&](void *t, size_t &bytes) {
+    return cub::DeviceRadixSort::SortPairs(t, bytes, k_in, k_out, v_in, v_out, (int64_t)n, 0, end_bit, st);
+  });
+  const cudaError_t s = cudaStreamSynchronize(st); /* before the temporary goes */
+  return e != cudaSuccess ? e : s;
 }
 
-template <int K>
-void launch_scan(const uint8_t *seq, const uint64_t *off, const wb_chunk *chunks, uint32_t n_chunks, int w, int s, int warm, unsigned char *slabs,
-                 const wb_slab_layout &L, wm_record *rec, uint32_t rec_cap, wb_chunk_out *outs, wb_open *ex, uint32_t stride, uint32_t grid,
-                 cudaStream_t st)
+struct stage_events { /* the builder's timing events (ms_scan, ms_post and ms_lookup lie between them), destroyed on every return */
+  cudaEvent_t e[4] = {};
+  ~stage_events() { for (cudaEvent_t x : e) if (x) cudaEventDestroy(x); }
+  cudaError_t create()
+  {
+    for (cudaEvent_t &x : e)
+      if (const cudaError_t r = cudaEventCreate(&x)) { x = nullptr; return r; }
+    return cudaSuccess;
+  }
+};
+
+/* ---- chunks ---- */
+struct chunk_plan {
+  std::vector<wb_chunk> chunks; /* contig by contig, in order */
+  int chunk_len;
+};
+int plan_chunks(int K, const uint64_t *h_contig_off, int32_t n_contigs, chunk_plan &plan, std::string &err)
 {
-  k_window_scan<K><<<grid, 128, 0, st>>>(seq, off, chunks, n_chunks, w, s, warm, slabs, L, rec, rec_cap, outs, ex, stride);
+  plan.chunk_len = 16384;
+  if (const char *e = getenv("MM_INDEX_CHUNK")) plan.chunk_len = std::max(1024, atoi(e)); /* tests: small chunks */
+  for (int32_t c = 0; c < n_contigs; c++) {
+    const uint64_t len = h_contig_off[c + 1] - h_contig_off[c];
+    if (len >= (1ULL << 31)) { err = "a contig is longer than 2^31 bases"; return MM_EINVAL; }
+    const int32_t npos = (int32_t)len - K + 1;
+    if (npos <= 0) continue;
+    for (int32_t a = 0; a < npos; a += plan.chunk_len) plan.chunks.push_back(wb_chunk{c, a, std::min(npos, a + plan.chunk_len), npos});
+  }
+  return MM_OK;
 }
-template <int K>
-void launch_fix(const uint8_t *seq, const uint64_t *off, const wb_chunk *chunks, const wb_chain *chains, uint32_t n_chains, int w, int s, int warm,
-                unsigned char *slabs, const wb_slab_layout &L, wm_record *fix, uint32_t fix_cap, wb_chunk_out *outs, wb_open *ex, uint32_t stride,
-                cudaStream_t st)
+
+/* ---- acceptance, fix-up rounds ----
+ * A chunk is good if it starts a contig and ran clean, or if its predecessor is good, it ran clean (no failure, no
+ * expired heap entry taken) and its state digest at its start equals its predecessor's at its end. A chunk that is not
+ * good starts a chain of rejected chunks, or joins the chain right before it; a chain starts right after a good chunk
+ * and is re-scanned by one thread from that chunk's exact end state.
+ * A chunk right after a chain that is not re-scanned yet is decided in a later round, against the chain's exact end
+ * state (it is pending, and so is every chunk after it), unless it failed on its own, which rejects it whatever came
+ * before it: then it joins the chain at once. A chain whose next chunk does not match its new end state is extended by
+ * that chunk and re-scanned as a whole. So each contig has at most one dirty chain per round, and all of the contig
+ * before that chain is good: the chain's start state (chunk first-1 and the resolved exports of first-2) depends on
+ * nothing that is rewritten in the same round. The export resolution stops at the dirty chain too, since the exports of
+ * pending chunks inherit record starts from the chunks the chain is about to rewrite; what it resolved is final, so
+ * the next round resolves from there on. A round decides at least the chunk after each chain it re-scanned, so there
+ * are at most as many rounds as chunks; a contig with r separate runs of rejected chunks takes about r rounds.
+ * chunk_rounds is that bookkeeping, on the host and without CUDA calls: it decides a round from the chunks' outputs as
+ * copied back after the scan or the last re-scan, and names the chains to re-scan and the exports to resolve first. */
+struct chunk_rounds {
+  enum : uint8_t { CH_GOOD, CH_DIRTY, CH_PENDING };
+  struct HostChain { uint32_t first, n; bool dirty; };
+  std::vector<uint32_t> cf, cnn; /* chunks of each contig (for the sequential resolution of inherited record starts) */
+  std::vector<uint8_t> state; std::vector<int32_t> in_chain; std::vector<HostChain> hchains;
+  std::vector<uint32_t> resolve_n; /* per contig: the chunks whose exports the next resolution may touch */
+  std::vector<uint32_t> resolved; /* per contig: its chunks up to this one have resolved exports */
+  std::vector<uint32_t> res_first, res_n; /* the resolution to run: chunks [res_first, res_first + res_n) of each contig */
+  uint64_t decided_before = 0;
+  uint32_t n_rounds = 0;
+  explicit chunk_rounds(const std::vector<wb_chunk> &chunks) : state(chunks.size(), CH_PENDING), in_chain(chunks.size(), -1)
+  {
+    for (uint32_t c = 0; c < (uint32_t)chunks.size(); c++) {
+      if (c == 0 || chunks[c].contig != chunks[c - 1].contig) { cf.push_back(c); cnn.push_back(0); }
+      cnn.back()++;
+    }
+    resolve_n.resize(cf.size()); resolved.assign(cf.size(), 0); res_first.resize(cf.size()); res_n.resize(cf.size());
+  }
+
+  /* decides every chunk it can from outs. chains: the dirty chains, re-scanned in this round (none: every chunk is
+   * decided); resolve_n: the exports to resolve before they are */
+  int next(const std::vector<wb_chunk_out> &outs, std::vector<wb_chain> &chains, std::string &err)
+  {
+    uint64_t decided = 0;
+    for (size_t g = 0; g < cf.size(); g++) {
+      resolve_n[g] = cnn[g];
+      for (uint32_t c = cf[g]; c < cf[g] + cnn[g]; c++) {
+        const bool first = c == cf[g];
+        if (in_chain[c] >= 0) { /* re-scanned in an earlier round: exact (a chain is only dirty from the chunk that made it so on) */
+          if (outs[c].flags & 3u) { err = "window machine capacity exceeded while re-scanning a chunk"; return MM_ECAPACITY; }
+          state[c] = CH_GOOD;
+        } else {
+          const uint8_t prev = first ? CH_GOOD : state[c - 1];
+          const bool own_fail = (outs[c].flags & (first ? 3u : 7u)) != 0;
+          if (prev == CH_GOOD && !own_fail && (first || outs[c].d_start == outs[c - 1].d_end)) {
+            state[c] = CH_GOOD;
+          } else if (prev == CH_PENDING || (prev == CH_DIRTY && !own_fail)) {
+            state[c] = CH_PENDING;
+          } else {
+            if (!first && in_chain[c - 1] >= 0) { /* the chain before it grows by this chunk and is re-scanned as a whole */
+              HostChain &hc = hchains[(size_t)in_chain[c - 1]];
+              hc.n++; hc.dirty = true;
+              in_chain[c] = in_chain[c - 1];
+            } else {
+              in_chain[c] = (int32_t)hchains.size();
+              hchains.push_back(HostChain{c, 1, true});
+            }
+            state[c] = CH_DIRTY;
+            resolve_n[g] = std::min(resolve_n[g], hchains[(size_t)in_chain[c]].first - cf[g]);
+          }
+        }
+        if (state[c] != CH_PENDING) decided++;
+      }
+    }
+    chains.clear();
+    for (HostChain &hc : hchains)
+      if (hc.dirty) { chains.push_back(wb_chain{hc.first, hc.n, 0}); hc.dirty = false; }
+    if (chains.empty()) return MM_OK;
+    if (n_rounds > 0 && decided <= decided_before) { err = "chunk stitching made no progress"; return MM_ECUDA; }
+    decided_before = decided;
+    n_rounds++;
+    return MM_OK;
+  }
+
+  /* the next resolution: chunks (resolved, limit) of each contig */
+  void resolve_upto(const std::vector<uint32_t> &limit)
+  {
+    for (size_t g = 0; g < cf.size(); g++) {
+      res_first[g] = cf[g] + resolved[g];
+      res_n[g] = limit[g] > resolved[g] ? limit[g] - resolved[g] : 0;
+      if (limit[g] > resolved[g]) resolved[g] = limit[g] - 1;
+    }
+  }
+
+  bool converged() const { return std::all_of(state.begin(), state.end(), [](uint8_t x) { return x == CH_GOOD; }); }
+  uint32_t n_fixed() const { uint32_t n = 0; for (const HostChain &hc : hchains) n += hc.n; return n; }
+};
+
+/* the records of every chunk in emission order, and per record: kept as it is (keep) / number of pieces it is cut into */
+struct raw_records { mm_rec_cols cols; mm_devbuf<uint32_t> keep, pieces; uint64_t n = 0; };
+
+/* the window scan of every chunk, the re-scan rounds and the record starts; sets out->fix_rounds and out->n_fixed_chunks */
+int scan_windows(const mm_params &p, const uint8_t *d_seq, const uint64_t *h_contig_off, int32_t n_contigs, const chunk_plan &plan,
+                 cudaStream_t st, int sm_count, raw_records &raw, mm_built_index *out, std::string &err)
 {
-  k_window_fix<K><<<(n_chains + 63) / 64, 64, 0, st>>>(seq, off, chunks, chains, n_chains, w, s, warm, slabs, L, fix, fix_cap, outs, ex, stride);
+  const std::vector<wb_chunk> &chunks = plan.chunks;
+  const uint32_t n_chunks = (uint32_t)chunks.size();
+  if (!n_chunks) return MM_OK;
+  const int K = p.kmer_size, w = p.seg_length, s = p.sketch_size, warm = w + 2 * K + 64;
+  mm_devbuf<uint64_t> d_off; mm_devbuf<wb_chunk> d_chunks;
+  CE(d_off.reserve((uint64_t)n_contigs + 1));
+  CE(cudaMemcpyAsync(d_off.get(), h_contig_off, ((size_t)n_contigs + 1) * 8, cudaMemcpyHostToDevice, st));
+  CE(d_chunks.reserve(n_chunks));
+  CE(cudaMemcpyAsync(d_chunks.get(), chunks.data(), (size_t)n_chunks * sizeof(wb_chunk), cudaMemcpyHostToDevice, st));
+  const wb_slab_layout L = slab_layout(w, s);
+  int tpsm = 768; /* machines per SM: the scan is latency-bound (dependent accesses to a per-thread slab), more threads hide more */
+  if (const char *e = getenv("MM_INDEX_TPSM")) tpsm = std::max(128, atoi(e) / 128 * 128);
+  uint32_t threads = (uint32_t)sm_count * (uint32_t)tpsm;
+  if (threads > n_chunks) threads = (n_chunks + 127) / 128 * 128;
+  const uint32_t rec_cap = (uint32_t)(plan.chunk_len / 4 + s + 64);
+  { /* one slab per machine (~0.4 MB at -s 5000): at 3 Gbp the slabs of a full grid and the chunks' record buffers
+     * together exceed an 80 GB device next to the caller's data, so the grid shrinks to the memory that is free
+     * (a smaller grid only scans more chunks per thread) */
+    size_t free_b = 0, total_b = 0;
+    CE(cudaMemGetInfo(&free_b, &total_b));
+    const uint64_t fixed = (uint64_t)n_chunks * rec_cap * sizeof(wm_record) + (uint64_t)n_chunks * wm_mem_cap(s) * sizeof(wb_open) + (1ULL << 30);
+    const uint64_t room = free_b > fixed ? (free_b - fixed) / 10 * 8 : 0;
+    const uint64_t fit = room / L.bytes / 128 * 128;
+    if (fit < threads) threads = (uint32_t)std::max<uint64_t>(fit, 128);
+  }
+  if (const char *e = getenv("MM_INDEX_MACHINES")) { /* tests: a small grid, so that each machine scans many chunks */
+    const uint32_t cap = (uint32_t)std::max<long>(128, (strtol(e, nullptr, 10) + 127) / 128 * 128);
+    threads = std::min(threads, cap);
+  }
+  const uint32_t grid = threads / 128;
+  const uint32_t stride = (uint32_t)wm_mem_cap(s);
+  mm_devbuf<unsigned char> slabs; mm_devbuf<wm_record> rec; mm_devbuf<wb_chunk_out> d_outs; mm_devbuf<wb_open> d_ex;
+  CE(slabs.reserve((uint64_t)threads * L.bytes)); CE(rec.reserve((uint64_t)n_chunks * rec_cap));
+  CE(d_outs.reserve(n_chunks)); CE(d_ex.reserve((uint64_t)n_chunks * stride));
+  for_kmer(K, [&](auto k) {
+    k_window_scan<decltype(k)::value><<<grid, 128, 0, st>>>(d_seq, d_off.get(), d_chunks.get(), n_chunks, w, s, warm, slabs.get(), L, rec.get(),
+                                                            rec_cap, d_outs.get(), d_ex.get(), stride);
+  });
+  CE(cudaGetLastError());
+  std::vector<wb_chunk_out> outs(n_chunks);
+  CE(cudaMemcpyAsync(outs.data(), d_outs.get(), (size_t)n_chunks * sizeof(wb_chunk_out), cudaMemcpyDeviceToHost, st));
+  CE(cudaStreamSynchronize(st));
+
+  chunk_rounds rounds(chunks);
+  const uint32_t n_used = (uint32_t)rounds.cf.size();
+  mm_devbuf<uint32_t> d_cf, d_cn, d_err;
+  CE(d_cf.reserve(n_used)); CE(d_cn.reserve(n_used)); CE(d_err.reserve(1));
+  CE(cudaMemsetAsync(d_err.get(), 0, 4, st));
+  auto resolve = [&](const std::vector<uint32_t> &limit) { /* resolve chunks (resolved, limit) of each contig */
+    rounds.resolve_upto(limit);
+    cudaError_t e = cudaMemcpyAsync(d_cf.get(), rounds.res_first.data(), (size_t)n_used * 4, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_cn.get(), rounds.res_n.data(), (size_t)n_used * 4, cudaMemcpyHostToDevice, st);
+    if (e != cudaSuccess) return e;
+    k_resolve_exports<<<n_used, 128, 0, st>>>(d_cf.get(), d_cn.get(), n_used, d_outs.get(), d_ex.get(), stride, d_err.get());
+    return cudaGetLastError();
+  };
+  mm_devbuf<wm_record> fix;
+  std::vector<uint64_t> fix_off(n_chunks, 0);
+  uint64_t fix_used = 0;
+  const uint32_t fix_cap = (uint32_t)(3 * plan.chunk_len + s + 64); /* at most three records per position */
+  for (;;) {
+    std::vector<wb_chain> chains;
+    const int rc = rounds.next(outs, chains, err);
+    if (rc != MM_OK) return rc;
+    if (chains.empty()) break;
+    out->fix_rounds = rounds.n_rounds;
+    uint64_t need = 0;
+    for (auto &cn : chains) { cn.out_offset = fix_used + need; need += (uint64_t)cn.n * fix_cap; }
+    if ((fix_used + need) * sizeof(wm_record) > (48ULL << 30)) { err = "too many chunks need an exact re-scan (N-rich / low-complexity reference): use the host builder"; return MM_ECAPACITY; }
+    if (fix_used + need > fix.capacity()) /* grow, keeping what earlier rounds wrote */
+      CE(fix.reserve_keep((fix_used + need) + (fix_used + need) / 2, fix_used, st));
+    for (auto &cn : chains)
+      for (uint32_t q = 0; q < cn.n; q++) fix_off[cn.first + q] = cn.out_offset + (uint64_t)q * fix_cap;
+    fix_used += need;
+    CE(resolve(rounds.resolve_n)); /* the re-scan takes record starts from the exports of the chunks before the chain */
+    const uint32_t n_chains = (uint32_t)chains.size();
+    mm_devbuf<wb_chain> d_chains;
+    CE(d_chains.reserve(n_chains));
+    CE(cudaMemcpyAsync(d_chains.get(), chains.data(), n_chains * sizeof(wb_chain), cudaMemcpyHostToDevice, st));
+    mm_devbuf<unsigned char> chain_slabs; /* more chains than machines */
+    if (n_chains > threads) CE(chain_slabs.reserve((uint64_t)n_chains * L.bytes));
+    unsigned char *fslabs = chain_slabs ? chain_slabs.get() : slabs.get();
+    for_kmer(K, [&](auto k) {
+      k_window_fix<decltype(k)::value><<<(n_chains + 63) / 64, 64, 0, st>>>(d_seq, d_off.get(), d_chunks.get(), d_chains.get(), n_chains, w, s,
+                                                                            warm, fslabs, L, fix.get(), fix_cap, d_outs.get(), d_ex.get(), stride);
+    });
+    CE(cudaGetLastError());
+    CE(cudaMemcpyAsync(outs.data(), d_outs.get(), (size_t)n_chunks * sizeof(wb_chunk_out), cudaMemcpyDeviceToHost, st));
+    CE(cudaStreamSynchronize(st));
+  }
+  out->n_fixed_chunks = rounds.n_fixed();
+  if (!rounds.converged()) { err = "chunk stitching did not converge"; return MM_ECUDA; }
+  slabs.reset();
+
+  CE(resolve(rounds.cnn));
+  k_patch_starts<<<n_chunks, 128, 0, st>>>(d_chunks.get(), d_outs.get(), n_chunks, rec.get(), rec_cap, d_ex.get(), stride, d_err.get());
+  CE(cudaGetLastError());
+  uint32_t h_err = 0;
+  CE(cudaMemcpyAsync(&h_err, d_err.get(), 4, cudaMemcpyDeviceToHost, st));
+  CE(cudaStreamSynchronize(st));
+  if (h_err) { err = "a record open at a chunk start is missing from the previous chunk's export (code " + std::to_string(h_err) + ")"; return MM_ECUDA; }
+  d_ex.reset();
+
+  /* ---- raw records in emission order ---- */
+  std::vector<uint64_t> raw_off(n_chunks + 1, 0);
+  for (uint32_t c = 0; c < n_chunks; c++) raw_off[c + 1] = raw_off[c] + outs[c].n_rec;
+  raw.n = raw_off[n_chunks];
+  mm_devbuf<uint64_t> d_raw_off, d_fix_off;
+  CE(d_raw_off.reserve((uint64_t)n_chunks + 1)); CE(d_fix_off.reserve(n_chunks));
+  CE(cudaMemcpyAsync(d_raw_off.get(), raw_off.data(), ((size_t)n_chunks + 1) * 8, cudaMemcpyHostToDevice, st));
+  CE(cudaMemcpyAsync(d_fix_off.get(), fix_off.data(), (size_t)n_chunks * 8, cudaMemcpyHostToDevice, st));
+  CE(raw.cols.reserve(raw.n)); CE(raw.keep.reserve(raw.n)); CE(raw.pieces.reserve(raw.n));
+  k_gather_raw<<<n_chunks, 256, 0, st>>>(d_chunks.get(), d_outs.get(), n_chunks, d_raw_off.get(), rec.get(), rec_cap, fix.get(), d_fix_off.get(),
+                                         w, raw.cols.view(), raw.keep.get(), raw.pieces.get());
+  CE(cudaGetLastError());
+  CE(cudaStreamSynchronize(st));
+  return MM_OK;
+}
+
+/* kept records + pieces -> the vector the reference sorts, ordered by (seqId, wpos, wpos_end) and de-duplicated: m[n_mi].
+ * raw is freed once it is expanded */
+int expand_and_sort(raw_records &raw, int32_t n_contigs, int w, cudaStream_t st, mm_rec_cols &m, uint64_t &n_mi, std::string &err)
+{
+  n_mi = 0;
+  if (!raw.n) return MM_OK;
+  const uint64_t n_raw = raw.n;
+  mm_rec_cols a; /* kept records, then pieces */
+  uint64_t n_all = 0;
+  {
+    mm_devbuf<uint64_t> keep_off, piece_off;
+    CE(keep_off.reserve(n_raw + 1)); CE(piece_off.reserve(n_raw + 1));
+    uint64_t n_keep = 0, n_pieces = 0;
+    CE(count_flags(raw.keep.get(), keep_off.get(), n_raw, st, n_keep));
+    CE(count_flags(raw.pieces.get(), piece_off.get(), n_raw, st, n_pieces));
+    n_all = n_keep + n_pieces;
+    if (n_all >= (1ULL << 32)) { err = "more than 2^32 minmer records"; return MM_EINVAL; }
+    CE(a.reserve(n_all));
+    k_scatter_records<<<blocks(n_raw), 256, 0, st>>>(n_raw, raw.cols.view(), raw.keep.get(), raw.pieces.get(), keep_off.get(), piece_off.get(),
+                                                     n_keep, w, a.view());
+    CE(cudaGetLastError());
+    CE(cudaStreamSynchronize(st));
+  }
+  raw.cols.reset(); raw.keep.reset(); raw.pieces.reset();
+  if (!n_all) return MM_OK;
+
+  /* ---- order by (seqId, wpos, wpos_end), stable; adjacent de-duplication ---- */
+  mm_devbuf<uint32_t> va, vb;
+  {
+    mm_devbuf<uint32_t> k32a, k32b;
+    CE(k32a.reserve(n_all)); CE(k32b.reserve(n_all)); CE(va.reserve(n_all)); CE(vb.reserve(n_all));
+    k_iota_keys32<<<blocks(n_all), 256, 0, st>>>(n_all, a.wend.get(), k32a.get(), va.get());
+    CE(sort_pairs<uint32_t>(k32a.get(), k32b.get(), va.get(), vb.get(), n_all, 32, st));   /* by wpos_end */
+  }
+  {
+    mm_devbuf<uint64_t> k64a, k64b;
+    CE(k64a.reserve(n_all)); CE(k64b.reserve(n_all));
+    k_keys_seq_wpos<<<blocks(n_all), 256, 0, st>>>(n_all, vb.get(), a.seq.get(), a.wpos.get(), k64a.get());
+    int end_bit = 32;
+    while ((1LL << (end_bit - 32)) < (long long)n_contigs + 1) end_bit++;
+    CE(sort_pairs<uint64_t>(k64a.get(), k64b.get(), vb.get(), va.get(), n_all, end_bit, st)); /* then by (seqId, wpos): LSD, stable */
+  }
+  vb.reset();
+  mm_rec_cols s; mm_devbuf<uint32_t> uniq;
+  CE(s.reserve(n_all)); CE(uniq.reserve(n_all));
+  k_gather_sorted<<<blocks(n_all), 256, 0, st>>>(n_all, va.get(), a.view(), s.view(), uniq.get());
+  CE(cudaGetLastError());
+  CE(cudaStreamSynchronize(st));
+  va.reset(); a.reset();
+  mm_devbuf<uint64_t> uoff;
+  CE(uoff.reserve(n_all + 1));
+  CE(count_flags(uniq.get(), uoff.get(), n_all, st, n_mi));
+  CE(m.reserve(n_mi));
+  k_compact5<<<blocks(n_all), 256, 0, st>>>(n_all, uniq.get(), uoff.get(), s.view(), m.view());
+  CE(cudaGetLastError());
+  CE(cudaStreamSynchronize(st));
+  return MM_OK;
+}
+
+/* Sketch::index over m[n_mi] (n_mi > 0): out's keys, offsets, points and every key's count; for the frequency filter, the
+ * index position of each record in hash order (perm) and its key (rec_key) */
+int index_lookup(const mm_rec_cols &m, uint64_t n_mi, cudaStream_t st, mm_devbuf<uint32_t> &perm, mm_devbuf<uint64_t> &rec_key,
+                 mm_built_index *out, std::string &err)
+{
+  mm_devbuf<uint64_t> hs;
+  {
+    mm_devbuf<uint64_t> hk; mm_devbuf<uint32_t> va;
+    CE(hk.reserve(n_mi)); CE(hs.reserve(n_mi)); CE(va.reserve(n_mi)); CE(perm.reserve(n_mi));
+    k_iota_keys64<<<blocks(n_mi), 256, 0, st>>>(n_mi, m.hash.get(), hk.get(), va.get());
+    CE(sort_pairs<uint64_t>(hk.get(), hs.get(), va.get(), perm.get(), n_mi, 64, st));
+  }
+  {
+    mm_devbuf<uint32_t> key_start, run_start; mm_devbuf<uint64_t> key_idx, run_idx;
+    CE(key_start.reserve(n_mi)); CE(run_start.reserve(n_mi)); CE(key_idx.reserve(n_mi + 1)); CE(run_idx.reserve(n_mi + 1));
+    CE(rec_key.reserve(n_mi));
+    k_lookup_flags<<<blocks(n_mi), 256, 0, st>>>(n_mi, hs.get(), perm.get(), m.wpos.get(), m.wend.get(), key_start.get(), run_start.get());
+    uint64_t n_runs = 0;
+    CE(count_flags(key_start.get(), key_idx.get(), n_mi, st, out->n_keys));
+    CE(count_flags(run_start.get(), run_idx.get(), n_mi, st, n_runs));
+    out->n_points = 2 * n_runs;
+    /* exclusive scans give, at a start flag, the index of the new key / run; at other records index + 1 of the current one */
+    CE(out->keys.reserve(out->n_keys)); CE(out->offs.reserve(out->n_keys + 1)); CE(out->pts.reserve(out->n_points + 1));
+    CE(out->is_freq.reserve(out->n_keys));
+    k_lookup_emit<<<blocks(n_mi), 256, 0, st>>>(n_mi, hs.get(), perm.get(), m.wpos.get(), m.wend.get(), m.seq.get(), key_start.get(),
+                                                run_start.get(), key_idx.get(), run_idx.get(), out->keys.get(), out->offs.get(), out->pts.get(),
+                                                rec_key.get());
+    CE(cudaGetLastError());
+    CE(cudaMemcpyAsync(out->offs.get() + out->n_keys, &out->n_points, 8, cudaMemcpyHostToDevice, st));
+    CE(cudaStreamSynchronize(st));
+  }
+  hs.reset();
+  /* histogram of interval points per key (winSketch.hpp:415-417) */
+  CE(out->counts.reserve(out->n_keys));
+  k_key_counts<<<blocks(out->n_keys), 256, 0, st>>>(out->n_keys, out->offs.get(), out->n_points, out->counts.get());
+  return MM_OK;
+}
+
+/* the frequent keys by `rule` (computeFreqHist, or the listed hashes) flagged in out->is_freq, then dropFreqSeedSet: the
+ * records of m[n_mi] with the other hashes, in out->mi. perm and rec_key are freed once used */
+int frequency_filter(const mm_freq_rule &rule, const mm_rec_cols &m, uint64_t n_mi, mm_devbuf<uint32_t> &perm, mm_devbuf<uint64_t> &rec_key,
+                     cudaStream_t st, mm_built_index *out, std::string &err)
+{
+  const uint64_t n_keys = out->n_keys;
+  uint32_t *cnt = out->counts.get();
+  if (rule.mode == mm_freq_rule::OWN_THRESHOLD) { /* the frequency threshold over this index alone */
+    uint32_t max_cnt = 0;
+    {
+      mm_devbuf<uint32_t> d_max; mm_devbuf<uint8_t> tmp;
+      CE(d_max.reserve(1));
+      const auto max_of = [&](void *t, size_t &bytes) { return cub::DeviceReduce::Max(t, bytes, cnt, d_max.get(), (int64_t)n_keys, st); };
+      CE(cub_run(tmp, max_of));
+      CE(cudaMemcpyAsync(&max_cnt, d_max.get(), 4, cudaMemcpyDeviceToHost, st));
+      CE(cudaStreamSynchronize(st));
+    }
+    const uint32_t hist_n = max_cnt + 2;
+    std::vector<unsigned long long> hist(hist_n);
+    {
+      mm_devbuf<unsigned long long> d_hist;
+      CE(d_hist.reserve(hist_n));
+      CE(cudaMemsetAsync(d_hist.get(), 0, (size_t)hist_n * 8, st));
+      k_histogram<<<blocks(n_keys), 256, 0, st>>>(n_keys, cnt, d_hist.get(), hist_n);
+      CE(cudaMemcpyAsync(hist.data(), d_hist.get(), (size_t)hist_n * 8, cudaMemcpyDeviceToHost, st));
+      CE(cudaStreamSynchronize(st));
+    }
+    int32_t threshold = 0x7fffffff;
+    { /* computeFreqHist :431-441, the same arithmetic (int64 * float / 100 -> int64; walk from the most frequent) */
+      const int64_t totalUniqueMinmers = (int64_t)n_keys;
+      const int64_t minmerToIgnore = totalUniqueMinmers * rule.pct / 100;
+      int64_t sum = 0;
+      for (int64_t f = (int64_t)hist_n - 1; f >= 0; f--) {
+        if (!hist[(size_t)f]) continue;
+        sum += (int64_t)hist[(size_t)f];
+        if (sum < minmerToIgnore) threshold = (int32_t)f;
+        else if (sum == minmerToIgnore) { threshold = (int32_t)f; break; }
+        else break;
+      }
+      out->hist_min_count = 0; out->hist_max_count = max_cnt;
+      for (uint32_t f = 0; f < hist_n; f++) if (hist[f]) { out->hist_min_count = f; out->hist_min_keys = hist[f]; break; }
+      out->hist_max_keys = hist[max_cnt];
+    }
+    out->freq_threshold = threshold;
+    k_mark_freq<<<blocks(n_keys), 256, 0, st>>>(n_keys, cnt, (uint32_t)threshold, out->is_freq.get());
+  } else {
+    k_mark_listed<<<blocks(n_keys), 256, 0, st>>>(n_keys, out->keys.get(), rule.d_freq, rule.n_freq, out->is_freq.get());
+  }
+  CE(cudaStreamSynchronize(st));
+  out->counts.reset();
+  /* dropFreqSeedSet: the frequent hashes leave minmerIndex (not the lookup) */
+  mm_devbuf<uint32_t> keep; mm_devbuf<uint64_t> koff;
+  CE(keep.reserve(n_mi)); CE(koff.reserve(n_mi + 1));
+  k_keep_not_freq<<<blocks(n_mi), 256, 0, st>>>(n_mi, perm.get(), rec_key.get(), out->is_freq.get(), keep.get());
+  CE(count_flags(keep.get(), koff.get(), n_mi, st, out->n_minmers));
+  perm.reset(); rec_key.reset();
+  CE(out->mi.reserve(out->n_minmers));
+  k_compact5<<<blocks(n_mi), 256, 0, st>>>(n_mi, keep.get(), koff.get(), m.view(), out->mi.view());
+  CE(cudaGetLastError());
+  CE(cudaStreamSynchronize(st));
+  return MM_OK;
+}
+
+/* the listed frequent hashes (rule.n_freq > 0) that the shard's keys lack: appended after them as frequent keys with no
+ * points, so that every shard drops them */
+int append_absent(const mm_freq_rule &rule, cudaStream_t st, mm_built_index *out, std::string &err)
+{
+  const uint64_t nf = rule.n_freq, n_keys = out->n_keys;
+  mm_devbuf<uint32_t> absent; mm_devbuf<uint64_t> at;
+  CE(absent.reserve(nf)); CE(at.reserve(nf + 1));
+  k_flag_absent<<<blocks(nf), 256, 0, st>>>(nf, rule.d_freq, out->keys.get(), n_keys, absent.get());
+  uint64_t n_abs = 0;
+  CE(count_flags(absent.get(), at.get(), nf, st, n_abs));
+  if (!n_abs) return MM_OK;
+  CE(out->keys.reserve_keep(n_keys + n_abs, n_keys, st)); CE(out->offs.reserve_keep(n_keys + n_abs + 1, n_keys, st));
+  CE(out->is_freq.reserve_keep(n_keys + n_abs, n_keys, st));
+  if (!out->pts) CE(out->pts.reserve(1));
+  k_append_absent<<<blocks(nf), 256, 0, st>>>(nf, rule.d_freq, absent.get(), at.get(), n_keys, out->n_points, out->keys.get(), out->offs.get(),
+                                              out->is_freq.get());
+  CE(cudaGetLastError());
+  out->n_keys = n_keys + n_abs;
+  CE(cudaMemcpyAsync(out->offs.get() + out->n_keys, &out->n_points, 8, cudaMemcpyHostToDevice, st));
+  CE(cudaStreamSynchronize(st));
+  return MM_OK;
 }
 
 /* ---- the index image (mm_capi.cu writes it from these) ---- */
@@ -590,439 +1016,44 @@ __global__ void k_unpack_points(uint64_t n, const uint64_t *__restrict__ pts, co
 
 } // namespace
 
-#define MM_FOR_EACH_K(X) \
-  X(8) X(9) X(10) X(11) X(12) X(13) X(14) X(15) X(16) X(17) X(18) X(19) X(20) X(21) X(22) X(23) X(24) X(25) X(26) X(27) \
-  X(28) X(29) X(30) X(31) X(32)
-
 int mm_build_index_device(const mm_params &p, const uint8_t *d_seq, const uint64_t *h_contig_off, int32_t n_contigs,
-                          float kmer_pct_threshold, const mm_shard_freq *shard, cudaStream_t st, int sm_count,
-                          mm_built_index *out, std::string &err)
+                          const mm_freq_rule &rule, cudaStream_t st, int sm_count, mm_built_index *out, std::string &err)
 {
   *out = mm_built_index{};
-  const int K = p.kmer_size, w = p.seg_length, s = p.sketch_size;
-  if (!mm_sketch_kmer_supported(K)) { err = "k-mer size not compiled in"; return MM_EINVAL; }
-  Dev dv;
-  cudaEvent_t ev[4];
-  for (auto &e : ev) cudaEventCreate(&e);
-  cudaEventRecord(ev[0], st);
-
-  /* ---- chunks ---- */
-  const int warm = w + 2 * K + 64;
-  int chunk_len = 16384;
-  if (const char *e = getenv("MM_INDEX_CHUNK")) chunk_len = std::max(1024, atoi(e)); /* tests: small chunks */
-  std::vector<wb_chunk> chunks;
-  for (int32_t c = 0; c < n_contigs; c++) {
-    const uint64_t len = h_contig_off[c + 1] - h_contig_off[c];
-    if (len >= (1ULL << 31)) { err = "a contig is longer than 2^31 bases"; return MM_EINVAL; }
-    const int32_t npos = (int32_t)len - K + 1;
-    if (npos <= 0) continue;
-    for (int32_t a = 0; a < npos; a += chunk_len) chunks.push_back(wb_chunk{c, a, std::min(npos, a + chunk_len), npos});
-  }
-  const uint32_t n_chunks = (uint32_t)chunks.size();
-  out->n_chunks = n_chunks;
-  uint64_t *d_off = nullptr;
-  CE(dv.alloc(d_off, (uint64_t)n_contigs + 1));
-  CE(cudaMemcpyAsync(d_off, h_contig_off, ((size_t)n_contigs + 1) * 8, cudaMemcpyHostToDevice, st));
-
-  uint64_t n_raw = 0;
-  uint64_t *r_hash = nullptr; int32_t *r_wpos = nullptr, *r_wend = nullptr, *r_seq = nullptr; int8_t *r_strand = nullptr;
-  uint32_t *r_keep = nullptr, *r_pieces = nullptr;
-  if (n_chunks) {
-    wb_chunk *d_chunks = nullptr;
-    CE(dv.alloc(d_chunks, n_chunks));
-    CE(cudaMemcpyAsync(d_chunks, chunks.data(), (size_t)n_chunks * sizeof(wb_chunk), cudaMemcpyHostToDevice, st));
-    const wb_slab_layout L = slab_layout(w, s);
-    int tpsm = 768; /* machines per SM: the scan is latency-bound (dependent accesses to a per-thread slab), more threads hide more */
-    if (const char *e = getenv("MM_INDEX_TPSM")) tpsm = std::max(128, atoi(e) / 128 * 128);
-    uint32_t threads = (uint32_t)sm_count * (uint32_t)tpsm;
-    if (threads > n_chunks) threads = (n_chunks + 127) / 128 * 128;
-    const uint32_t rec_cap = (uint32_t)(chunk_len / 4 + s + 64);
-    { /* one slab per machine (~0.4 MB at -s 5000): at 3 Gbp the slabs of a full grid and the chunks' record buffers
-       * together exceed an 80 GB device next to the caller's data, so the grid shrinks to the memory that is free
-       * (a smaller grid only scans more chunks per thread) */
-      size_t free_b = 0, total_b = 0;
-      CE(cudaMemGetInfo(&free_b, &total_b));
-      const uint64_t fixed = (uint64_t)n_chunks * rec_cap * sizeof(wm_record) + (uint64_t)n_chunks * wm_mem_cap(s) * sizeof(wb_open) + (1ULL << 30);
-      const uint64_t room = free_b > fixed ? (free_b - fixed) / 10 * 8 : 0;
-      const uint64_t fit = room / L.bytes / 128 * 128;
-      if (fit < threads) threads = (uint32_t)std::max<uint64_t>(fit, 128);
-    }
-    if (const char *e = getenv("MM_INDEX_MACHINES")) { /* tests: a small grid, so that each machine scans many chunks */
-      const uint32_t cap = (uint32_t)std::max<long>(128, (strtol(e, nullptr, 10) + 127) / 128 * 128);
-      threads = std::min(threads, cap);
-    }
-    const uint32_t grid = threads / 128;
-    unsigned char *slabs = nullptr;
-    CE(dv.alloc(slabs, (uint64_t)threads * L.bytes));
-    wm_record *rec = nullptr;
-    CE(dv.alloc(rec, (uint64_t)n_chunks * rec_cap));
-    wb_chunk_out *d_outs = nullptr;
-    CE(dv.alloc(d_outs, n_chunks));
-    const uint32_t stride = (uint32_t)wm_mem_cap(s);
-    wb_open *d_ex = nullptr;
-    CE(dv.alloc(d_ex, (uint64_t)n_chunks * stride));
-    switch (K) {
-#define X(KK) case KK: launch_scan<KK>(d_seq, d_off, d_chunks, n_chunks, w, s, warm, slabs, L, rec, rec_cap, d_outs, d_ex, stride, grid, st); break;
-      MM_FOR_EACH_K(X)
-#undef X
-    }
-    CE(cudaGetLastError());
-    std::vector<wb_chunk_out> outs(n_chunks);
-    CE(cudaMemcpyAsync(outs.data(), d_outs, (size_t)n_chunks * sizeof(wb_chunk_out), cudaMemcpyDeviceToHost, st));
-    CE(cudaStreamSynchronize(st));
-
-    /* chunks of each contig (for the sequential resolution of inherited record starts) */
-    std::vector<uint32_t> cf, cnn;
-    for (uint32_t c = 0; c < n_chunks; c++) {
-      if (c == 0 || chunks[c].contig != chunks[c - 1].contig) { cf.push_back(c); cnn.push_back(0); }
-      cnn.back()++;
-    }
-    uint32_t *d_cf = nullptr, *d_cn = nullptr, *d_err = nullptr;
-    CE(dv.alloc(d_cf, cf.size())); CE(dv.alloc(d_cn, cf.size())); CE(dv.alloc(d_err, 1));
-    CE(cudaMemcpyAsync(d_cf, cf.data(), cf.size() * 4, cudaMemcpyHostToDevice, st));
-    CE(cudaMemcpyAsync(d_cn, cnn.data(), cf.size() * 4, cudaMemcpyHostToDevice, st));
-    CE(cudaMemsetAsync(d_err, 0, 4, st));
-    auto resolve = [&]() {
-      k_resolve_exports<<<(uint32_t)cf.size(), 128, 0, st>>>(d_cf, d_cn, (uint32_t)cf.size(), d_outs, d_ex, stride, d_err);
-      return cudaGetLastError();
-    };
-
-    /* ---- acceptance, fix-up rounds ----
-     * A chunk is good if it starts a contig and ran clean, or if its predecessor is good, it ran clean (no failure, no
-     * expired heap entry taken) and its state digest at its start equals its predecessor's at its end. A chunk that is not
-     * good starts a chain of rejected chunks, or joins the chain right before it; a chain starts right after a good chunk
-     * and is re-scanned by one thread from that chunk's exact end state.
-     * A chunk right after a chain that is not re-scanned yet is decided in a later round, against the chain's exact end
-     * state (it is pending, and so is every chunk after it), unless it failed on its own, which rejects it whatever came
-     * before it: then it joins the chain at once. A chain whose next chunk does not match its new end state is extended by
-     * that chunk and re-scanned as a whole. So each contig has at most one dirty chain per round, and all of the contig
-     * before that chain is good: the chain's start state (chunk first-1 and the resolved exports of first-2) depends on
-     * nothing that is rewritten in the same round. The export resolution stops at the dirty chain too, since the exports of
-     * pending chunks inherit record starts from the chunks the chain is about to rewrite; what it resolved is final, so
-     * the next round resolves from there on. A round decides at least the chunk after each chain it re-scanned, so there
-     * are at most as many rounds as chunks; a contig with r separate runs of rejected chunks takes about r rounds. */
-    enum : uint8_t { CH_GOOD, CH_DIRTY, CH_PENDING };
-    std::vector<uint8_t> state(n_chunks, CH_PENDING);
-    std::vector<int32_t> in_chain(n_chunks, -1);
-    struct HostChain { uint32_t first, n; bool dirty; };
-    std::vector<HostChain> hchains;
-    std::vector<uint32_t> resolve_n(cf.size()); /* per contig: the chunks whose exports the next resolution may touch */
-    std::vector<uint32_t> resolved(cf.size(), 0); /* per contig: its chunks up to this one have resolved exports */
-    std::vector<uint32_t> res_first(cf.size()), res_n(cf.size());
-    auto resolve_upto = [&](const std::vector<uint32_t> &limit) { /* resolve chunks (resolved, limit) of each contig */
-      for (size_t g = 0; g < cf.size(); g++) {
-        res_first[g] = cf[g] + resolved[g];
-        res_n[g] = limit[g] > resolved[g] ? limit[g] - resolved[g] : 0;
-        if (limit[g] > resolved[g]) resolved[g] = limit[g] - 1;
-      }
-      cudaError_t e = cudaMemcpyAsync(d_cf, res_first.data(), cf.size() * 4, cudaMemcpyHostToDevice, st);
-      if (e == cudaSuccess) e = cudaMemcpyAsync(d_cn, res_n.data(), cf.size() * 4, cudaMemcpyHostToDevice, st);
-      return e == cudaSuccess ? resolve() : e;
-    };
-    wm_record *fix = nullptr;
-    std::vector<uint64_t> fix_off(n_chunks, 0);
-    uint64_t fix_used = 0, fix_capacity = 0, decided_before = 0;
-    const uint32_t fix_cap = (uint32_t)(3 * chunk_len + s + 64); /* at most three records per position */
-    for (uint32_t round = 0;; round++) {
-      uint64_t decided = 0;
-      for (size_t g = 0; g < cf.size(); g++) {
-        resolve_n[g] = cnn[g];
-        for (uint32_t c = cf[g]; c < cf[g] + cnn[g]; c++) {
-          const bool first = c == cf[g];
-          if (in_chain[c] >= 0) { /* re-scanned in an earlier round: exact (a chain is only dirty from the chunk that made it so on) */
-            if (outs[c].flags & 3u) { err = "window machine capacity exceeded while re-scanning a chunk"; return MM_ECAPACITY; }
-            state[c] = CH_GOOD;
-          } else {
-            const uint8_t prev = first ? CH_GOOD : state[c - 1];
-            const bool own_fail = (outs[c].flags & (first ? 3u : 7u)) != 0;
-            if (prev == CH_GOOD && !own_fail && (first || outs[c].d_start == outs[c - 1].d_end)) {
-              state[c] = CH_GOOD;
-            } else if (prev == CH_PENDING || (prev == CH_DIRTY && !own_fail)) {
-              state[c] = CH_PENDING;
-            } else {
-              if (!first && in_chain[c - 1] >= 0) { /* the chain before it grows by this chunk and is re-scanned as a whole */
-                HostChain &hc = hchains[(size_t)in_chain[c - 1]];
-                hc.n++; hc.dirty = true;
-                in_chain[c] = in_chain[c - 1];
-              } else {
-                in_chain[c] = (int32_t)hchains.size();
-                hchains.push_back(HostChain{c, 1, true});
-              }
-              state[c] = CH_DIRTY;
-              resolve_n[g] = std::min(resolve_n[g], hchains[(size_t)in_chain[c]].first - cf[g]);
-            }
-          }
-          if (state[c] != CH_PENDING) decided++;
-        }
-      }
-      std::vector<wb_chain> chains;
-      for (auto &hc : hchains)
-        if (hc.dirty) chains.push_back(wb_chain{hc.first, hc.n, 0});
-      if (chains.empty()) break;
-      if (round > 0 && decided <= decided_before) { err = "chunk stitching made no progress"; return MM_ECUDA; }
-      decided_before = decided;
-      out->fix_rounds = round + 1;
-      uint64_t need = 0;
-      for (auto &cn : chains) { cn.out_offset = fix_used + need; need += (uint64_t)cn.n * fix_cap; }
-      if ((fix_used + need) * sizeof(wm_record) > (48ULL << 30)) { err = "too many chunks need an exact re-scan (N-rich / low-complexity reference): use the host builder"; return MM_ECAPACITY; }
-      if (fix_used + need > fix_capacity) { /* grow, keeping what earlier rounds wrote */
-        wm_record *bigger = nullptr;
-        const uint64_t cap2 = (fix_used + need) + (fix_used + need) / 2;
-        CE(dv.alloc(bigger, cap2));
-        if (fix_used) CE(cudaMemcpyAsync(bigger, fix, fix_used * sizeof(wm_record), cudaMemcpyDeviceToDevice, st));
+  if (!mm_sketch_kmer_supported(p.kmer_size)) { err = "k-mer size not compiled in"; return MM_EINVAL; }
+  stage_events ev;
+  CE(ev.create());
+  cudaEventRecord(ev.e[0], st);
+  int rc;
+  chunk_plan plan;
+  if ((rc = plan_chunks(p.kmer_size, h_contig_off, n_contigs, plan, err)) != MM_OK) return rc;
+  out->n_chunks = (uint32_t)plan.chunks.size();
+  {
+    raw_records raw;
+    if ((rc = scan_windows(p, d_seq, h_contig_off, n_contigs, plan, st, sm_count, raw, out, err)) != MM_OK) return rc;
+    cudaEventRecord(ev.e[1], st);
+    mm_rec_cols m; /* minmerIndex before the frequent-seed drop */
+    uint64_t n_mi = 0;
+    if ((rc = expand_and_sort(raw, n_contigs, p.seg_length, st, m, n_mi, err)) != MM_OK) return rc;
+    out->n_minmers_before_filter = n_mi;
+    cudaEventRecord(ev.e[2], st);
+    if (n_mi) {
+      mm_devbuf<uint32_t> perm; mm_devbuf<uint64_t> rec_key;
+      if ((rc = index_lookup(m, n_mi, st, perm, rec_key, out, err)) != MM_OK) return rc;
+      if (rule.mode == mm_freq_rule::COUNT_ONLY) {
         CE(cudaStreamSynchronize(st));
-        dv.free_now(fix);
-        fix = bigger; fix_capacity = cap2;
+        out->offs.reset(); out->pts.reset(); out->is_freq.reset();
+        return MM_OK;
       }
-      for (auto &cn : chains)
-        for (uint32_t q = 0; q < cn.n; q++) fix_off[cn.first + q] = cn.out_offset + (uint64_t)q * fix_cap;
-      fix_used += need;
-      CE(resolve_upto(resolve_n)); /* the re-scan takes record starts from the exports of the chunks before the chain */
-      wb_chain *d_chains = nullptr;
-      CE(dv.alloc(d_chains, chains.size()));
-      CE(cudaMemcpyAsync(d_chains, chains.data(), chains.size() * sizeof(wb_chain), cudaMemcpyHostToDevice, st));
-      unsigned char *fslabs = slabs;
-      if (chains.size() > threads) { CE(dv.alloc(fslabs, (uint64_t)chains.size() * L.bytes)); }
-      switch (K) {
-#define X(KK) case KK: launch_fix<KK>(d_seq, d_off, d_chunks, d_chains, (uint32_t)chains.size(), w, s, warm, fslabs, L, fix, fix_cap, d_outs, d_ex, stride, st); break;
-        MM_FOR_EACH_K(X)
-#undef X
-      }
-      CE(cudaGetLastError());
-      CE(cudaMemcpyAsync(outs.data(), d_outs, (size_t)n_chunks * sizeof(wb_chunk_out), cudaMemcpyDeviceToHost, st));
-      CE(cudaStreamSynchronize(st));
-      if (fslabs != slabs) dv.free_now(fslabs);
-      dv.free_now(d_chains);
-      for (auto &hc : hchains) hc.dirty = false;
-    }
-    out->n_fixed_chunks = 0;
-    for (auto &hc : hchains) out->n_fixed_chunks += hc.n;
-    for (uint32_t c = 0; c < n_chunks; c++)
-      if (state[c] != CH_GOOD) { err = "chunk stitching did not converge"; return MM_ECUDA; }
-    dv.free_now(slabs);
-
-    CE(resolve_upto(cnn));
-    k_patch_starts<<<n_chunks, 128, 0, st>>>(d_chunks, d_outs, n_chunks, rec, rec_cap, d_ex, stride, d_err);
-    CE(cudaGetLastError());
-    uint32_t h_err = 0;
-    CE(cudaMemcpyAsync(&h_err, d_err, 4, cudaMemcpyDeviceToHost, st));
-    CE(cudaStreamSynchronize(st));
-    if (h_err) { err = "a record open at a chunk start is missing from the previous chunk's export (code " + std::to_string(h_err) + ")"; return MM_ECUDA; }
-    dv.free_now(d_ex);
-
-    /* ---- raw records in emission order ---- */
-    std::vector<uint64_t> raw_off(n_chunks + 1, 0);
-    for (uint32_t c = 0; c < n_chunks; c++) raw_off[c + 1] = raw_off[c] + outs[c].n_rec;
-    n_raw = raw_off[n_chunks];
-    uint64_t *d_raw_off = nullptr, *d_fix_off = nullptr;
-    CE(dv.alloc(d_raw_off, (uint64_t)n_chunks + 1));
-    CE(dv.alloc(d_fix_off, n_chunks));
-    CE(cudaMemcpyAsync(d_raw_off, raw_off.data(), ((size_t)n_chunks + 1) * 8, cudaMemcpyHostToDevice, st));
-    CE(cudaMemcpyAsync(d_fix_off, fix_off.data(), (size_t)n_chunks * 8, cudaMemcpyHostToDevice, st));
-    CE(dv.alloc(r_hash, n_raw)); CE(dv.alloc(r_wpos, n_raw)); CE(dv.alloc(r_wend, n_raw)); CE(dv.alloc(r_seq, n_raw)); CE(dv.alloc(r_strand, n_raw));
-    CE(dv.alloc(r_keep, n_raw)); CE(dv.alloc(r_pieces, n_raw));
-    k_gather_raw<<<n_chunks, 256, 0, st>>>(d_chunks, d_outs, n_chunks, d_raw_off, rec, rec_cap, fix, d_fix_off, w, r_hash, r_wpos, r_wend, r_seq,
-                                           r_strand, r_keep, r_pieces);
-    CE(cudaGetLastError());
-    CE(cudaStreamSynchronize(st));
-    dv.free_now(rec); dv.free_now(fix); dv.free_now(d_outs); dv.free_now(d_chunks); dv.free_now(d_raw_off); dv.free_now(d_fix_off);
-  }
-  cudaEventRecord(ev[1], st);
-
-  /* ---- kept records + pieces -> the vector the reference sorts ---- */
-  uint64_t n_all = 0;
-  uint64_t *a_hash = nullptr; int32_t *a_wpos = nullptr, *a_wend = nullptr, *a_seq = nullptr; int8_t *a_strand = nullptr;
-  if (n_raw) {
-    uint64_t *keep_off = nullptr, *piece_off = nullptr;
-    CE(dv.alloc(keep_off, n_raw + 1)); CE(dv.alloc(piece_off, n_raw + 1));
-    CE(exclusive_sum_u32_to_u64(r_keep, keep_off, n_raw, st, dv));
-    CE(exclusive_sum_u32_to_u64(r_pieces, piece_off, n_raw, st, dv));
-    uint64_t last_k = 0, last_p = 0;
-    uint32_t lk = 0, lp = 0;
-    CE(cudaMemcpy(&last_k, keep_off + n_raw - 1, 8, cudaMemcpyDeviceToHost)); CE(cudaMemcpy(&lk, r_keep + n_raw - 1, 4, cudaMemcpyDeviceToHost));
-    CE(cudaMemcpy(&last_p, piece_off + n_raw - 1, 8, cudaMemcpyDeviceToHost)); CE(cudaMemcpy(&lp, r_pieces + n_raw - 1, 4, cudaMemcpyDeviceToHost));
-    const uint64_t n_keep = last_k + lk, n_pieces = last_p + lp;
-    n_all = n_keep + n_pieces;
-    if (n_all >= (1ULL << 32)) { err = "more than 2^32 minmer records"; return MM_EINVAL; }
-    CE(dv.alloc(a_hash, n_all)); CE(dv.alloc(a_wpos, n_all)); CE(dv.alloc(a_wend, n_all)); CE(dv.alloc(a_seq, n_all)); CE(dv.alloc(a_strand, n_all));
-    k_scatter_records<<<blocks(n_raw), 256, 0, st>>>(n_raw, r_hash, r_wpos, r_wend, r_seq, r_strand, r_keep, r_pieces, keep_off, piece_off, n_keep, w,
-                                                     a_hash, a_wpos, a_wend, a_seq, a_strand);
-    CE(cudaGetLastError());
-    CE(cudaStreamSynchronize(st));
-    dv.free_now(keep_off); dv.free_now(piece_off);
-    dv.free_now(r_hash); dv.free_now(r_wpos); dv.free_now(r_wend); dv.free_now(r_seq); dv.free_now(r_strand); dv.free_now(r_keep); dv.free_now(r_pieces);
-  }
-
-  /* ---- order by (seqId, wpos, wpos_end), stable; adjacent de-duplication ---- */
-  uint64_t n_mi = 0;
-  uint64_t *m_hash = nullptr; int32_t *m_wpos = nullptr, *m_wend = nullptr, *m_seq = nullptr; int8_t *m_strand = nullptr;
-  if (n_all) {
-    uint32_t *k32a = nullptr, *k32b = nullptr, *va = nullptr, *vb = nullptr;
-    CE(dv.alloc(k32a, n_all)); CE(dv.alloc(k32b, n_all)); CE(dv.alloc(va, n_all)); CE(dv.alloc(vb, n_all));
-    k_iota_keys32<<<blocks(n_all), 256, 0, st>>>(n_all, a_wend, k32a, va);
-    CE(sort_pairs<uint32_t>(k32a, k32b, va, vb, n_all, 32, st));   /* by wpos_end */
-    dv.free_now(k32a); dv.free_now(k32b);
-    uint64_t *k64a = nullptr, *k64b = nullptr;
-    CE(dv.alloc(k64a, n_all)); CE(dv.alloc(k64b, n_all));
-    k_keys_seq_wpos<<<blocks(n_all), 256, 0, st>>>(n_all, vb, a_seq, a_wpos, k64a);
-    int end_bit = 32;
-    while ((1LL << (end_bit - 32)) < (long long)n_contigs + 1) end_bit++;
-    CE(sort_pairs<uint64_t>(k64a, k64b, vb, va, n_all, end_bit, st)); /* then by (seqId, wpos): LSD, stable */
-    dv.free_now(k64a); dv.free_now(k64b); dv.free_now(vb);
-    uint64_t *s_hash = nullptr; int32_t *s_wpos = nullptr, *s_wend = nullptr, *s_seq = nullptr; int8_t *s_strand = nullptr; uint32_t *uniq = nullptr;
-    CE(dv.alloc(s_hash, n_all)); CE(dv.alloc(s_wpos, n_all)); CE(dv.alloc(s_wend, n_all)); CE(dv.alloc(s_seq, n_all)); CE(dv.alloc(s_strand, n_all));
-    CE(dv.alloc(uniq, n_all));
-    k_gather_sorted<<<blocks(n_all), 256, 0, st>>>(n_all, va, a_hash, a_wpos, a_wend, a_seq, a_strand, s_hash, s_wpos, s_wend, s_seq, s_strand, uniq);
-    CE(cudaGetLastError());
-    CE(cudaStreamSynchronize(st));
-    dv.free_now(va);
-    dv.free_now(a_hash); dv.free_now(a_wpos); dv.free_now(a_wend); dv.free_now(a_seq); dv.free_now(a_strand);
-    uint64_t *uoff = nullptr;
-    CE(dv.alloc(uoff, n_all + 1));
-    CE(exclusive_sum_u32_to_u64(uniq, uoff, n_all, st, dv));
-    uint64_t lo = 0; uint32_t lu = 0;
-    CE(cudaMemcpy(&lo, uoff + n_all - 1, 8, cudaMemcpyDeviceToHost)); CE(cudaMemcpy(&lu, uniq + n_all - 1, 4, cudaMemcpyDeviceToHost));
-    n_mi = lo + lu;
-    CE(dv.alloc(m_hash, n_mi)); CE(dv.alloc(m_wpos, n_mi)); CE(dv.alloc(m_wend, n_mi)); CE(dv.alloc(m_seq, n_mi)); CE(dv.alloc(m_strand, n_mi));
-    k_compact5<<<blocks(n_all), 256, 0, st>>>(n_all, uniq, uoff, s_hash, s_wpos, s_wend, s_seq, s_strand, m_hash, m_wpos, m_wend, m_seq, m_strand);
-    CE(cudaGetLastError());
-    CE(cudaStreamSynchronize(st));
-    dv.free_now(uoff); dv.free_now(uniq);
-    dv.free_now(s_hash); dv.free_now(s_wpos); dv.free_now(s_wend); dv.free_now(s_seq); dv.free_now(s_strand);
-  }
-  out->n_minmers_before_filter = n_mi;
-  cudaEventRecord(ev[2], st);
-
-  /* ---- Sketch::index + frequency filter ---- */
-  uint64_t n_keys = 0, n_points = 0;
-  uint64_t *keys = nullptr, *offs = nullptr, *pts = nullptr; uint8_t *is_freq = nullptr;
-  int32_t threshold = 0x7fffffff;
-  uint64_t n_final = 0;
-  if (n_mi) {
-    uint64_t *hk = nullptr, *hs = nullptr; uint32_t *va = nullptr, *perm = nullptr;
-    CE(dv.alloc(hk, n_mi)); CE(dv.alloc(hs, n_mi)); CE(dv.alloc(va, n_mi)); CE(dv.alloc(perm, n_mi));
-    k_iota_keys64<<<blocks(n_mi), 256, 0, st>>>(n_mi, m_hash, hk, va);
-    CE(sort_pairs<uint64_t>(hk, hs, va, perm, n_mi, 64, st));
-    dv.free_now(hk); dv.free_now(va);
-    uint32_t *key_start = nullptr, *run_start = nullptr; uint64_t *key_idx = nullptr, *run_idx = nullptr, *rec_key = nullptr;
-    CE(dv.alloc(key_start, n_mi)); CE(dv.alloc(run_start, n_mi)); CE(dv.alloc(key_idx, n_mi + 1)); CE(dv.alloc(run_idx, n_mi + 1)); CE(dv.alloc(rec_key, n_mi));
-    k_lookup_flags<<<blocks(n_mi), 256, 0, st>>>(n_mi, hs, perm, m_wpos, m_wend, key_start, run_start);
-    CE(exclusive_sum_u32_to_u64(key_start, key_idx, n_mi, st, dv));
-    CE(exclusive_sum_u32_to_u64(run_start, run_idx, n_mi, st, dv));
-    uint64_t lk = 0, lr = 0; uint32_t fk = 0, fr = 0;
-    CE(cudaMemcpy(&lk, key_idx + n_mi - 1, 8, cudaMemcpyDeviceToHost)); CE(cudaMemcpy(&fk, key_start + n_mi - 1, 4, cudaMemcpyDeviceToHost));
-    CE(cudaMemcpy(&lr, run_idx + n_mi - 1, 8, cudaMemcpyDeviceToHost)); CE(cudaMemcpy(&fr, run_start + n_mi - 1, 4, cudaMemcpyDeviceToHost));
-    n_keys = lk + fk;
-    n_points = 2 * (lr + fr);
-    /* exclusive scans give, at a start flag, the index of the new key / run; at other records index + 1 of the current one */
-    CE(out->keys.reserve(n_keys)); CE(out->offs.reserve(n_keys + 1)); CE(out->pts.reserve(n_points + 1)); CE(out->is_freq.reserve(n_keys));
-    keys = out->keys.get(); offs = out->offs.get(); pts = out->pts.get(); is_freq = out->is_freq.get();
-    k_lookup_emit<<<blocks(n_mi), 256, 0, st>>>(n_mi, hs, perm, m_wpos, m_wend, m_seq, key_start, run_start, key_idx, run_idx, keys, offs, pts, rec_key);
-    CE(cudaGetLastError());
-    CE(cudaMemcpyAsync(offs + n_keys, &n_points, 8, cudaMemcpyHostToDevice, st));
-    CE(cudaStreamSynchronize(st));
-    dv.free_now(key_start); dv.free_now(run_start); dv.free_now(key_idx); dv.free_now(run_idx); dv.free_now(hs);
-    /* histogram of interval points per key (winSketch.hpp:415-417) */
-    CE(out->counts.reserve(n_keys));
-    uint32_t *cnt = out->counts.get();
-    k_key_counts<<<blocks(n_keys), 256, 0, st>>>(n_keys, offs, n_points, cnt);
-    if (shard && shard->count_only) {
-      CE(cudaStreamSynchronize(st));
-      out->offs.reset(); out->pts.reset(); out->is_freq.reset();
-      for (auto &e : ev) cudaEventDestroy(e);
-      out->n_keys = n_keys; out->n_points = n_points; out->n_minmers_before_filter = n_mi;
-      return MM_OK;
-    }
-    if (!shard) { /* the frequency threshold over this index alone */
-      uint32_t max_cnt = 0;
-      {
-        uint32_t *d_max = nullptr;
-        CE(dv.alloc(d_max, 1));
-        void *tmp = nullptr; size_t bytes = 0;
-        cub::DeviceReduce::Max(nullptr, bytes, cnt, d_max, (int64_t)n_keys, st);
-        CE(cudaMalloc(&tmp, bytes + 16));
-        cub::DeviceReduce::Max(tmp, bytes, cnt, d_max, (int64_t)n_keys, st);
-        CE(cudaMemcpyAsync(&max_cnt, d_max, 4, cudaMemcpyDeviceToHost, st));
-        CE(cudaStreamSynchronize(st));
-        cudaFree(tmp);
-        dv.free_now(d_max);
-      }
-      const uint32_t hist_n = max_cnt + 2;
-      unsigned long long *d_hist = nullptr;
-      CE(dv.alloc(d_hist, hist_n));
-      CE(cudaMemsetAsync(d_hist, 0, (size_t)hist_n * 8, st));
-      k_histogram<<<blocks(n_keys), 256, 0, st>>>(n_keys, cnt, d_hist, hist_n);
-      std::vector<unsigned long long> hist(hist_n);
-      CE(cudaMemcpyAsync(hist.data(), d_hist, (size_t)hist_n * 8, cudaMemcpyDeviceToHost, st));
-      CE(cudaStreamSynchronize(st));
-      dv.free_now(d_hist);
-      { /* computeFreqHist :431-441, the same arithmetic (int64 * float / 100 -> int64; walk from the most frequent) */
-        const int64_t totalUniqueMinmers = (int64_t)n_keys;
-        const int64_t minmerToIgnore = totalUniqueMinmers * kmer_pct_threshold / 100;
-        int64_t sum = 0;
-        for (int64_t f = (int64_t)hist_n - 1; f >= 0; f--) {
-          if (!hist[(size_t)f]) continue;
-          sum += (int64_t)hist[(size_t)f];
-          if (sum < minmerToIgnore) threshold = (int32_t)f;
-          else if (sum == minmerToIgnore) { threshold = (int32_t)f; break; }
-          else break;
-        }
-        out->hist_min_count = 0; out->hist_max_count = max_cnt;
-        for (uint32_t f = 0; f < hist_n; f++) if (hist[f]) { out->hist_min_count = f; out->hist_min_keys = hist[f]; break; }
-        out->hist_max_keys = hist[max_cnt];
-      }
-    }
-    if (shard) k_mark_listed<<<blocks(n_keys), 256, 0, st>>>(n_keys, keys, shard->d_freq, shard->n_freq, is_freq);
-    else k_mark_freq<<<blocks(n_keys), 256, 0, st>>>(n_keys, cnt, (uint32_t)threshold, is_freq);
-    CE(cudaStreamSynchronize(st));
-    out->counts.reset();
-    /* dropFreqSeedSet: the frequent hashes leave minmerIndex (not the lookup) */
-    uint32_t *keep = nullptr; uint64_t *koff = nullptr;
-    CE(dv.alloc(keep, n_mi)); CE(dv.alloc(koff, n_mi + 1));
-    k_keep_not_freq<<<blocks(n_mi), 256, 0, st>>>(n_mi, perm, rec_key, is_freq, keep);
-    CE(exclusive_sum_u32_to_u64(keep, koff, n_mi, st, dv));
-    uint64_t lo = 0; uint32_t lu = 0;
-    CE(cudaMemcpy(&lo, koff + n_mi - 1, 8, cudaMemcpyDeviceToHost)); CE(cudaMemcpy(&lu, keep + n_mi - 1, 4, cudaMemcpyDeviceToHost));
-    n_final = lo + lu;
-    dv.free_now(perm); dv.free_now(rec_key);
-    CE(out->hash.reserve(n_final)); CE(out->wpos.reserve(n_final)); CE(out->wend.reserve(n_final)); CE(out->seq.reserve(n_final));
-    CE(out->strand.reserve(n_final));
-    k_compact5<<<blocks(n_mi), 256, 0, st>>>(n_mi, keep, koff, m_hash, m_wpos, m_wend, m_seq, m_strand, out->hash.get(), out->wpos.get(),
-                                             out->wend.get(), out->seq.get(), out->strand.get());
-    CE(cudaGetLastError());
-    CE(cudaStreamSynchronize(st));
-    dv.free_now(keep); dv.free_now(koff);
-    dv.free_now(m_hash); dv.free_now(m_wpos); dv.free_now(m_wend); dv.free_now(m_seq); dv.free_now(m_strand);
-  }
-  if (shard && shard->n_freq) { /* global frequent hashes this shard does not contain */
-    const uint64_t nf = shard->n_freq;
-    uint32_t *absent = nullptr; uint64_t *at = nullptr;
-    CE(dv.alloc(absent, nf)); CE(dv.alloc(at, nf + 1));
-    k_flag_absent<<<blocks(nf), 256, 0, st>>>(nf, shard->d_freq, keys, n_keys, absent);
-    CE(exclusive_sum_u32_to_u64(absent, at, nf, st, dv));
-    uint64_t lo = 0; uint32_t lu = 0;
-    CE(cudaMemcpy(&lo, at + nf - 1, 8, cudaMemcpyDeviceToHost)); CE(cudaMemcpy(&lu, absent + nf - 1, 4, cudaMemcpyDeviceToHost));
-    const uint64_t n_abs = lo + lu;
-    if (n_abs) {
-      CE(out->keys.reserve_keep(n_keys + n_abs, n_keys, st)); CE(out->offs.reserve_keep(n_keys + n_abs + 1, n_keys, st));
-      CE(out->is_freq.reserve_keep(n_keys + n_abs, n_keys, st));
-      if (!out->pts) CE(out->pts.reserve(1));
-      keys = out->keys.get(); offs = out->offs.get(); is_freq = out->is_freq.get();
-      k_append_absent<<<blocks(nf), 256, 0, st>>>(nf, shard->d_freq, absent, at, n_keys, n_points, keys, offs, is_freq);
-      CE(cudaGetLastError());
-      n_keys += n_abs;
-      CE(cudaMemcpyAsync(offs + n_keys, &n_points, 8, cudaMemcpyHostToDevice, st));
-      CE(cudaStreamSynchronize(st));
+      if ((rc = frequency_filter(rule, m, n_mi, perm, rec_key, st, out, err)) != MM_OK) return rc;
     }
   }
-  cudaEventRecord(ev[3], st);
+  if (rule.mode == mm_freq_rule::LISTED && rule.n_freq && (rc = append_absent(rule, st, out, err)) != MM_OK) return rc;
+  cudaEventRecord(ev.e[3], st);
   CE(cudaStreamSynchronize(st));
-  cudaEventElapsedTime(&out->ms_scan, ev[0], ev[1]);
-  cudaEventElapsedTime(&out->ms_post, ev[1], ev[2]);
-  cudaEventElapsedTime(&out->ms_lookup, ev[2], ev[3]);
-  for (auto &e : ev) cudaEventDestroy(e);
-
-  out->n_minmers = n_final; out->n_keys = n_keys; out->n_points = n_points; out->freq_threshold = threshold;
+  cudaEventElapsedTime(&out->ms_scan, ev.e[0], ev.e[1]);
+  cudaEventElapsedTime(&out->ms_post, ev.e[1], ev.e[2]);
+  cudaEventElapsedTime(&out->ms_lookup, ev.e[2], ev.e[3]);
   return MM_OK;
 }
 
@@ -1059,8 +1090,7 @@ cudaError_t mm_build_death_order(const uint64_t *idx_hash, const int32_t *idx_we
   if (n >= (1ULL << 32)) return cudaErrorInvalidValue;
   mm_devbuf<uint64_t> keys, keys2;
   mm_devbuf<uint32_t> vals, vals2;
-  mm_devbuf<unsigned char> tmp;
-  size_t tmp_bytes = 0;
+  mm_devbuf<uint8_t> tmp;
   cudaError_t e;
   if ((e = keys.reserve(n)) != cudaSuccess || (e = keys2.reserve(n)) != cudaSuccess || (e = vals.reserve(n)) != cudaSuccess ||
       (e = vals2.reserve(n)) != cudaSuccess)
@@ -1069,9 +1099,9 @@ cudaError_t mm_build_death_order(const uint64_t *idx_hash, const int32_t *idx_we
   k_fill_death_keys<<<grid, 256, 0, st>>>(idx_wend, contig_start, n_contigs, n, keys.get(), vals.get());
   int end_bit = 32;
   while ((1LL << (end_bit - 32)) < (long long)n_contigs + 1) end_bit++;
-  cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys.get(), keys2.get(), vals.get(), vals2.get(), (int64_t)n, 0, end_bit, st);
-  if ((e = tmp.reserve(tmp_bytes)) != cudaSuccess) return e;
-  e = cub::DeviceRadixSort::SortPairs(tmp.get(), tmp_bytes, keys.get(), keys2.get(), vals.get(), vals2.get(), (int64_t)n, 0, end_bit, st);
+  e = cub_run(tmp, [&](void *t, size_t &bytes) {
+    return cub::DeviceRadixSort::SortPairs(t, bytes, keys.get(), keys2.get(), vals.get(), vals2.get(), (int64_t)n, 0, end_bit, st);
+  });
   if (e == cudaSuccess) k_gather_death<<<grid, 256, 0, st>>>(idx_hash, keys2.get(), vals2.get(), n, idx2_hash, idx2_wend);
   const cudaError_t s = cudaStreamSynchronize(st); /* before the temporaries go */
   return e != cudaSuccess ? e : s != cudaSuccess ? s : cudaGetLastError();

@@ -9,14 +9,37 @@
 #include "mm_devbuf.h"
 #include "mm_internal.h"
 
+/* the five columns of a set of minmer records, as kernels take them (by value) */
+struct mm_rec_view {
+  uint64_t *hash;
+  int32_t *wpos, *wend, *seq;
+  int8_t *strand;
+};
+struct mm_rec_cols {
+  mm_devbuf<uint64_t> hash;
+  mm_devbuf<int32_t> wpos, wend, seq;
+  mm_devbuf<int8_t> strand;
+
+  cudaError_t reserve(uint64_t n)
+  {
+    cudaError_t e;
+    if ((e = hash.reserve(n)) != cudaSuccess || (e = wpos.reserve(n)) != cudaSuccess || (e = wend.reserve(n)) != cudaSuccess ||
+        (e = seq.reserve(n)) != cudaSuccess || (e = strand.reserve(n)) != cudaSuccess)
+      return e;
+    return cudaSuccess;
+  }
+  void reset() { hash.reset(); wpos.reset(); wend.reset(); seq.reset(); strand.reset(); }
+  mm_rec_view view() const { return mm_rec_view{hash.get(), wpos.get(), wend.get(), seq.get(), strand.get()}; }
+};
+
 /* device arrays the builder leaves behind (owned by the struct) */
 struct mm_built_index {
   uint64_t n_minmers = 0, n_keys = 0, n_points = 0;
   /* minmerIndex after the frequent-seed drop, in reference order (seqId, wpos, wpos_end, emission order) */
-  mm_devbuf<uint64_t> hash; mm_devbuf<int32_t> wpos, wend, seq; mm_devbuf<int8_t> strand;
+  mm_rec_cols mi;
   /* minmerPosLookupIndex, keys ascending: keys[n_keys], offs[n_keys + 1], pts[n_points] (packed, mm_pack_point), is_freq[n_keys] */
   mm_devbuf<uint64_t> keys, offs, pts; mm_devbuf<uint8_t> is_freq;
-  mm_devbuf<uint32_t> counts; /* mm_shard_freq::count_only: the interval points of every key */
+  mm_devbuf<uint32_t> counts; /* mm_freq_rule::COUNT_ONLY: the interval points of every key */
   int32_t freq_threshold = 0x7fffffff;
   /* statistics */
   uint64_t n_minmers_before_filter = 0;
@@ -25,21 +48,27 @@ struct mm_built_index {
   unsigned long long hist_min_keys = 0, hist_max_keys = 0;
   float ms_scan = 0, ms_post = 0, ms_lookup = 0;
 };
-/* One shard of a contig-sharded index (--indexShards, DESIGN.md). count_only: stop after Sketch::index and leave every
- * distinct hash (ascending) in out->keys and its interval-point count in out->counts. Otherwise d_freq[n_freq] (device,
- * ascending) are the frequent hashes of the WHOLE reference: exactly those are flagged and dropped, in place of the
- * builder's own threshold, and the listed hashes this shard does not contain are appended after its keys as frequent keys
- * with no points. */
-struct mm_shard_freq {
-  int count_only;
+/* Which keys the builder flags as frequent seeds and drops from minmerIndex.
+ * OWN_THRESHOLD: the frequency threshold of kmer_pct_threshold `pct` over these contigs (an unsharded index).
+ * The two passes over one shard of a contig-sharded index (--indexShards, DESIGN.md):
+ * COUNT_ONLY: stop after Sketch::index and leave every distinct hash (ascending) in out->keys and its interval-point count
+ *   in out->counts.
+ * LISTED: d_freq[n_freq] (device, ascending) are the frequent hashes of the WHOLE reference: exactly those are flagged and
+ *   dropped, in place of the builder's own threshold, and the listed hashes this shard does not contain are appended after
+ *   its keys as frequent keys with no points. */
+struct mm_freq_rule {
+  enum { OWN_THRESHOLD, COUNT_ONLY, LISTED } mode;
+  float pct;
   const uint64_t *d_freq;
   uint64_t n_freq;
+
+  static mm_freq_rule own_threshold(float pct) { return mm_freq_rule{OWN_THRESHOLD, pct, nullptr, 0}; }
+  static mm_freq_rule count_only() { return mm_freq_rule{COUNT_ONLY, 0.f, nullptr, 0}; }
+  static mm_freq_rule listed(const uint64_t *d_freq, uint64_t n_freq) { return mm_freq_rule{LISTED, 0.f, d_freq, n_freq}; }
 };
 /* d_seq: the contigs as text, back to back, on the device (readable up to h_contig_off[n_contigs]); a contig of length 0
- * gets no records (so a shard keeps the global seqIds of its contigs). shard: nullptr = the frequency threshold of
- * kmer_pct_threshold over these contigs. Returns MM_OK or MM_E* */
+ * gets no records (so a shard keeps the global seqIds of its contigs). Returns MM_OK or MM_E* */
 int mm_build_index_device(const mm_params &p, const uint8_t *d_seq, const uint64_t *h_contig_off, int32_t n_contigs,
-                          float kmer_pct_threshold, const mm_shard_freq *shard, cudaStream_t st, int sm_count,
-                          mm_built_index *out, std::string &err);
+                          const mm_freq_rule &rule, cudaStream_t st, int sm_count, mm_built_index *out, std::string &err);
 
 #endif
