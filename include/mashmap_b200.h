@@ -331,6 +331,43 @@ int mm_inflate_blocks(mm_inflater *inf, const uint8_t *comp, const uint64_t *com
  * call (uploads, kernels, downloads) */
 int mm_inflater_last_ms(const mm_inflater *inf, float ms[2]);
 
+/* ---- FASTQ parsed on the device (mm_fastq.cu) ---------------------------------------------------------
+ * A handle that keeps one window of FASTQ text in device memory, on a stream of its own. Text goes in at the end of
+ * the window: as text (mm_fastq_append_text: a plain file, or members inflated on the host) or as BGZF members inflated
+ * straight into the window (mm_fastq_append_blocks: mm_inflate_blocks' arguments, without its output buffer). Inflated
+ * text never crosses PCIe. mm_fastq_cut parses the window (the record semantics of mashmap_b200/csrc/mm_fastq.h: four
+ * lines per record, the line reader's) and returns the names and the bases, packed to nibbles in the batch buffer's
+ * format (mm_map_segments_packed), byte-aligned per record. The window's first byte must start a record.
+ *   last = 0: only records whose fourth line ends inside the window; the rest, from the next header on, stays at the
+ *             front of the window for the next append. Zero records is possible: append more (a record larger than the
+ *             window grows it).
+ *   last = 1: the end of the file: every record whose header starts in the window; the window is emptied.
+ * An empty line in header position ends the file (ended = 1, the window is emptied). The arrays live in pinned memory
+ * owned by the handle and stay valid until the cut after next, so a caller can use window i while window i + 1 is
+ * parsed. Errors: MM_EINVAL (bad argument; a BGZF block that does not inflate, *bad_block = its index), MM_ENOMEM,
+ * MM_ECUDA; the text of the window is then undefined, and the caller drops the file. */
+typedef struct mm_fastq mm_fastq;
+typedef struct {
+  uint64_t n_records;
+  const uint64_t *name_off; /* [n_records + 1]: record i's name is names[name_off[i], name_off[i + 1]) */
+  const uint64_t *seq_len;  /* [n_records]: bases */
+  const uint64_t *nib_off;  /* [n_records + 1]: its nibbles are nibbles[nib_off[i], nib_off[i + 1]), (seq_len + 1) / 2 bytes */
+  const char *names;
+  const uint8_t *nibbles;
+  uint64_t consumed;        /* bytes of window text this cut took */
+  int ended;                /* 1: an empty header line ended the file */
+} mm_fastq_records;
+int mm_fastq_create(int device, mm_fastq **out);
+int mm_fastq_destroy(mm_fastq *fq);
+const char *mm_fastq_error(const mm_fastq *fq); /* NULL handle: the last mm_fastq_create error */
+int mm_fastq_append_text(mm_fastq *fq, const uint8_t *text, uint64_t n);
+int mm_fastq_append_blocks(mm_fastq *fq, const uint8_t *comp, const uint64_t *comp_off, const uint64_t *out_off,
+                           const uint32_t *crc, uint64_t n_blocks, int64_t *bad_block);
+int mm_fastq_cut(mm_fastq *fq, int last, mm_fastq_records *out);
+/* CUDA-event time of the last successful mm_fastq_cut, in milliseconds: [0] its kernels, [1] the whole call (kernels,
+ * copies and the host waits between them) */
+int mm_fastq_last_ms(const mm_fastq *fq, float ms[2]);
+
 #ifdef __cplusplus
 }
 #endif

@@ -68,6 +68,12 @@ class IndexStats(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_}
 
 
+class FastqRecords(C.Structure):
+    _fields_ = [("n_records", C.c_uint64), ("name_off", C.POINTER(C.c_uint64)), ("seq_len", C.POINTER(C.c_uint64)),
+                ("nib_off", C.POINTER(C.c_uint64)), ("names", C.c_void_p), ("nibbles", C.c_void_p), ("consumed", C.c_uint64),
+                ("ended", C.c_int)]
+
+
 _lib = None
 
 
@@ -120,6 +126,14 @@ def lib():
         L.mm_inflater_error.restype = C.c_char_p
         L.mm_inflate_blocks.argtypes = [vp, vp, vp, vp, vp, u64, vp, C.POINTER(C.c_int64)]
         L.mm_inflater_last_ms.argtypes = [vp, C.POINTER(C.c_float * 2)]
+        L.mm_fastq_create.argtypes = [C.c_int, C.POINTER(vp)]
+        L.mm_fastq_destroy.argtypes = [vp]
+        L.mm_fastq_error.argtypes = [vp]
+        L.mm_fastq_error.restype = C.c_char_p
+        L.mm_fastq_append_text.argtypes = [vp, vp, u64]
+        L.mm_fastq_append_blocks.argtypes = [vp, vp, vp, vp, vp, u64, C.POINTER(C.c_int64)]
+        L.mm_fastq_cut.argtypes = [vp, C.c_int, C.POINTER(FastqRecords)]
+        L.mm_fastq_last_ms.argtypes = [vp, C.POINTER(C.c_float * 2)]
         _lib = L
     return _lib
 
@@ -131,6 +145,8 @@ EXPORTED_SYMBOLS = [
     "mm_last_stage_ms", "mm_ctx_set_phase_hook", "mm_ctx_set_wait_mode", "mm_params_check", "mm_host_alloc", "mm_host_free",
     "mm_index_key_counts", "mm_index_build_shard", "mm_map_resident_l1_best", "mm_map_resident_with_best",
     "mm_inflater_create", "mm_inflater_destroy", "mm_inflater_error", "mm_inflate_blocks", "mm_inflater_last_ms",
+    "mm_fastq_create", "mm_fastq_destroy", "mm_fastq_error", "mm_fastq_append_text", "mm_fastq_append_blocks", "mm_fastq_cut",
+    "mm_fastq_last_ms",
 ]
 
 
@@ -219,6 +235,63 @@ class Inflater:
     def close(self):
         if self._h:
             lib().mm_inflater_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class FastqParser:
+    """mm_fastq: a window of FASTQ text in device memory, cut into records and packed to nibbles on the device"""
+
+    def __init__(self, device=0):
+        self._h = C.c_void_p()
+        rc = lib().mm_fastq_create(device, C.byref(self._h))
+        if rc != MM_OK:
+            raise MashmapError(rc, lib().mm_fastq_error(None).decode())
+
+    def _check(self, rc, what):
+        if rc != MM_OK:
+            raise MashmapError(rc, f"{what}: " + lib().mm_fastq_error(self._h).decode())
+
+    def append_text(self, text):
+        a = np.frombuffer(bytes(text), dtype=np.uint8)
+        self._check(lib().mm_fastq_append_text(self._h, _ptr(a), len(a)), "mm_fastq_append_text")
+
+    def append_blocks(self, comp, comp_off, out_off, crc):
+        """(rc, bad_block, error): BGZF member data inflated straight into the window"""
+        comp = _c(comp, np.uint8)
+        comp_off, out_off, crc = _c(comp_off, np.uint64), _c(out_off, np.uint64), _c(crc, np.uint32)
+        bad = C.c_int64()
+        rc = lib().mm_fastq_append_blocks(self._h, _ptr(comp), _ptr(comp_off), _ptr(out_off), _ptr(crc), len(crc), C.byref(bad))
+        return rc, bad.value, lib().mm_fastq_error(self._h).decode()
+
+    def cut(self, last):
+        """dict of the cut's records, copied out of the handle's buffers: names [bytes], seq_len, nibbles [bytes per
+        record], consumed, ended"""
+        r = FastqRecords()
+        self._check(lib().mm_fastq_cut(self._h, int(last), C.byref(r)), "mm_fastq_cut")
+        n = int(r.n_records)
+        noff = np.ctypeslib.as_array(r.name_off, shape=(n + 1,)).copy() if n else np.zeros(1, np.uint64)
+        boff = np.ctypeslib.as_array(r.nib_off, shape=(n + 1,)).copy() if n else np.zeros(1, np.uint64)
+        slen = np.ctypeslib.as_array(r.seq_len, shape=(n,)).copy() if n else np.zeros(0, np.uint64)
+        names = C.string_at(r.names, int(noff[-1])) if n else b""
+        nib = C.string_at(r.nibbles, int(boff[-1])) if n else b""
+        return {"names": [names[int(noff[i]):int(noff[i + 1])] for i in range(n)], "seq_len": slen,
+                "nibbles": [nib[int(boff[i]):int(boff[i + 1])] for i in range(n)], "nib_off": boff, "nib_all": nib,
+                "consumed": int(r.consumed), "ended": int(r.ended)}
+
+    def last_ms(self):
+        a = (C.c_float * 2)()
+        lib().mm_fastq_last_ms(self._h, C.byref(a))
+        return a[0], a[1]
+
+    def close(self):
+        if self._h:
+            lib().mm_fastq_destroy(self._h)
             self._h = C.c_void_p()
 
     def __del__(self):

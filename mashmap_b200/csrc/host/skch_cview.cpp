@@ -602,6 +602,54 @@ int skch_bgzf_read_digest(const char *path, uint64_t window_bytes, int threads, 
   return 0;
 }
 
+/* ---- FASTQ input (tests) ---- */
+
+namespace {
+thread_local std::string g_fastq_error;
+}  // namespace
+
+const char *skch_fastq_error() { return g_fastq_error.c_str(); }
+
+/* an FNV-1a digest of every record's name, length and nibbles (seqio::pack_bases' format) of a file, in order: through
+ * the line reader (window_bytes = 0), or through FastqReader in windows of window_bytes with the host build of
+ * mm_fastq.h (device < 0) or mm_fastq on `device`. out[4]: records, bases, digest, windows handed over. Returns 0; -1
+ * if FastqReader declines the file; -2 if the line reader cannot read it; -3 on an error (skch_fastq_error). */
+int skch_fastq_digest(const char *path, uint64_t window_bytes, int threads, int device, uint64_t *out)
+{
+  uint64_t h = 1469598103934665603ULL, nr = 0, nb = 0, nw = 0;
+  auto eat = [&h](const void *p, uint64_t n) {
+    for (uint64_t i = 0; i < n; i++) { h ^= ((const uint8_t *)p)[i]; h *= 1099511628211ULL; }
+    h ^= 0xFF; h *= 1099511628211ULL;
+  };
+  auto record = [&](const char *name, uint64_t name_len, uint64_t len, const uint8_t *nib) {
+    eat(name, name_len); eat(&len, 8); eat(nib, (len + 1) / 2);
+    nr++; nb += len;
+  };
+  if (window_bytes == 0) {
+    std::vector<uint8_t> nib;
+    if (!seqio::for_each_seq_in_file(path, {}, "", [&](const std::string &name, const std::string &seq) {
+          nib.assign((seq.size() + 1) / 2 + 1, 0);
+          seqio::pack_bases(seq.data(), seq.size(), nib.data());
+          record(name.data(), name.size(), seq.size(), nib.data());
+        }))
+      return -2;
+  } else {
+    seqio::FastqReader rd;
+    if (!rd.open(path)) return -1;
+    std::unique_ptr<seqio::FastqParser> p;
+    if (device < 0) p.reset(new seqio::HostFastqParser());
+    else p.reset(new seqio::DeviceFastqParser(device));
+    const int rc = rd.for_each_window(*p, window_bytes, threads, [&](const mm_fastq_records &r) {
+      for (uint64_t i = 0; i < r.n_records; i++)
+        record(r.names + r.name_off[i], r.name_off[i + 1] - r.name_off[i], r.seq_len[i], r.nibbles + r.nib_off[i]);
+      nw++;
+    });
+    if (rc != 0) { g_fastq_error = rd.error(); return -3; }
+  }
+  out[0] = nr; out[1] = nb; out[2] = h; out[3] = nw;
+  return 0;
+}
+
 /* records, bases and an FNV-1a digest of every (name, sequence) pair of a file in order, through the line reader (bulk = 0)
  * or the memory-mapped bulk reader (bulk = 1; returns -1 when it declines the file): compared with the same digest taken
  * through the reference's own reader (oracle/_ref, refh_read_file_digest) */

@@ -804,6 +804,7 @@ struct Map::Impl {
   std::vector<MappingResultsVector_t> results;
   std::vector<std::string> text;
   std::unique_ptr<seqio::DeviceInflater> inflater;  // BGZF queries, on the run's first device
+  std::unique_ptr<seqio::DeviceFastqParser> fastqParser;  // FASTQ queries, on the run's first device
 
   Impl(const Parameters &p, const Sketch &s, PostProcessResultsFn_t f, Map &m, Clock::time_point tCtor = Clock::now())
       : param(p), refSketch(s), processMappingResults(f), self(m), bm(p, s)
@@ -900,13 +901,14 @@ struct Map::Impl {
     seqCounter++;
   }
 
-  /* onSequence for every record of a mapped FASTA file; the bases go from the file mapping straight into the pinned
-   * batch buffer, copied by all host threads just before the batch is mapped (a BGZF window: from the inflated text) */
-  void ingestMapped(const seqio::FastaText &ff)
+  /* onSequence for every record of a window cut by a bulk reader; the bases go straight into the pinned batch buffer,
+   * written by all host threads just before the batch is mapped. Src gives size(), name(i), seq_len(i) and pack(i, dst),
+   * which writes record i's nibbles to dst. */
+  template <class Src>
+  void ingestRecords(const Src &src)
   {
     struct CopyJob { size_t rec; uint64_t dst; };
     std::vector<CopyJob> jobs;
-    const auto &recs = ff.records();
     auto runCopies = [&]() {
       if (jobs.empty()) return;
       const int T = std::max(1, std::min<int>(param.threads, (int)(jobs.size() / 16 + 1)));
@@ -916,7 +918,7 @@ struct Map::Impl {
           const size_t b = next.fetch_add(64);
           if (b >= jobs.size()) break;
           const size_t e = std::min(jobs.size(), b + 64);
-          for (size_t j = b; j < e; j++) ff.pack_bases(recs[jobs[j].rec], batch.nibbles(jobs[j].dst));
+          for (size_t j = b; j < e; j++) src.pack(jobs[j].rec, batch.nibbles(jobs[j].dst));
         }
       };
       if (T == 1) worker();
@@ -927,14 +929,13 @@ struct Map::Impl {
       }
       jobs.clear();
     };
-    for (size_t i = 0; i < recs.size(); i++) {
-      const seqio::FastaRecord &r = recs[i];
-      if (r.seq_len > (uint64_t)std::numeric_limits<offset_t>::max()) {
-        std::cerr << "[mashmap-b200] ERROR: sequence " << ff.name(r) << " is longer than 2^31 bases" << std::endl;
+    for (size_t i = 0; i < src.size(); i++) {
+      if (src.seq_len(i) > (uint64_t)std::numeric_limits<offset_t>::max()) {
+        std::cerr << "[mashmap-b200] ERROR: sequence " << src.name(i) << " is longer than 2^31 bases" << std::endl;
         exit(1);
       }
-      const offset_t len = (offset_t)r.seq_len;
-      const std::string name = ff.name(r);
+      const offset_t len = (offset_t)src.seq_len(i);
+      const std::string name = src.name(i);
       if (param.filterMode == filter::ONETOONE) qmetadata.push_back(ContigInfo{name, len});
       if (len < param.kmerSize) {
         std::cerr << std::endl << "WARNING, skch::Map::mapQuery, read " << name << " of " << len << "bp "
@@ -958,6 +959,32 @@ struct Map::Impl {
     runCopies();
   }
 
+  /* a mapped FASTA file, or one window of an inflated BGZF one: bases packed from the text */
+  void ingestMapped(const seqio::FastaText &ff)
+  {
+    struct Src {
+      const seqio::FastaText &ff;
+      size_t size() const { return ff.records().size(); }
+      std::string name(size_t i) const { return ff.name(ff.records()[i]); }
+      uint64_t seq_len(size_t i) const { return ff.records()[i].seq_len; }
+      void pack(size_t i, uint8_t *dst) const { ff.pack_bases(ff.records()[i], dst); }
+    };
+    ingestRecords(Src{ff});
+  }
+
+  /* one window of FASTQ records parsed on the device: bases already packed, copied */
+  void ingestPacked(const mm_fastq_records &r)
+  {
+    struct Src {
+      const mm_fastq_records &r;
+      size_t size() const { return (size_t)r.n_records; }
+      std::string name(size_t i) const { return std::string(r.names + r.name_off[i], r.name_off[i + 1] - r.name_off[i]); }
+      uint64_t seq_len(size_t i) const { return r.seq_len[i]; }
+      void pack(size_t i, uint8_t *dst) const { memcpy(dst, r.nibbles + r.nib_off[i], r.nib_off[i + 1] - r.nib_off[i]); }
+    };
+    ingestRecords(Src{r});
+  }
+
   void mapQuery()
   {  // computeMap.hpp:263-415
     outstrm.open(param.outFileName);
@@ -966,6 +993,21 @@ struct Map::Impl {
       seqio::FastaFile ff;
       if (!getenv("MM_SERIAL_INPUT") && ff.open(fileName, param.threads)) {  // plain FASTA: bulk path
         ingestMapped(ff);
+        continue;
+      }
+      seqio::FastqReader fq;
+      if (!getenv("MM_SERIAL_INPUT") && fq.open(fileName)) {  // FASTQ, plain or BGZF: parsed on the device, window by window
+        const int dev = param.devices.empty() ? param.device : param.devices[0];
+        if (!fastqParser) fastqParser.reset(new seqio::DeviceFastqParser(dev));
+        uint64_t windows = 0;
+        const int rc = fq.for_each_window(*fastqParser, seqio::fastq_window_bytes(param.batch_bases), param.threads,
+                                          [&](const mm_fastq_records &r) { ingestPacked(r); windows++; });
+        if (rc < 0) {
+          std::cerr << fq.error() << std::endl;
+          exit(1);
+        }
+        std::cerr << "[mashmap-b200::skch::Map::mapQuery] " << fileName << ": FASTQ, parsed on device " << dev << " in "
+                  << windows << " windows" << std::endl;
         continue;
       }
       seqio::BgzfFasta bz;

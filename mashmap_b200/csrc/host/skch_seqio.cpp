@@ -7,6 +7,7 @@
 #include <zlib.h>
 
 #include "../../../include/mashmap_b200.h"
+#include "../mm_fastq.h"
 #include "../mm_inflate.h"
 #if defined(__x86_64__)
 #include <immintrin.h>
@@ -224,8 +225,7 @@ struct NibTable {
   uint8_t t[256];
   NibTable()
   {
-    for (int i = 0; i < 256; i++) t[i] = 8;
-    t[(int)'A'] = t[(int)'a'] = 0; t[(int)'C'] = t[(int)'c'] = 1; t[(int)'T'] = t[(int)'t'] = 2; t[(int)'G'] = t[(int)'g'] = 3;
+    for (int i = 0; i < 256; i++) t[i] = mmf_nib((uint8_t)i);
   }
 };
 const NibTable NIB;
@@ -354,6 +354,11 @@ void DeviceInflater::release(void *p) { mm_host_free(p); }
 
 uint64_t bgzf_window_bytes(uint64_t batch_bases) { return std::min<uint64_t>(std::max<uint64_t>(batch_bases, 1 << 16), 1ULL << 28); }
 
+uint64_t fastq_window_bytes(uint64_t batch_bases)
+{
+  return std::min<uint64_t>(std::max<uint64_t>(2 * std::min<uint64_t>(batch_bases, 1ULL << 40), 1 << 16), 1ULL << 29);
+}
+
 namespace {
 
 inline uint32_t le16(const uint8_t *p) { return p[0] | ((uint32_t)p[1] << 8); }
@@ -391,13 +396,13 @@ int scan_member(const uint8_t *d, uint64_t size, uint64_t p, Member &m)
 
 }  // namespace
 
-BgzfFasta::~BgzfFasta()
+BgzfMembers::~BgzfMembers()
 {
   if (d_) munmap((void *)d_, size_);
   if (fd_ >= 0) close(fd_);
 }
 
-bool BgzfFasta::open(const std::string &filename)
+bool BgzfMembers::open(const std::string &filename)
 {
   path_ = filename;
   fd_ = ::open(filename.c_str(), O_RDONLY);
@@ -413,55 +418,40 @@ bool BgzfFasta::open(const std::string &filename)
   return scan_member(d_, size_, 0, mb) == 1;
 }
 
-bool BgzfFasta::corrupt(uint64_t off, const std::string &why)
+bool BgzfMembers::corrupt(uint64_t off, const std::string &why, std::string &error)
 {
-  error_ = "[mashmap-b200] ERROR: " + path_ + ": corrupt gzip/BGZF block at byte offset " + std::to_string(off) + ": " + why;
+  error = "[mashmap-b200] ERROR: " + path_ + ": corrupt gzip/BGZF block at byte offset " + std::to_string(off) + ": " + why;
   return false;
 }
 
-bool BgzfFasta::grow(BlockInflater &inf, Buf &b, uint64_t need)
+bool BgzfMembers::next(uint64_t want, const BlocksFn &blocks, const TextFn &text, std::string &error)
 {
-  if (need <= b.cap) return true;
-  const uint64_t cap = std::max<uint64_t>(need, b.cap + b.cap / 2);
-  char *q = (char *)inf.alloc(cap);
-  if (!q) {
-    error_ = "[mashmap-b200] ERROR: cannot allocate " + std::to_string(cap) + " bytes of host memory to read " + path_;
-    return false;
-  }
-  if (b.used) memcpy(q, b.p, b.used);
-  if (b.p) inf.release(b.p);
-  b.p = q;
-  b.cap = cap;
-  return true;
-}
-
-/* appends text to b until it holds `target` bytes or the members end */
-bool BgzfFasta::fill(BlockInflater &inf, Buf &b, uint64_t target)
-{
-  while (b.used < target && !eof_) {
+  uint64_t sent = 0;
+  while (sent < want && !eof_) {
     Member m;
     const int kind = scan_member(d_, size_, pos_, m);
     if (kind < 0) { eof_ = true; break; }
     if (kind == 0) { /* one gzip member through zlib, as gzread would inflate it */
       z_stream zs;
       memset(&zs, 0, sizeof zs);
-      if (inflateInit2(&zs, 15 + 16) != Z_OK) return corrupt(pos_, "zlib cannot start");
+      if (inflateInit2(&zs, 15 + 16) != Z_OK) return corrupt(pos_, "zlib cannot start", error);
       const uint64_t start = pos_;
       uint64_t in_left = size_ - pos_;
       const uint8_t *in = d_ + pos_;
       int rc = Z_OK;
+      chunk_.resize(1 << 20);
       while (true) {
-        if (!grow(inf, b, b.used + (1 << 20))) { inflateEnd(&zs); return false; }
-        zs.next_out = (Bytef *)b.p + b.used;
-        zs.avail_out = (uInt)std::min<uint64_t>(b.cap - b.used, 1u << 30);
+        zs.next_out = (Bytef *)chunk_.data();
+        zs.avail_out = (uInt)chunk_.size();
         const uInt feed = (uInt)std::min<uint64_t>(in_left, 1u << 30);
         zs.next_in = (Bytef *)in;
         zs.avail_in = feed;
-        const uInt out0 = zs.avail_out;
         rc = inflate(&zs, Z_NO_FLUSH);
-        b.used += out0 - zs.avail_out;
+        const uint64_t got = chunk_.size() - zs.avail_out;
         in += feed - zs.avail_in;
         in_left -= feed - zs.avail_in;
+        if (got && !text(chunk_.data(), got, error)) { inflateEnd(&zs); return false; }
+        sent += got;
         if (rc == Z_STREAM_END) break;
         if (rc == Z_BUF_ERROR && in_left == 0) break; /* cut short: gzread hands over what inflated, then ends */
         if (rc != Z_OK && rc != Z_BUF_ERROR) break;
@@ -471,10 +461,10 @@ bool BgzfFasta::fill(BlockInflater &inf, Buf &b, uint64_t target)
       inflateEnd(&zs);
       if (rc == Z_STREAM_END) pos_ = (uint64_t)(in - d_);
       else if (rc == Z_BUF_ERROR) eof_ = true;
-      else return corrupt(start, msg ? msg : "zlib error");
+      else return corrupt(start, msg ? msg : "zlib error", error);
       continue;
     }
-    /* consecutive BGZF members up to the target, at least one: one call of the inflater */
+    /* consecutive BGZF members up to `want`, at least one: one call of the inflater */
     coff_.assign(1, 0);
     ooff_.assign(1, 0);
     moff_.clear();
@@ -487,7 +477,7 @@ bool BgzfFasta::fill(BlockInflater &inf, Buf &b, uint64_t target)
       out += m.isize;
       ooff_.push_back(out);
       p = m.next;
-      if (b.used + out >= target || scan_member(d_, size_, p, m) != 1) break;
+      if (sent + out >= want || scan_member(d_, size_, p, m) != 1) break;
     }
     stage_.resize(coff_.back());
     for (size_t i = 0; i < moff_.size(); i++) {
@@ -495,15 +485,53 @@ bool BgzfFasta::fill(BlockInflater &inf, Buf &b, uint64_t target)
       scan_member(d_, size_, moff_[i], mi);
       memcpy(stage_.data() + coff_[i], d_ + mi.data_off, mi.data_len);
     }
-    if (!grow(inf, b, b.used + out + 1)) return false;
     int64_t bad = -1;
     std::string why;
-    if (inf.inflate(stage_.data(), coff_.data(), ooff_.data(), crc_.data(), moff_.size(), (uint8_t *)b.p + b.used, &bad, why) != 0)
-      return corrupt(bad >= 0 && (size_t)bad < moff_.size() ? moff_[(size_t)bad] : pos_, why);
-    b.used += out;
+    const int rc = blocks(stage_.data(), coff_.data(), ooff_.data(), crc_.data(), moff_.size(), &bad, why, error);
+    if (rc < 0) return false;
+    if (rc != 0) return corrupt(bad >= 0 && (size_t)bad < moff_.size() ? moff_[(size_t)bad] : pos_, why, error);
+    sent += out;
     pos_ = p;
   }
   return true;
+}
+
+bool BgzfFasta::grow(BlockInflater &inf, Buf &b, uint64_t need, std::string &error)
+{
+  if (need <= b.cap) return true;
+  const uint64_t cap = std::max<uint64_t>(need, b.cap + b.cap / 2);
+  char *q = (char *)inf.alloc(cap);
+  if (!q) {
+    error = "[mashmap-b200] ERROR: cannot allocate " + std::to_string(cap) + " bytes of host memory to read " + mem_.path();
+    return false;
+  }
+  if (b.used) memcpy(q, b.p, b.used);
+  if (b.p) inf.release(b.p);
+  b.p = q;
+  b.cap = cap;
+  return true;
+}
+
+/* appends text to b until it holds `target` bytes or the members end */
+bool BgzfFasta::fill(BlockInflater &inf, Buf &b, uint64_t target, std::string &error)
+{
+  if (b.used >= target) return true;
+  return mem_.next(
+      target - b.used,
+      [&](const uint8_t *comp, const uint64_t *coff, const uint64_t *ooff, const uint32_t *crc, uint64_t n, int64_t *bad,
+          std::string &why, std::string &err) {
+        if (!grow(inf, b, b.used + ooff[n] + 1, err)) return -1;
+        const int rc = inf.inflate(comp, coff, ooff, crc, n, (uint8_t *)b.p + b.used, bad, why);
+        if (rc == 0) b.used += ooff[n];
+        return rc == 0 ? 0 : 1;
+      },
+      [&](const uint8_t *t, uint64_t n, std::string &err) {
+        if (!grow(inf, b, b.used + n, err)) return false;
+        memcpy(b.p + b.used, t, n);
+        b.used += n;
+        return true;
+      },
+      error);
 }
 
 int BgzfFasta::for_each_window(BlockInflater &inf, uint64_t window_bytes, int threads, const std::function<void(const FastaText &)> &fn)
@@ -515,13 +543,13 @@ int BgzfFasta::for_each_window(BlockInflater &inf, uint64_t window_bytes, int th
     ~Release() { if (a.p) inf.release(a.p); if (b.p) inf.release(b.p); }
   } release{inf, cur, nxt};
   window_bytes = std::max<uint64_t>(window_bytes, 1);
-  if (!fill(inf, cur, window_bytes)) return -1;
+  if (!fill(inf, cur, window_bytes, error_)) return -1;
   if (cur.used == 0 || cur.p[0] != '>') return 1;
   FastaText text;
   while (cur.used) {
     /* cut after the last record start that is not the window's first byte; a record longer than the window grows it */
     uint64_t cut = cur.used;
-    if (!eof_) {
+    if (!mem_.at_end()) {
       cut = 0;
       for (uint64_t q = cur.used; q > 1;) {
         const char *g = (const char *)memrchr(cur.p + 1, '>', q - 1);
@@ -530,25 +558,262 @@ int BgzfFasta::for_each_window(BlockInflater &inf, uint64_t window_bytes, int th
         q = (uint64_t)(g - cur.p);
       }
       if (cut == 0) {
-        if (!fill(inf, cur, cur.used + window_bytes)) return -1;
+        if (!fill(inf, cur, cur.used + window_bytes, error_)) return -1;
         continue;
       }
     }
     const uint64_t carry = cur.used - cut;
-    if (!grow(inf, nxt, carry + window_bytes + 1)) return -1;
+    if (!grow(inf, nxt, carry + window_bytes + 1, error_)) return -1;
     memcpy(nxt.p, cur.p + cut, carry);
     nxt.used = carry;
     bool ok = true;
+    std::string err;
     std::thread next;
-    if (!eof_) next = std::thread([&]() { ok = fill(inf, nxt, carry + window_bytes); });
+    if (!mem_.at_end()) next = std::thread([&]() { ok = fill(inf, nxt, carry + window_bytes, err); });
     text.parse(cur.p, cut, threads);
     fn(text);
     if (next.joinable()) next.join();
-    if (!ok) return -1;
+    if (!ok) { error_ = err; return -1; }
     std::swap(cur, nxt);
     nxt.used = 0;
   }
   return 0;
+}
+
+/* ---- FASTQ ---- */
+
+void *FastqParser::alloc(uint64_t bytes) { return malloc(bytes); }
+void FastqParser::release(void *p) { free(p); }
+
+int HostFastqParser::append_text(const uint8_t *text, uint64_t n, std::string &)
+{
+  win_.insert(win_.end(), text, text + n);
+  return 0;
+}
+
+int HostFastqParser::append_blocks(const uint8_t *comp, const uint64_t *comp_off, const uint64_t *out_off, const uint32_t *crc,
+                                   uint64_t n_blocks, int64_t *bad_block, std::string &error)
+{
+  const uint64_t at = win_.size();
+  win_.resize(at + out_off[n_blocks] - out_off[0]);
+  HostInflater inf;
+  const int rc = inf.inflate(comp, comp_off, out_off, crc, n_blocks, win_.data() + at - out_off[0], bad_block, error);
+  if (rc != 0) win_.resize(at);
+  return rc;
+}
+
+/* the host build of mm_fastq_cut: the same statement (mm_fastq.h) with one lane */
+int HostFastqParser::cut(int last, mm_fastq_records &res, std::string &)
+{
+  const uint8_t *text = win_.data();
+  const uint64_t n = win_.size();
+  nl_.clear();
+  for (uint64_t p = 0; p < n; p += 4)
+    for (uint32_t w = mmf_newline_mask(mmf_word(text, n, p)); w; w &= w - 1) nl_.push_back(p + (uint64_t)(__builtin_ctz(w) >> 3));
+  const uint64_t N = nl_.size();
+  uint64_t first_empty = mmf_empty_header_after(text, n, ~0ULL, ~0ULL);
+  for (uint64_t j = 0; j < N; j++) first_empty = std::min(first_empty, mmf_empty_header_after(text, n, j, nl_[j]));
+  uint64_t consumed = 0;
+  int ended = 0;
+  const uint64_t R = mmf_extent(nl_.data(), N, n, last, first_empty, &consumed, &ended);
+  Out &o = out_[next_];
+  next_ ^= 1;
+  o.name_off.assign(1, 0);
+  o.nib_off.assign(1, 0);
+  o.seq_len.clear();
+  o.names.clear();
+  o.nibbles.clear();
+  for (uint64_t r = 0; r < R; r++) {
+    const mmf_record f = mmf_fields(text, n, nl_.data(), N, r);
+    o.names.append((const char *)text + f.name, f.name_len);
+    for (uint64_t k = 0; k < (f.seq_len + 1) / 2; k++) o.nibbles.push_back(mmf_nib_byte(text + f.seq, f.seq_len, k));
+    o.name_off.push_back(o.names.size());
+    o.nib_off.push_back(o.nibbles.size());
+    o.seq_len.push_back(f.seq_len);
+  }
+  res.n_records = R;
+  res.name_off = o.name_off.data();
+  res.nib_off = o.nib_off.data();
+  res.seq_len = o.seq_len.data();
+  res.names = o.names.data();
+  res.nibbles = o.nibbles.data();
+  res.consumed = consumed;
+  res.ended = ended;
+  win_.erase(win_.begin(), win_.begin() + (ptrdiff_t)consumed);
+  return 0;
+}
+
+DeviceFastqParser::DeviceFastqParser(int device)
+{
+  if (mm_fastq_create(device, &fq_) != MM_OK) {
+    std::cerr << "[mashmap-b200] ERROR: mm_fastq_create: " << mm_fastq_error(nullptr) << std::endl;
+    exit(1);
+  }
+}
+
+DeviceFastqParser::~DeviceFastqParser() { mm_fastq_destroy(fq_); }
+
+int DeviceFastqParser::append_text(const uint8_t *text, uint64_t n, std::string &error)
+{
+  const int rc = mm_fastq_append_text(fq_, text, n);
+  if (rc != MM_OK) error = mm_fastq_error(fq_);
+  return rc;
+}
+
+int DeviceFastqParser::append_blocks(const uint8_t *comp, const uint64_t *comp_off, const uint64_t *out_off, const uint32_t *crc,
+                                     uint64_t n_blocks, int64_t *bad_block, std::string &error)
+{
+  const int rc = mm_fastq_append_blocks(fq_, comp, comp_off, out_off, crc, n_blocks, bad_block);
+  if (rc != MM_OK) error = mm_fastq_error(fq_);
+  return rc;
+}
+
+int DeviceFastqParser::cut(int last, mm_fastq_records &out, std::string &error)
+{
+  const int rc = mm_fastq_cut(fq_, last, &out);
+  if (rc != MM_OK) error = mm_fastq_error(fq_);
+  return rc;
+}
+
+void *DeviceFastqParser::alloc(uint64_t bytes)
+{
+  void *p = nullptr;
+  return mm_host_alloc(&p, bytes) == MM_OK ? p : nullptr;
+}
+
+void DeviceFastqParser::release(void *p) { mm_host_free(p); }
+
+FastqReader::~FastqReader()
+{
+  if (d_) munmap((void *)d_, size_);
+  if (fd_ >= 0) close(fd_);
+}
+
+bool FastqReader::open(const std::string &filename)
+{
+  path_ = filename;
+  fd_ = ::open(filename.c_str(), O_RDONLY);
+  if (fd_ < 0) return false;
+  struct stat st;
+  if (fstat(fd_, &st) != 0 || !S_ISREG(st.st_mode) || st.st_size < 1) return false;
+  char first = 0;
+  if (pread(fd_, &first, 1, 0) != 1) return false;
+  if (first == '@') {
+    size_ = (uint64_t)st.st_size;
+    void *m = mmap(nullptr, size_, PROT_READ, MAP_PRIVATE, fd_, 0);
+    if (m == MAP_FAILED) { size_ = 0; return false; }
+    d_ = (const uint8_t *)m;
+    madvise(m, size_, MADV_SEQUENTIAL);
+    return true;
+  }
+  if (!mem_.open(filename)) return false;
+  /* the first byte of the text, as the line reader sees it */
+  gzFile f = gzopen(filename.c_str(), "rb");
+  if (!f) return false;
+  const int got = gzread(f, &first, 1);
+  gzclose(f);
+  bgzf_ = got == 1 && first == '@';
+  return bgzf_;
+}
+
+/* appends text to the parser's window until it holds `target` bytes or the input ends */
+bool FastqReader::load(FastqParser &p, uint64_t target, int threads)
+{
+  std::string why;
+  if (bgzf_) {
+    if (held_ >= target) return true;
+    return mem_.next(
+        target - held_,
+        [&](const uint8_t *comp, const uint64_t *coff, const uint64_t *ooff, const uint32_t *crc, uint64_t n, int64_t *bad,
+            std::string &w, std::string &) {
+          const int rc = p.append_blocks(comp, coff, ooff, crc, n, bad, w);
+          if (rc == 0) held_ += ooff[n];
+          return rc == 0 ? 0 : 1;
+        },
+        [&](const uint8_t *t, uint64_t n, std::string &err) {
+          if (p.append_text(t, n, why) == 0) { held_ += n; return true; }
+          err = "[mashmap-b200] ERROR: " + path_ + ": " + why;
+          return false;
+        },
+        error_);
+  }
+  while (held_ < target && pos_ < size_) {
+    const uint64_t n = std::min(target - held_, size_ - pos_);
+    const uint64_t chunk = std::min<uint64_t>(n, 1ULL << 28);
+    if (chunk > stage_cap_) {
+      if (stage_) p.release(stage_);
+      stage_cap_ = std::max(chunk, std::min<uint64_t>(target, 1ULL << 28));
+      stage_ = (uint8_t *)p.alloc(stage_cap_);
+      if (!stage_) {
+        stage_cap_ = 0;
+        error_ = "[mashmap-b200] ERROR: cannot allocate " + std::to_string(chunk) + " bytes of host memory to read " + path_;
+        return false;
+      }
+    }
+    /* the mapped file into the pinned stage, by all host threads (the page faults of the mapping are most of the cost) */
+    const int T = (int)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)std::max(1, threads), chunk / (1 << 20) + 1));
+    auto copy = [&](int t) {
+      const uint64_t lo = chunk * (uint64_t)t / (uint64_t)T, hi = chunk * (uint64_t)(t + 1) / (uint64_t)T;
+      memcpy(stage_ + lo, d_ + pos_ + lo, hi - lo);
+    };
+    if (T == 1) copy(0);
+    else {
+      std::vector<std::thread> pool;
+      for (int t = 0; t < T; t++) pool.emplace_back(copy, t);
+      for (auto &th : pool) th.join();
+    }
+    if (p.append_text(stage_, chunk, why) != 0) {
+      error_ = "[mashmap-b200] ERROR: " + path_ + ": " + why;
+      return false;
+    }
+    pos_ += chunk;
+    held_ += chunk;
+  }
+  return true;
+}
+
+int FastqReader::for_each_window(FastqParser &p, uint64_t window_bytes, int threads, const std::function<void(const mm_fastq_records &)> &fn)
+{
+  window_bytes = std::max<uint64_t>(window_bytes, 1);
+  struct Release {
+    FastqParser &p;
+    uint8_t *&stage;
+    uint64_t &cap;
+    ~Release() { if (stage) p.release(stage); stage = nullptr; cap = 0; }
+  } release{p, stage_, stage_cap_};
+  struct Cut { mm_fastq_records rec; bool done = false; };
+  /* appends and cuts until a cut returns records or the file ends (a record larger than the window grows it), or after
+   * one cut when `once`: a cut's results last until the cut after next, so only one cut may run while fn reads */
+  auto step = [&](Cut &c, bool once) {
+    uint64_t target = held_ + window_bytes;
+    while (true) {
+      if (!load(p, target, threads)) return false;
+      const int last = at_end() ? 1 : 0;
+      std::string why;
+      if (p.cut(last, c.rec, why) != 0) {
+        error_ = "[mashmap-b200] ERROR: " + path_ + ": " + why;
+        return false;
+      }
+      held_ -= c.rec.consumed;
+      c.done = last || c.rec.ended;
+      if (c.rec.n_records || c.done || once) return true;
+      target = std::max(held_ + window_bytes, 2 * held_);
+    }
+  };
+  Cut cur;
+  if (!step(cur, false)) return -1;
+  while (true) {
+    Cut nxt;
+    bool ok = true;
+    std::thread th;
+    if (!cur.done) th = std::thread([&]() { ok = step(nxt, true); });
+    if (cur.rec.n_records) fn(cur.rec);
+    if (th.joinable()) th.join();
+    if (!ok) return -1;
+    if (cur.done) return 0;
+    if (!nxt.rec.n_records && !nxt.done && !step(nxt, false)) return -1;
+    cur = nxt;
+  }
 }
 
 }  // namespace seqio

@@ -14,6 +14,8 @@
 #include <unordered_set>
 #include <vector>
 
+#include "../../../include/mashmap_b200.h"
+
 namespace skch {
 namespace seqio {
 
@@ -107,19 +109,52 @@ class DeviceInflater : public BlockInflater {
 };
 
 /*
- * FASTA in BGZF (bgzip) members, read window by window. A member is BGZF when its gzip header has FEXTRA with a 'BC'
- * subfield of length 2; its BSIZE, CRC32 and ISIZE place its data and its text before anything is inflated, so a
- * window's members go to the BlockInflater in one call. A member that is not BGZF, or one cut short by the end of the
+ * The gzip members of a BGZF file, walked in order. A member is BGZF when its gzip header has FEXTRA with a 'BC'
+ * subfield of length 2; its BSIZE, CRC32 and ISIZE place its data and its text before anything is inflated, so a run of
+ * BGZF members goes to the caller's inflater in one call. A member that is not BGZF, or one cut short by the end of the
  * file, is inflated on the host by zlib, in order, and bytes after the last member are ignored: the text is the one
  * gzread gives the line reader. A corrupt member is an error, where gzread would end the text early.
  */
+class BgzfMembers {
+ public:
+  BgzfMembers() = default;
+  ~BgzfMembers();
+  BgzfMembers(const BgzfMembers &) = delete;
+  /* false if the file cannot be mapped or its first member is not BGZF */
+  bool open(const std::string &filename);
+  bool at_end() const { return eof_; }
+  const std::string &path() const { return path_; }
+  /* a run of BGZF members: mm_inflate_blocks' arguments (ooff[0] = 0, ooff[n] = its text bytes); 0, or nonzero with
+   * *bad_block = the failing member's index in the run (or -1) and `why`; a negative return means the callee set
+   * `error` itself (not a corrupt member) */
+  typedef std::function<int(const uint8_t *comp, const uint64_t *coff, const uint64_t *ooff, const uint32_t *crc, uint64_t n,
+                            int64_t *bad_block, std::string &why, std::string &error)> BlocksFn;
+  /* text that zlib inflated on the host; false if the callee set `error` */
+  typedef std::function<bool(const uint8_t *text, uint64_t n, std::string &error)> TextFn;
+  /* hands the members' text on, in order, until `want` bytes went out or the members end; false on an error (a corrupt
+   * member: `error` names the file and the member's byte offset) */
+  bool next(uint64_t want, const BlocksFn &blocks, const TextFn &text, std::string &error);
+
+ private:
+  bool corrupt(uint64_t off, const std::string &why, std::string &error);
+
+  std::string path_;
+  const uint8_t *d_ = nullptr;
+  uint64_t size_ = 0, pos_ = 0;
+  bool eof_ = false;
+  int fd_ = -1;
+  std::vector<uint8_t> stage_, chunk_;
+  std::vector<uint64_t> coff_, ooff_, moff_;
+  std::vector<uint32_t> crc_;
+};
+
+/* FASTA in BGZF (bgzip) members (BgzfMembers), read window by window. */
 class BgzfFasta {
  public:
   BgzfFasta() = default;
-  ~BgzfFasta();
   BgzfFasta(const BgzfFasta &) = delete;
   /* false if the file cannot be mapped or its first member is not BGZF: the line reader handles it */
-  bool open(const std::string &filename);
+  bool open(const std::string &filename) { return mem_.open(filename); }
   /*
    * Inflates the text in windows of about window_bytes (grown while one record does not fit), cuts each window at its
    * last record start, carries the rest into the next window, and hands each window's records, parsed by `threads`
@@ -132,22 +167,104 @@ class BgzfFasta {
 
  private:
   struct Buf { char *p = nullptr; uint64_t cap = 0, used = 0; };
-  bool grow(BlockInflater &inf, Buf &b, uint64_t need);
-  bool fill(BlockInflater &inf, Buf &b, uint64_t target);
-  bool corrupt(uint64_t off, const std::string &why);
+  bool grow(BlockInflater &inf, Buf &b, uint64_t need, std::string &error);
+  bool fill(BlockInflater &inf, Buf &b, uint64_t target, std::string &error);
+
+  BgzfMembers mem_;
+  std::string error_;
+};
+
+/*
+ * The one step of the FASTQ window reader that a caller chooses: a window of FASTQ text that grows at its end and is
+ * cut into records, with the contract of mm_fastq_append_text / mm_fastq_append_blocks / mm_fastq_cut
+ * (include/mashmap_b200.h; record semantics in mm_fastq.h). The program passes DeviceFastqParser; the tests pass
+ * HostFastqParser (the host build of mm_fastq.h). Each returns 0, or nonzero with `error` (and *bad_block) set. alloc /
+ * release give the reader's staging buffers (pinned ones for the device).
+ */
+class FastqParser {
+ public:
+  virtual ~FastqParser() = default;
+  virtual int append_text(const uint8_t *text, uint64_t n, std::string &error) = 0;
+  virtual int append_blocks(const uint8_t *comp, const uint64_t *comp_off, const uint64_t *out_off, const uint32_t *crc,
+                            uint64_t n_blocks, int64_t *bad_block, std::string &error) = 0;
+  virtual int cut(int last, mm_fastq_records &out, std::string &error) = 0;
+  virtual void *alloc(uint64_t bytes);
+  virtual void release(void *p);
+};
+
+class HostFastqParser : public FastqParser {
+ public:
+  int append_text(const uint8_t *text, uint64_t n, std::string &error) override;
+  int append_blocks(const uint8_t *comp, const uint64_t *comp_off, const uint64_t *out_off, const uint32_t *crc,
+                    uint64_t n_blocks, int64_t *bad_block, std::string &error) override;
+  int cut(int last, mm_fastq_records &out, std::string &error) override;
+
+ private:
+  struct Out { std::vector<uint64_t> name_off, nib_off, seq_len; std::string names; std::vector<uint8_t> nibbles; };
+  std::vector<uint8_t> win_;
+  std::vector<uint64_t> nl_;
+  Out out_[2];
+  int next_ = 0;
+};
+
+class DeviceFastqParser : public FastqParser {
+ public:
+  /* exits the program (status 1) if the device cannot be used */
+  explicit DeviceFastqParser(int device);
+  ~DeviceFastqParser() override;
+  int append_text(const uint8_t *text, uint64_t n, std::string &error) override;
+  int append_blocks(const uint8_t *comp, const uint64_t *comp_off, const uint64_t *out_off, const uint32_t *crc,
+                    uint64_t n_blocks, int64_t *bad_block, std::string &error) override;
+  int cut(int last, mm_fastq_records &out, std::string &error) override;
+  void *alloc(uint64_t bytes) override;
+  void release(void *p) override;
+
+ private:
+  mm_fastq *fq_ = nullptr;
+};
+
+/*
+ * FASTQ read window by window through a FastqParser: a plain file (mapped, staged by the host threads and appended as
+ * text) or a BGZF one (BgzfMembers: BGZF runs appended as blocks, zlib members as text). The records are exactly the line
+ * reader's (mm_fastq.h).
+ */
+class FastqReader {
+ public:
+  FastqReader() = default;
+  ~FastqReader();
+  FastqReader(const FastqReader &) = delete;
+  /* false unless the file is plain or BGZF and its text starts with '@': the line reader handles it */
+  bool open(const std::string &filename);
+  bool bgzf() const { return bgzf_; }
+  /*
+   * Appends about window_bytes of text at a time (more while one record does not fit), cuts the window, and hands each
+   * cut's records to fn, in order. Window i+1 is appended and cut while fn runs on window i. Stops after an empty line in
+   * header position. Returns 0, or -1 on an error (error() says which; a corrupt member: the file and its byte offset).
+   */
+  int for_each_window(FastqParser &p, uint64_t window_bytes, int threads, const std::function<void(const mm_fastq_records &)> &fn);
+  const std::string &error() const { return error_; }
+
+ private:
+  bool load(FastqParser &p, uint64_t target, int threads);
+  bool at_end() const { return bgzf_ ? mem_.at_end() : pos_ == size_; }
 
   std::string path_, error_;
-  const uint8_t *d_ = nullptr;
+  bool bgzf_ = false;
+  BgzfMembers mem_;
+  const uint8_t *d_ = nullptr; /* plain: the mapped file */
   uint64_t size_ = 0, pos_ = 0;
-  bool eof_ = false;
   int fd_ = -1;
-  std::vector<uint8_t> stage_;
-  std::vector<uint64_t> coff_, ooff_, moff_;
-  std::vector<uint32_t> crc_;
+  uint64_t held_ = 0;          /* bytes in the parser's window */
+  uint8_t *stage_ = nullptr;    /* plain: pinned staging from the parser, for one for_each_window */
+  uint64_t stage_cap_ = 0;
 };
 
 /* text bytes per BGZF window for a run of --batchBases b: b, kept within [64 KiB, 256 MiB] */
 uint64_t bgzf_window_bytes(uint64_t batch_bases);
+
+/* text bytes per FASTQ window for a run of --batchBases b: 2 b (a FASTQ record's text is about twice its bases: the
+ * quality line), kept within [64 KiB, 512 MiB] */
+uint64_t fastq_window_bytes(uint64_t batch_bases);
 
 /*
  * The device's input format (include/mashmap_b200.h, mm_map_segments_packed): one nibble per base, base i of the

@@ -66,6 +66,22 @@ const char *status_text(int rc)
 
 }  // namespace
 
+const char *mmi_status_text(int rc) { return status_text(rc); }
+
+cudaError_t mmi_launch_inflate(const uint8_t *comp, const uint64_t *coff, const uint64_t *ooff, const uint32_t *crc, uint64_t n,
+                               uint8_t *out, int32_t *status, cudaStream_t st)
+{
+  if (n == 0) return cudaSuccess;
+  int dev = 0, per_sm = 0, sms = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_inflate, kWarps * 32, 0);
+  if (e != cudaSuccess) return e;
+  const unsigned grid = (unsigned)std::min<uint64_t>((uint64_t)std::max(per_sm, 1) * (uint64_t)sms, (n + kWarps - 1) / kWarps);
+  k_inflate<<<grid, kWarps * 32, 0, st>>>(comp, coff, ooff, crc, n, out, status);
+  return cudaGetLastError();
+}
+
 struct mm_inflater {
   int device = -1;
   int grid = 0;

@@ -36,6 +36,15 @@ enum mmi_status {
   MMI_E_CRC = 10,     /* inflated text whose CRC-32 differs from the member's (checked by the callers) */
 };
 
+#if defined(__CUDACC__)
+/* internal to libmashmap_b200.so (mm_fastq.cu inflates BGZF members into its window): k_inflate over n blocks whose
+ * arrays are all in device memory, as mm_inflate_blocks lays them out, on stream st; status[i] gets block i's mmi_status
+ * (the CRC-32 checked). mmi_status_text says what a status means. */
+cudaError_t mmi_launch_inflate(const uint8_t *comp, const uint64_t *coff, const uint64_t *ooff, const uint32_t *crc, uint64_t n,
+                               uint8_t *out, int32_t *status, cudaStream_t st);
+const char *mmi_status_text(int rc);
+#endif
+
 #define MMI_FAST 9 /* lookup-table bits: codes up to 9 bits decode in one table read, longer ones canonically */
 
 template <int N>

@@ -65,6 +65,8 @@ def lib():
         L.skch_bgzf_readers_diff.restype = C.c_int64
         L.skch_bgzf_read_digest.argtypes = [C.c_char_p, C.c_uint64, C.c_int, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64),
                                             C.POINTER(C.c_uint64)]
+        L.skch_fastq_error.restype = C.c_char_p
+        L.skch_fastq_digest.argtypes = [C.c_char_p, C.c_uint64, C.c_int, C.c_int, C.POINTER(C.c_uint64 * 4)]
         L.skch_index_from_minmers.argtypes = [C.c_void_p, C.c_uint64, C.c_int, C.c_float]
         L.skch_index_from_minmers.restype = C.c_void_p
         L.skch_index_build.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float]
@@ -333,6 +335,19 @@ def gzread_text(path):
     buf = np.zeros(max(n, 1), dtype=np.uint8)
     lib().skch_gzread_text(path.encode(), buf.ctypes.data_as(C.c_void_p), n)
     return buf[:n].tobytes()
+
+
+def fastq_digest(path, window_bytes=0, threads=2, device=-1):
+    """(records, bases, digest, windows) of a file's records (name, length, nibbles): the line reader (window_bytes = 0),
+    or the FASTQ window reader with the host build of mm_fastq.h (device < 0) or mm_fastq on that device. None if the
+    window reader declines the file; RuntimeError on a read error."""
+    out = (C.c_uint64 * 4)()
+    rc = lib().skch_fastq_digest(path.encode(), int(window_bytes), threads, device, C.byref(out))
+    if rc == -1:
+        return None
+    if rc != 0:
+        raise RuntimeError(lib().skch_fastq_error().decode() if rc == -3 else f"cannot read {path}")
+    return tuple(int(x) for x in out)
 
 
 def bgzf_readers_diff(path, window_bytes, threads=2):
