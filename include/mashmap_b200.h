@@ -162,7 +162,12 @@ int mm_index_upload(mm_ctx *ctx,
  * (contig i = [contig_offsets[i], contig_offsets[i+1])), in host memory or (seqs_on_device != 0) in device memory.
  * Lower case and IUPAC codes are normalised as the reference does. Records are the reference's; where its std::sort on
  * (wpos, wpos_end) leaves exact ties in an unspecified order, this builder keeps emission order (DESIGN.md).
- * keep_lookup != 0 keeps the flat lookup arrays on the device for mm_index_download. */
+ * keep: MM_KEEP_* bits. MM_KEEP_LOOKUP keeps the flat lookup arrays on the device for mm_index_download;
+ * MM_KEEP_UNFILTERED keeps minmerIndex as it was BEFORE dropFreqSeedSet -- what the reference writes with --saveIndex
+ * (winSketch.hpp:127-134) -- for mm_index_download_unfiltered. Both stay until taken, released (mm_index_release_kept),
+ * or the context's index is replaced (a build, mm_index_upload, an adopted blob, a shared index) or destroyed. */
+#define MM_KEEP_LOOKUP 1
+#define MM_KEEP_UNFILTERED 2
 typedef struct mm_index_stats {
   uint64_t n_minmers;                /* minmerIndex.size() after dropFreqSeedSet                     */
   uint64_t n_minmers_before_filter;  /* "minmer windows picked from reference" (winSketch.hpp:228)  */
@@ -175,8 +180,19 @@ typedef struct mm_index_stats {
   float ms_scan, ms_post, ms_lookup, ms_total;
 } mm_index_stats;
 int mm_index_build(mm_ctx *ctx, const char *seqs, int seqs_on_device, const uint64_t *contig_offsets, int32_t n_contigs,
-                   const int32_t *contig_name_id, const int32_t *contig_group, float kmer_pct_threshold, int keep_lookup,
+                   const int32_t *contig_name_id, const int32_t *contig_group, float kmer_pct_threshold, int keep,
                    mm_index_stats *stats);
+/* The same index from a minmer list instead of the sequence: replaces what skch::Sketch does with --loadIndex --
+ * loadBinaryIndex / readIndexTSV (winSketch.hpp:321-348), then index() (:379-404) and computeFreqHist / computeFreqSeedSet
+ * / dropFreqSeedSet (:410-453, :488-504) -- and leaves the context as mm_index_build would. mi[n]: the records as
+ * --saveIndex writes them (before the frequent-seed drop), in host memory or (mi_on_device != 0) in device memory; their
+ * _pad is ignored. contig_len / contig_name_id / contig_group as mm_index_upload's. Every record is checked before it is
+ * used: a seqId outside [0, n_contigs), a record out of (seqId, wpos) order, or a negative wpos / wpos_end returns
+ * MM_EINVAL with mm_last_error naming the first such record, and the context then has no index. keep: MM_KEEP_* bits.
+ * stats: n_minmers_before_filter = n, n_chunks = 0. */
+int mm_index_build_minmers(mm_ctx *ctx, const mm_minmer *mi, uint64_t n, int mi_on_device, const int32_t *contig_len,
+                           const int32_t *contig_name_id, const int32_t *contig_group, int32_t n_contigs,
+                           float kmer_pct_threshold, int keep, mm_index_stats *stats);
 /* A reference index sharded by contig (DESIGN.md, "Index shards"): each shard is one context's image of a contiguous range
  * of contigs, built in two passes so that the frequent seeds are those of the WHOLE reference (computeFreqHist counts a
  * hash's interval points over all contigs, winSketch.hpp:410-453).
@@ -196,11 +212,17 @@ int mm_index_key_counts(mm_ctx *ctx, const char *seqs, int seqs_on_device, const
 int mm_index_build_shard(mm_ctx *ctx, const char *seqs, int seqs_on_device, const uint64_t *contig_offsets, int32_t first_contig,
                          int32_t n_shard_contigs, const int32_t *contig_len, const int32_t *contig_name_id,
                          const int32_t *contig_group, int32_t n_contigs, const uint64_t *freq_hashes, uint64_t n_freq,
-                         int keep_lookup, mm_index_stats *stats);
+                         int keep, mm_index_stats *stats);
 /* Host copies of the index mm_index_build left on the device, in mm_index_upload's argument formats (any pointer may be
- * NULL; the lookup arrays need keep_lookup). Sizes: mm_index_stats. */
+ * NULL; the lookup arrays need MM_KEEP_LOOKUP). Sizes: mm_index_stats. */
 int mm_index_download(mm_ctx *ctx, mm_minmer *minmer_index, uint64_t *keys, uint64_t *offsets, mm_ipoint *points,
                       uint8_t *key_is_freq);
+/* Host copy of the records a build kept with MM_KEEP_UNFILTERED: minmerIndex before dropFreqSeedSet, in reference order,
+ * _pad = 0 -- the records Sketch::saveIndex writes (winSketch.hpp:127-134, :270-293). out[cap]; *n = their count. On
+ * MM_ECAPACITY they stay kept: call again with room for *n. Once taken they are freed on the device. */
+int mm_index_download_unfiltered(mm_ctx *ctx, mm_minmer *out, uint64_t cap, uint64_t *n);
+/* Frees what MM_KEEP_LOOKUP and MM_KEEP_UNFILTERED kept on the device; the index stays. Replaces nothing in the reference. */
+int mm_index_release_kept(mm_ctx *ctx);
 
 /* sketchCutoffs (Map::setProbs, computeMap.hpp:178-258) and
  * min_hits[s] = Stat::estimateMinimumHitsRelaxed(s, k, pi, 0.95) for s in [0, n_min_hits)

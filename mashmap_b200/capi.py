@@ -15,6 +15,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libmashmap_b200.so")
 
 MM_OK, MM_EINVAL, MM_ENODEVICE, MM_ECUDA, MM_ENOMEM, MM_ECAPACITY, MM_ESTATE = 0, -1, -2, -3, -4, -5, -6
+MM_KEEP_LOOKUP, MM_KEEP_UNFILTERED = 1, 2
 
 # record layouts == include/mashmap_b200.h
 minmer_dtype = np.dtype(
@@ -100,6 +101,9 @@ def lib():
         L.mm_tables_upload.argtypes = [vp, vp, i32, vp, i32]
         L.mm_index_build.argtypes = [vp, vp, C.c_int, vp, i32, vp, vp, C.c_float, C.c_int, C.POINTER(IndexStats)]
         L.mm_index_download.argtypes = [vp, vp, vp, vp, vp, vp]
+        L.mm_index_build_minmers.argtypes = [vp, vp, u64, C.c_int, vp, vp, vp, i32, C.c_float, C.c_int, C.POINTER(IndexStats)]
+        L.mm_index_download_unfiltered.argtypes = [vp, vp, u64, C.POINTER(u64)]
+        L.mm_index_release_kept.argtypes = [vp]
         L.mm_index_blob.argtypes = [vp, C.POINTER(vp), C.POINTER(u64)]
         L.mm_index_blob_alloc.argtypes = [vp, u64, C.POINTER(vp)]
         L.mm_index_adopt_blob.argtypes = [vp]
@@ -146,7 +150,7 @@ EXPORTED_SYMBOLS = [
     "mm_index_key_counts", "mm_index_build_shard", "mm_map_resident_l1_best", "mm_map_resident_with_best",
     "mm_inflater_create", "mm_inflater_destroy", "mm_inflater_error", "mm_inflate_blocks", "mm_inflater_last_ms",
     "mm_fastq_create", "mm_fastq_destroy", "mm_fastq_error", "mm_fastq_append_text", "mm_fastq_append_blocks", "mm_fastq_cut",
-    "mm_fastq_last_ms",
+    "mm_fastq_last_ms", "mm_index_build_minmers", "mm_index_download_unfiltered", "mm_index_release_kept",
 ]
 
 
@@ -160,6 +164,10 @@ def params_check(kmer_size, seg_length, sketch_size):
 
 def _ptr(a):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
+
+
+def _keep(keep_lookup, keep_unfiltered):
+    return (MM_KEEP_LOOKUP if keep_lookup else 0) | (MM_KEEP_UNFILTERED if keep_unfiltered else 0)
 
 
 def _c(a, dtype):
@@ -368,24 +376,58 @@ class Context:
                                             _ptr(cg), len(contig_len)))
 
     def index_build(self, seqs, contig_offsets, contig_name_id=None, contig_group=None, kmer_pct_threshold=0.001, keep_lookup=False,
-                    device_ptr=None):
+                    device_ptr=None, keep_unfiltered=False):
         """mm_index_build: the reference index built on the device. seqs: uint8 array (contigs back to back) on the host, or
         pass device_ptr (int) for text that is already in device memory. Returns the statistics as a dict."""
         offs = _c(contig_offsets, np.uint64)
         n = len(offs) - 1
         cn = None if contig_name_id is None else _c(contig_name_id, np.int32)
         cg = None if contig_group is None else _c(contig_group, np.int32)
+        keep = _keep(keep_lookup, keep_unfiltered)
         st = IndexStats()
         if device_ptr is not None:
             rc = self._L.mm_index_build(self._h, C.c_void_p(int(device_ptr)), 1, _ptr(offs), n, _ptr(cn), _ptr(cg), kmer_pct_threshold,
-                                        1 if keep_lookup else 0, C.byref(st))
+                                        keep, C.byref(st))
         else:
             a = np.ascontiguousarray(seqs, dtype=np.uint8)
             rc = self._L.mm_index_build(self._h, _ptr(a), 0, _ptr(offs), n, _ptr(cn), _ptr(cg), kmer_pct_threshold,
-                                        1 if keep_lookup else 0, C.byref(st))
+                                        keep, C.byref(st))
         self._check(rc)
         self._index_stats = st.as_dict()
         return self._index_stats
+
+    def index_build_minmers(self, minmers, contig_len, contig_name_id=None, contig_group=None, kmer_pct_threshold=0.001,
+                            keep_lookup=False, keep_unfiltered=False, device_ptr=None):
+        """mm_index_build_minmers: the index built on the device from a minmer list as --saveIndex writes it (minmer_dtype,
+        host), or from device_ptr (int) holding len(minmers) such records in device memory. Returns the statistics."""
+        n = len(minmers)
+        cl = _c(contig_len, np.int32)
+        cn = None if contig_name_id is None else _c(contig_name_id, np.int32)
+        cg = None if contig_group is None else _c(contig_group, np.int32)
+        st = IndexStats()
+        if device_ptr is not None:
+            src, on_device = C.c_void_p(int(device_ptr)), 1
+        else:
+            mi = _c(minmers, minmer_dtype)
+            src, on_device = _ptr(mi), 0
+        self._check(self._L.mm_index_build_minmers(self._h, src, n, on_device, _ptr(cl), _ptr(cn), _ptr(cg), len(cl), kmer_pct_threshold,
+                                                   _keep(keep_lookup, keep_unfiltered), C.byref(st)))
+        self._index_stats = st.as_dict()
+        return self._index_stats
+
+    def index_download_unfiltered(self):
+        """mm_index_download_unfiltered: the records a build kept with keep_unfiltered=True (before the frequent-seed drop)"""
+        n = C.c_uint64()
+        rc = self._L.mm_index_download_unfiltered(self._h, None, 0, C.byref(n))
+        out = np.zeros(n.value, dtype=minmer_dtype)
+        if rc == MM_ECAPACITY:
+            rc = self._L.mm_index_download_unfiltered(self._h, _ptr(out), n.value, C.byref(n))
+        self._check(rc)
+        return out
+
+    def index_release_kept(self):
+        """mm_index_release_kept: free what keep_lookup / keep_unfiltered kept on the device"""
+        self._check(self._L.mm_index_release_kept(self._h))
 
     def index_key_counts(self, seqs, contig_offsets):
         """pass 1 of a contig-sharded index (mm_index_key_counts): (distinct hashes ascending, their interval-point counts,

@@ -274,7 +274,7 @@ void parseandSave(int argc, char **argv, Parameters &parameters)
     if (parameters.index_shards > 1) {
       if (parameters.host_index || !parameters.saveIndexFilename.empty() || !parameters.loadIndexFilename.empty())
         usage_error("ERROR, --indexShards builds every shard on its device: it cannot be combined with --hostIndex, --saveIndex or "
-                    "--loadIndex, which keep one index on the host");
+                    "--loadIndex, which build, save or load one unsharded index");
       if (parameters.devices.size() > (size_t)parameters.index_shards)
         usage_error("ERROR, --indexShards " + v + " with " + std::to_string(parameters.devices.size()) +
                     " devices: every device must hold a shard (read-parallel copies of a sharded index are not supported)");

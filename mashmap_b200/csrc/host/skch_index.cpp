@@ -18,6 +18,10 @@
 #include <tuple>
 #include <unordered_set>
 
+#include <fcntl.h>
+#include <sys/stat.h>
+#include <unistd.h>
+
 #include "../mm_hash.h"
 #include "../mm_winmachine.h"
 #include "skch_seqio.hpp"
@@ -283,17 +287,43 @@ Sketch::Sketch(const Parameters &p) : param(p)
 {
   checkPathLimits(param);
   build();
-  if (!deviceBuildPending()) finish();
+  if (!deviceBuildPending() && !deviceLoadPending()) finish();
 }
 
-Sketch::~Sketch() { free(deviceText_); }
+Sketch::~Sketch()
+{
+  free(deviceText_);
+  if (loaded_) mm_host_free(loaded_);
+}
 
 void Sketch::deviceBuildDone(int freq_threshold) const
 {
   free(deviceText_);
   deviceText_ = nullptr;
   deviceTextOffsets_.clear();
+  if (loaded_) mm_host_free(loaded_);
+  loaded_ = nullptr;
   freqThreshold = freq_threshold;
+}
+
+void Sketch::saveDeviceIndex(mm_ctx *ctx, const mm_index_stats &st) const
+{
+  auto t0 = std::chrono::steady_clock::now();
+  BigVec<MinmerInfo> mi(st.n_minmers_before_filter);
+  BigVec<hash_t> keys(st.n_keys);
+  BigVec<uint64_t> offsets(st.n_keys + 1, 0);
+  BigVec<IntervalPoint> points(st.n_points);
+  uint64_t n = 0;
+  int rc = mm_index_download_unfiltered(ctx, mi.data(), mi.size(), &n);
+  if (rc == MM_OK && st.n_keys) rc = mm_index_download(ctx, nullptr, keys.data(), offsets.data(), points.data(), nullptr);
+  if (rc == MM_OK) rc = mm_index_release_kept(ctx);  // before the batch buffers are sized: mapping sees the memory of a run without --saveIndex
+  if (rc != MM_OK) {
+    std::cerr << "[mashmap-b200::skch::Sketch] ERROR: cannot download the index to save it: " << mm_last_error(ctx) << std::endl;
+    exit(1);
+  }
+  writeIndexFiles(mi.data(), n, keys.data(), offsets.data(), points.data(), keys.size());
+  std::cerr << "[mashmap-b200::skch::Sketch] index saved to " << param.saveIndexFilename << " in "
+            << std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count() << " s" << std::endl;
 }
 
 Sketch::Sketch(const Parameters &p, const std::vector<ContigInfo> &contigs, const std::vector<const char *> &seqs)
@@ -361,9 +391,7 @@ void Sketch::finish()
     saving_ = true;
     index();
     saving_ = false;
-    if (param.saveIndexFilename.extension() == ".tsv") saveIndexTSV(param.saveIndexFilename.string());
-    else saveIndexBinary(param.saveIndexFilename.string());
-    savePosListBinary(param.saveIndexFilename.string());
+    writeIndexFiles(minmerIndex.data(), minmerIndex.size(), lookupKeys.data(), lookupOffsets.data(), lookupPoints.data(), lookupKeys.size());
   }
   index();
   std::cerr << "[mashmap-b200::skch::Sketch] lookup index + frequency filter in "
@@ -378,17 +406,18 @@ void Sketch::build()
     std::string name;
     while (getline(fl, name)) allowed.insert(name);
   }
+  // the device builds the index unless --hostIndex asks for the host: from the text, or from the records of --loadIndex
+  const bool device = !param.host_index && param.kmerSize >= 8 && param.kmerSize <= 32;
+  const bool on_device = device && param.loadIndexFilename.empty();
   if (!param.loadIndexFilename.empty()) {
-    bool ok = param.loadIndexFilename.extension() == ".tsv" ? loadIndexTSV(param.loadIndexFilename.string())
-                                                            : loadIndexBinary(param.loadIndexFilename.string());
+    bool ok = device ? loadIndexForDevice()
+                     : param.loadIndexFilename.extension() == ".tsv" ? loadIndexTSV(param.loadIndexFilename.string())
+                                                                     : loadIndexBinary(param.loadIndexFilename.string());
     if (!ok) {
       std::cerr << "[mashmap-b200::skch::Sketch::build] ERROR: cannot load index " << param.loadIndexFilename << std::endl;
       exit(1);
     }
   }
-  // the device builds the index unless the host arrays are needed (index files) or asked for
-  const bool on_device = !param.host_index && param.loadIndexFilename.empty() && param.saveIndexFilename.empty() &&
-                         param.kmerSize >= 8 && param.kmerSize <= 32;
   // contigs are read by this thread and sketched by a pool; outputs are appended in input order
   struct Task { std::string seq; seqno_t id; };
   std::vector<std::unique_ptr<Task>> tasks;
@@ -453,6 +482,7 @@ void Sketch::build()
     if (!deviceText_) deviceText_ = (char *)malloc(64);  // only empty contigs: still "pending", the device reports an empty index
     return;
   }
+  if (deviceLoadPending()) return;
   if (param.loadIndexFilename.empty()) {
     std::vector<MI_Type> outputs(tasks.size());
     std::atomic<size_t> next{0};
@@ -732,33 +762,45 @@ std::vector<hash_t> globalFrequentSeeds(const std::vector<const hash_t *> &keys,
   return freq;
 }
 
-void Sketch::saveIndexTSV(const std::string &path) const
+void Sketch::writeIndexFiles(const MinmerInfo *mi, size_t n, const hash_t *keys, const uint64_t *offsets, const IntervalPoint *points,
+                             size_t n_keys) const
+{
+  const std::string path = param.saveIndexFilename.string();
+  if (param.saveIndexFilename.extension() == ".tsv") saveIndexTSV(path, mi, n);
+  else saveIndexBinary(path, mi, n);
+  savePosListBinary(path, keys, offsets, points, n_keys);
+}
+
+void Sketch::saveIndexTSV(const std::string &path, const MinmerInfo *records, size_t n)
 {  // winSketch.hpp:270-279
   std::ofstream o(path);
   o << "seqId" << "\t" << "strand" << "\t" << "start" << "\t" << "end" << "\t" << "hash\n";
-  for (auto &mi : minmerIndex)
+  for (size_t i = 0; i < n; i++) {
+    const MinmerInfo &mi = records[i];
     o << mi.seqId << "\t" << std::to_string(mi.strand) << "\t" << mi.wpos << "\t" << mi.wpos_end << "\t" << mi.hash << "\n";
+  }
 }
 
-void Sketch::saveIndexBinary(const std::string &prefix) const
+void Sketch::saveIndexBinary(const std::string &prefix, const MinmerInfo *records, size_t n)
 {  // winSketch.hpp:284-293
   std::ofstream o(prefix + ".index", std::ios::binary);
-  size_t size = minmerIndex.size();
+  size_t size = n;
   o.write((const char *)&size, sizeof(size));
-  o.write((const char *)minmerIndex.data(), size * sizeof(MinmerInfo));
+  o.write((const char *)records, size * sizeof(MinmerInfo));
 }
 
-void Sketch::savePosListBinary(const std::string &prefix) const
+void Sketch::savePosListBinary(const std::string &prefix, const hash_t *keys, const uint64_t *offsets, const IntervalPoint *points,
+                               size_t n_keys)
 {  // winSketch.hpp:298-315 (key order is unspecified in the reference's hash map; ascending here)
   std::ofstream o(prefix + ".map", std::ios::binary);
-  size_t size = lookupKeys.size();
+  size_t size = n_keys;
   o.write((const char *)&size, sizeof(size));
-  for (size_t i = 0; i < lookupKeys.size(); i++) {
-    hash_t key = lookupKeys[i];
+  for (size_t i = 0; i < n_keys; i++) {
+    hash_t key = keys[i];
     o.write((const char *)&key, sizeof(key));
-    size_t n = lookupOffsets[i + 1] - lookupOffsets[i];
+    size_t n = offsets[i + 1] - offsets[i];
     o.write((const char *)&n, sizeof(n));
-    o.write((const char *)&lookupPoints[lookupOffsets[i]], n * sizeof(IntervalPoint));
+    o.write((const char *)&points[offsets[i]], n * sizeof(IntervalPoint));
   }
 }
 
@@ -775,15 +817,84 @@ bool Sketch::loadIndexTSV(const std::string &path)
   return true;
 }
 
+/* PREFIX.index (winSketch.hpp:338-348): the header's record count n, then n records, read by `threads` threads in disjoint
+ * ranges into alloc(n). A file too short for its header's count stops the run (exit status 1) with a message naming the
+ * file and its size, before anything is allocated; bytes after the records are ignored, as in the reference. false: the
+ * file cannot be opened. */
+template <class Alloc>
+static bool readIndexBinary(const std::string &path, int threads, Alloc &&alloc, uint64_t &n)
+{
+  const int fd = open(path.c_str(), O_RDONLY);
+  if (fd < 0) return false;
+  auto die = [&](const std::string &m) {
+    std::cerr << "[mashmap-b200::skch::Sketch::build] ERROR: " << path << ": " << m << std::endl;
+    exit(1);
+  };
+  struct stat sb;
+  if (fstat(fd, &sb) != 0) die("cannot read its size");
+  const uint64_t bytes = (uint64_t)sb.st_size;
+  uint64_t count = 0;
+  if (bytes < 8 || pread(fd, &count, 8, 0) != 8)
+    die("the file holds " + std::to_string(bytes) + " bytes, too few for the 8-byte record count");
+  if (count > (bytes - 8) / sizeof(MinmerInfo))
+    die("the file holds " + std::to_string(bytes) + " bytes, too few for the " + std::to_string(count) +
+        " records its header counts (8 + 24 x " + std::to_string(count) + " bytes)");
+  char *dst = (char *)alloc(count);
+  const uint64_t total = count * sizeof(MinmerInfo);
+  const uint64_t T = (uint64_t)std::max(1, std::min(threads, 64));
+  const uint64_t part = (total + T - 1) / T;
+  std::atomic<bool> failed{false};
+  std::vector<std::thread> pool;
+  for (uint64_t t = 0; t < T; t++)
+    pool.emplace_back([&, t]() {
+      for (uint64_t at = std::min(total, t * part), end = std::min(total, at + part); at < end;) {
+        const ssize_t got = pread(fd, dst + at, (size_t)std::min<uint64_t>(end - at, 1ULL << 30), (off_t)(8 + at));
+        if (got <= 0) { failed = true; return; }
+        at += (uint64_t)got;
+      }
+    });
+  for (auto &th : pool) th.join();
+  close(fd);
+  if (failed) die("read error");
+  n = count;
+  return true;
+}
+
 bool Sketch::loadIndexBinary(const std::string &prefix)
 {  // winSketch.hpp:338-348 (the interval points are rebuilt from the minmers, which gives the same lists)
-  std::ifstream in(prefix + ".index", std::ios::binary);
-  if (!in) return false;
-  size_t size = 0;
-  in.read((char *)&size, sizeof(size));
-  minmerIndex.resize(size);
-  in.read((char *)minmerIndex.data(), size * sizeof(MinmerInfo));
-  return (bool)in;
+  uint64_t n = 0;
+  return readIndexBinary(prefix + ".index", param.threads, [&](uint64_t count) {
+    minmerIndex.resize(count);
+    return minmerIndex.data();
+  }, n);
+}
+
+/* --loadIndex for the device: the records in pinned memory, as the file holds them (the device checks them); a TSV is
+ * parsed into minmerIndex first and moved there */
+bool Sketch::loadIndexForDevice()
+{
+  auto pinned = [&](uint64_t count) {
+    void *p = nullptr;
+    const uint64_t bytes = std::max<uint64_t>(count, 1) * sizeof(MinmerInfo);
+    if (mm_host_alloc(&p, bytes) != MM_OK) {
+      std::cerr << "[mashmap-b200::skch::Sketch::build] ERROR: cannot allocate " << bytes << " bytes of pinned host memory for the index" << std::endl;
+      exit(1);
+    }
+    loaded_ = (MinmerInfo *)p;
+    return loaded_;
+  };
+  const std::string path = param.loadIndexFilename.string();
+  if (param.loadIndexFilename.extension() == ".tsv") {
+    if (!loadIndexTSV(path)) return false;
+    nLoaded_ = minmerIndex.size();
+    if (nLoaded_) memcpy(pinned(nLoaded_), minmerIndex.data(), nLoaded_ * sizeof(MinmerInfo));
+    else pinned(0);
+    MI_Type().swap(minmerIndex);
+    loadedFile_ = path;
+    return true;
+  }
+  loadedFile_ = path + ".index";
+  return readIndexBinary(loadedFile_, param.threads, pinned, nLoaded_);
 }
 
 }  // namespace skch

@@ -84,13 +84,23 @@ class Sketch {
   BigVec<IntervalPoint> lookupPoints;
   std::vector<uint8_t> lookupKeyIsFreq;      // frequentSeeds membership per key (winSketch.hpp:488-495)
 
-  /* The index is built ON THE DEVICE by default (mm_index_build, called by skch::BatchMapper which owns the device
-   * context): the constructor then only reads the contigs; minmerIndex and the lookup arrays stay empty on the host.
-   * --hostIndex, --saveIndex and --loadIndex keep everything on the host as before. */
+  /* The index is built ON THE DEVICE unless --hostIndex is given (by skch::BatchMapper, which owns the device context):
+   * the constructor then only reads the contigs, and with --loadIndex the file's records; minmerIndex and the lookup
+   * arrays stay empty on the host. From the text (mm_index_build) or from the loaded records (mm_index_build_minmers);
+   * with --saveIndex, after either, the build keeps what the files hold and saveDeviceIndex writes them. --hostIndex
+   * keeps everything on the host, --saveIndex and --loadIndex included. */
   bool deviceBuildPending() const { return deviceText_ != nullptr; }
   const char *deviceText() const { return deviceText_; }
   const std::vector<uint64_t> &deviceTextOffsets() const { return deviceTextOffsets_; }
-  void deviceBuildDone(int freq_threshold) const;  // releases the text, records the threshold
+  bool deviceLoadPending() const { return loaded_ != nullptr; }
+  const MinmerInfo *loadedRecords() const { return loaded_; }  // pinned host memory (mm_host_alloc)
+  uint64_t loadedCount() const { return nLoaded_; }
+  const std::string &loadedFile() const { return loadedFile_; }
+  void deviceBuildDone(int freq_threshold) const;  // releases the text or the loaded records, records the threshold
+  /* --saveIndex of an index mm_index_build or mm_index_build_minmers made with MM_KEEP_LOOKUP | MM_KEEP_UNFILTERED (st:
+   * its statistics): downloads the records before the frequent-seed drop and the lookup, releases what the build kept on
+   * the device, and writes the files finish() would write (records' _pad bytes zero) */
+  void saveDeviceIndex(mm_ctx *ctx, const mm_index_stats &st) const;
 
   /* --align: the bases of contig i (metadata[i]) as nibbles (seqio::pack_bases: ACGT, everything else N), base 0 in the
    * low nibble of the first byte. Read with the contigs in every index mode and kept for the whole run (not kept by the
@@ -103,9 +113,10 @@ class Sketch {
   MI_Type::const_iterator getMinmerIndexEnd() const { return minmerIndex.end(); }
 
   // --saveIndex / --loadIndex (winSketch.hpp:270-374): TSV and PREFIX.index/.map binary formats
-  void saveIndexTSV(const std::string &path) const;
-  void saveIndexBinary(const std::string &prefix) const;
-  void savePosListBinary(const std::string &prefix) const;
+  static void saveIndexTSV(const std::string &path, const MinmerInfo *mi, size_t n);
+  static void saveIndexBinary(const std::string &prefix, const MinmerInfo *mi, size_t n);
+  static void savePosListBinary(const std::string &prefix, const hash_t *keys, const uint64_t *offsets, const IntervalPoint *points,
+                                size_t n_keys);
 
  private:
   const Parameters &param;
@@ -113,6 +124,9 @@ class Sketch {
   bool saving_ = false;
   mutable char *deviceText_ = nullptr;           // contigs back to back (text), until the device has built the index
   mutable std::vector<uint64_t> deviceTextOffsets_;
+  mutable MinmerInfo *loaded_ = nullptr;         // --loadIndex: the file's records, until the device has indexed them
+  uint64_t nLoaded_ = 0;
+  std::string loadedFile_;
   BigVec<uint8_t> refNibbles_;                   // --align only
   std::vector<uint64_t> refNibbleOffsets_;       // byte offset of each contig in refNibbles_
 
@@ -120,6 +134,10 @@ class Sketch {
   void keepForAlign(const char *seq, size_t len);  // appends a contig to refNibbles_
   void buildFromMemory(const std::vector<const char *> &seqs);
   void finish();
+  // the --saveIndex files (the records before the frequent-seed drop, and the lookup), as the extension asks
+  void writeIndexFiles(const MinmerInfo *mi, size_t n, const hash_t *keys, const uint64_t *offsets, const IntervalPoint *points,
+                       size_t n_keys) const;
+  bool loadIndexForDevice();
   void index();
   void computeFreqHist();
   void dropFreqSeedSet();

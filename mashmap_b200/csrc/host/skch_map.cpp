@@ -27,6 +27,25 @@ namespace {
 typedef std::chrono::steady_clock Clock;
 double since(Clock::time_point t0) { return std::chrono::duration<double>(Clock::now() - t0).count(); }
 
+/* the reference's log lines of an index (winSketch.hpp:228, :403, :418-449) from the statistics of a device build */
+void logIndexStats(const Parameters &param, const mm_index_stats &st)
+{
+  std::cerr << "[mashmap-b200::skch::Sketch::build] minmer windows picked from reference = " << st.n_minmers_before_filter << std::endl;
+  std::cerr << "[mashmap-b200::skch::Sketch::index] unique minmers = " << st.n_keys << std::endl;
+  if (!st.n_keys) {
+    std::cerr << "[mashmap-b200::skch::Sketch::computeFreqHist] No minmers." << std::endl;
+    return;
+  }
+  std::cerr << "[mashmap-b200::skch::Sketch::computeFreqHist] Frequency histogram of minmer interval points = (" << st.hist_min_count << ", "
+            << st.hist_min_keys << ") ... (" << st.hist_max_count << ", " << st.hist_max_keys << ")" << std::endl;
+  if (st.freq_threshold != std::numeric_limits<int>::max())
+    std::cerr << "[mashmap-b200::skch::Sketch::computeFreqHist] With threshold " << param.kmer_pct_threshold
+              << "%, ignore minmers occurring >= " << st.freq_threshold << " times during lookup." << std::endl;
+  else
+    std::cerr << "[mashmap-b200::skch::Sketch::computeFreqHist] With threshold " << param.kmer_pct_threshold
+              << "%, consider all minmers during lookup." << std::endl;
+}
+
 [[noreturn]] void die(const std::string &msg)
 {
   std::cerr << "[mashmap-b200] ERROR: " << msg << std::endl;
@@ -209,30 +228,34 @@ BatchMapper::BatchMapper(const Parameters &p, const Sketch &refsketch) : param(p
     std::vector<int32_t> clen(refSketch.metadata.size());
     for (size_t i = 0; i < clen.size(); i++) clen[i] = refSketch.metadata[i].len;
     if (refSketch.deviceBuildPending()) {
-      // skch::Sketch's build / index / computeFreqHist / dropFreqSeedSet on the device (mm_index_build.cu); the log lines
-      // are the reference's (winSketch.hpp:228, :403, :418-449)
+      // skch::Sketch's build / index / computeFreqHist / dropFreqSeedSet on the device (mm_index_build.cu); with --saveIndex
+      // the builder keeps the records before the frequent-seed drop and the lookup, which the files hold
+      const bool save = !param.saveIndexFilename.empty();
       mm_index_stats st;
       auto t0 = Clock::now();
       rc = mm_index_build(ctx, refSketch.deviceText(), 0, refSketch.deviceTextOffsets().data(), (int32_t)clen.size(), contigNameId.data(),
-                          refIdGroup.data(), param.kmer_pct_threshold, 0, &st);
+                          refIdGroup.data(), param.kmer_pct_threshold, save ? MM_KEEP_LOOKUP | MM_KEEP_UNFILTERED : 0, &st);
       if (rc != MM_OK) die(std::string("mm_index_build: ") + mm_last_error(ctx) + " (--hostIndex builds the index on the host)");
-      std::cerr << "[mashmap-b200::skch::Sketch::build] minmer windows picked from reference = " << st.n_minmers_before_filter << std::endl;
-      std::cerr << "[mashmap-b200::skch::Sketch::index] unique minmers = " << st.n_keys << std::endl;
-      if (st.n_keys) {
-        std::cerr << "[mashmap-b200::skch::Sketch::computeFreqHist] Frequency histogram of minmer interval points = (" << st.hist_min_count << ", "
-                  << st.hist_min_keys << ") ... (" << st.hist_max_count << ", " << st.hist_max_keys << ")" << std::endl;
-        if (st.freq_threshold != std::numeric_limits<int>::max())
-          std::cerr << "[mashmap-b200::skch::Sketch::computeFreqHist] With threshold " << param.kmer_pct_threshold
-                    << "%, ignore minmers occurring >= " << st.freq_threshold << " times during lookup." << std::endl;
-        else
-          std::cerr << "[mashmap-b200::skch::Sketch::computeFreqHist] With threshold " << param.kmer_pct_threshold
-                    << "%, consider all minmers during lookup." << std::endl;
-      } else {
-        std::cerr << "[mashmap-b200::skch::Sketch::computeFreqHist] No minmers." << std::endl;
-      }
+      logIndexStats(param, st);
       std::cerr << "[mashmap-b200::skch::Sketch] index built on the device in " << since(t0) << " s (window scan " << st.ms_scan * 1e-3
                 << " s over " << st.n_chunks << " chunks, " << st.n_fixed_chunks << " re-scanned exactly; records " << st.ms_post * 1e-3
                 << " s; lookup + frequency filter " << st.ms_lookup * 1e-3 << " s)" << std::endl;
+      if (save) refSketch.saveDeviceIndex(ctx, st);
+      refSketch.deviceBuildDone(st.freq_threshold);
+    } else if (refSketch.deviceLoadPending()) {
+      // --loadIndex: Sketch::index / computeFreqHist / dropFreqSeedSet over the file's records on the device; with
+      // --saveIndex too, the loaded records and their lookup are written again (winSketch.hpp:122-134 saves after a load)
+      const bool save = !param.saveIndexFilename.empty();
+      mm_index_stats st;
+      auto t0 = Clock::now();
+      rc = mm_index_build_minmers(ctx, refSketch.loadedRecords(), refSketch.loadedCount(), 0, clen.data(), contigNameId.data(),
+                                  refIdGroup.data(), (int32_t)clen.size(), param.kmer_pct_threshold,
+                                  save ? MM_KEEP_LOOKUP | MM_KEEP_UNFILTERED : 0, &st);
+      if (rc != MM_OK) die("cannot load index " + refSketch.loadedFile() + ": " + mm_last_error(ctx));
+      logIndexStats(param, st);
+      std::cerr << "[mashmap-b200::skch::Sketch] index built on the device from the " << refSketch.loadedCount() << " records of "
+                << refSketch.loadedFile() << " in " << since(t0) << " s (lookup + frequency filter " << st.ms_lookup * 1e-3 << " s)" << std::endl;
+      if (save) refSketch.saveDeviceIndex(ctx, st);
       refSketch.deviceBuildDone(st.freq_threshold);
     } else {
       rc = mm_index_upload(ctx, refSketch.minmerIndex.data(), refSketch.minmerIndex.size(), refSketch.lookupKeys.data(),

@@ -107,7 +107,7 @@ struct Parameters {
   uint64_t sparsity_hash_threshold = std::numeric_limits<uint64_t>::max();
   bool legacy_output = false;
   // B200 additions (not in the reference)
-  bool host_index = false;        // --hostIndex: build the reference index on the host (implied by --saveIndex / --loadIndex)
+  bool host_index = false;        // --hostIndex: build the reference index on the host (also for --saveIndex / --loadIndex)
   int device = 0;                 // CUDA device ordinal (--device)
   std::vector<int> devices;       // --devices 0-7 / 0,2,5: several GPUs driven by this process (empty = {device})
   int index_shards = 1;           // --indexShards N: the index cut by contig into N images, shard i on devices[i % D]

@@ -50,8 +50,10 @@ struct mm_ctx {
   /* batch */
   mm_devbuf<uint8_t> d_bases; uint64_t n_bases = 0;
   mm_devbuf<uint8_t> d_packed; /* nibbles */
-  mm_built_index built{}; /* lookup arrays of an index built on the device, kept for mm_index_download (keep_lookup) */
+  mm_built_index built{}; /* lookup arrays of an index built on the device, kept for mm_index_download (MM_KEEP_LOOKUP) */
   bool built_kept = false;
+  /* its records before the frequent-seed drop, kept for mm_index_download_unfiltered (MM_KEEP_UNFILTERED) */
+  mm_rec_cols unf; uint64_t unf_n = 0; bool unf_kept = false;
   bool batch_is_ascii = false; /* the resident batch came in as text: K0 (pack) runs in front of K1 */
   float pack_ms = 0;
   mm_devbuf<mm_segment> d_segs; uint64_t n_segs = 0;
@@ -180,11 +182,14 @@ int write_tables(mm_ctx *c)
   return MM_OK;
 }
 
-/* the context has no index afterwards: its own image is freed, a shared one is no longer read */
+/* the context has no index afterwards: its own image is freed, a shared one is no longer read, and what a build kept
+ * for the download calls (MM_KEEP_*) goes with it */
 void drop_index(mm_ctx *c)
 {
   c->own_blob.reset();
   c->blob = nullptr; c->blob_bytes = 0; c->blob_ready = false; c->share_src = nullptr;
+  c->built = mm_built_index{}; c->built_kept = false;
+  c->unf.reset(); c->unf_n = 0; c->unf_kept = false;
 }
 
 /* an index upload or build that returns before its image is complete leaves the context with no index */
@@ -193,13 +198,11 @@ struct image_guard {
   ~image_guard() { if (!c->blob_ready) drop_index(c); }
 };
 
-/* a device build replaces the context's index: the old image and kept lookup arrays go first, and the returned guard
- * leaves the context with no index if the build does not complete */
+/* a device build replaces the context's index: the old image and kept arrays go first, and the returned guard leaves
+ * the context with no index if the build does not complete */
 image_guard start_build(mm_ctx *c)
 {
   drop_index(c);
-  c->built = mm_built_index{};
-  c->built_kept = false;
   return image_guard{c};
 }
 
@@ -1184,7 +1187,7 @@ int mm_host_free(void *ptr) { return cudaFreeHost(ptr) == cudaSuccess ? MM_OK : 
 namespace {
 /* the device builder over contigs [0, n_contigs) of contig_offsets (text at seqs, host or device) */
 int run_builder(mm_ctx *c, const char *seqs, int seqs_on_device, const uint64_t *contig_offsets, int32_t n_contigs,
-                const mm_freq_rule &rule, mm_built_index &B)
+                const mm_freq_rule &rule, int keep, mm_built_index &B)
 {
   const uint64_t total = contig_offsets[n_contigs];
   mm_devbuf<uint8_t> staged;
@@ -1194,7 +1197,7 @@ int run_builder(mm_ctx *c, const char *seqs, int seqs_on_device, const uint64_t 
   }
   std::string err;
   int rc = mm_build_index_device(c->params, seqs_on_device ? (const uint8_t *)seqs : staged.get(), contig_offsets, n_contigs, rule,
-                                 c->stream, c->sm_count, &B, err);
+                                 (keep & MM_KEEP_UNFILTERED) != 0, c->stream, c->sm_count, &B, err);
   if (rc != MM_OK) return fail(c, rc, "index build: %s", err.c_str());
   c->launches += 12;
   return MM_OK;
@@ -1212,9 +1215,9 @@ void fill_stats(mm_index_stats *stats, const mm_built_index &B, std::chrono::ste
   stats->ms_total = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
 }
 
-/* the image of what run_builder left in B (contig tables of n_contigs entries) */
+/* the image of what the builder left in B (contig tables of n_contigs entries); keep: MM_KEEP_* */
 int image_from_build(mm_ctx *c, mm_built_index &B, int32_t n_contigs, const int32_t *clen, const int32_t *contig_name_id,
-                     const int32_t *contig_group, int keep_lookup, mm_index_stats *stats, std::chrono::steady_clock::time_point t0)
+                     const int32_t *contig_group, int keep, mm_index_stats *stats, std::chrono::steady_clock::time_point t0)
 {
   int rc = MM_OK;
 
@@ -1249,14 +1252,15 @@ int image_from_build(mm_ctx *c, mm_built_index &B, int32_t n_contigs, const int3
   rc = finish_image(c, cstart, B.keys.get(), B.offs.get(), B.is_freq.get(), d_err.get(), clen, contig_name_id, contig_group);
   if (!c->blob_ready) return rc; /* else rc is write_tables': the index stands either way */
   fill_stats(stats, B, t0);
-  if (keep_lookup) { c->built = std::move(B); c->built_kept = true; }
+  if (keep & MM_KEEP_UNFILTERED) { c->unf = std::move(B.mi_unfiltered); c->unf_n = B.n_minmers_before_filter; c->unf_kept = true; }
+  if (keep & MM_KEEP_LOOKUP) { c->built = std::move(B); c->built_kept = true; }
   return rc;
 }
 } // namespace
 
 /* skch::Sketch's build + index + computeFreqHist + dropFreqSeedSet on the device (mm_index_build.cu) */
 int mm_index_build(mm_ctx *c, const char *seqs, int seqs_on_device, const uint64_t *contig_offsets, int32_t n_contigs,
-                   const int32_t *contig_name_id, const int32_t *contig_group, float kmer_pct_threshold, int keep_lookup,
+                   const int32_t *contig_name_id, const int32_t *contig_group, float kmer_pct_threshold, int keep,
                    mm_index_stats *stats)
 {
   if (!c) return MM_EINVAL;
@@ -1265,11 +1269,11 @@ int mm_index_build(mm_ctx *c, const char *seqs, int seqs_on_device, const uint64
   const auto t0 = std::chrono::steady_clock::now();
   const image_guard guard = start_build(c);
   mm_built_index B;
-  int rc = run_builder(c, seqs, seqs_on_device, contig_offsets, n_contigs, mm_freq_rule::own_threshold(kmer_pct_threshold), B);
+  int rc = run_builder(c, seqs, seqs_on_device, contig_offsets, n_contigs, mm_freq_rule::own_threshold(kmer_pct_threshold), keep, B);
   if (rc) return rc;
   std::vector<int32_t> clen((size_t)n_contigs);
   for (int32_t q = 0; q < n_contigs; q++) clen[(size_t)q] = (int32_t)(contig_offsets[q + 1] - contig_offsets[q]);
-  return image_from_build(c, B, n_contigs, clen.data(), contig_name_id, contig_group, keep_lookup, stats, t0);
+  return image_from_build(c, B, n_contigs, clen.data(), contig_name_id, contig_group, keep, stats, t0);
 }
 
 int mm_index_key_counts(mm_ctx *c, const char *seqs, int seqs_on_device, const uint64_t *contig_offsets, int32_t n_contigs,
@@ -1282,7 +1286,7 @@ int mm_index_key_counts(mm_ctx *c, const char *seqs, int seqs_on_device, const u
     c->kc_keys.reset(); c->kc_counts.reset(); c->kc_n = 0; c->kc_ready = false;
     const auto t0 = std::chrono::steady_clock::now();
     mm_built_index B;
-    int rc = run_builder(c, seqs, seqs_on_device, contig_offsets, n_contigs, mm_freq_rule::count_only(), B);
+    int rc = run_builder(c, seqs, seqs_on_device, contig_offsets, n_contigs, mm_freq_rule::count_only(), 0, B);
     if (rc) return rc;
     c->kc_keys = std::move(B.keys); c->kc_counts = std::move(B.counts); c->kc_n = B.n_keys; c->kc_ready = true;
     fill_stats(stats, B, t0);
@@ -1304,7 +1308,7 @@ int mm_index_key_counts(mm_ctx *c, const char *seqs, int seqs_on_device, const u
 int mm_index_build_shard(mm_ctx *c, const char *seqs, int seqs_on_device, const uint64_t *contig_offsets, int32_t first_contig,
                          int32_t n_shard_contigs, const int32_t *contig_len, const int32_t *contig_name_id,
                          const int32_t *contig_group, int32_t n_contigs, const uint64_t *freq_hashes, uint64_t n_freq,
-                         int keep_lookup, mm_index_stats *stats)
+                         int keep, mm_index_stats *stats)
 {
   if (!c) return MM_EINVAL;
   if (n_shard_contigs < 1 || !contig_offsets || !seqs || !contig_len) return fail(c, MM_EINVAL, "no contigs");
@@ -1323,17 +1327,37 @@ int mm_index_build_shard(mm_ctx *c, const char *seqs, int seqs_on_device, const 
   CU(c, d_freq.reserve(n_freq + 1));
   if (n_freq) CU(c, cudaMemcpyAsync(d_freq.get(), freq_hashes, n_freq * 8, cudaMemcpyHostToDevice, c->stream));
   mm_built_index B;
-  int rc = run_builder(c, seqs, seqs_on_device, off.data(), n_contigs, mm_freq_rule::listed(d_freq.get(), n_freq), B);
+  int rc = run_builder(c, seqs, seqs_on_device, off.data(), n_contigs, mm_freq_rule::listed(d_freq.get(), n_freq), keep, B);
   d_freq.reset();
   if (rc) return rc;
-  return image_from_build(c, B, n_contigs, contig_len, contig_name_id, contig_group, keep_lookup, stats, t0);
+  return image_from_build(c, B, n_contigs, contig_len, contig_name_id, contig_group, keep, stats, t0);
 }
 
-/* host copies of what mm_index_build left on the device (needs keep_lookup); any output may be NULL */
+/* Sketch::index + computeFreqHist + dropFreqSeedSet over a loaded minmer list, on the device (mm_index_build.cu) */
+int mm_index_build_minmers(mm_ctx *c, const mm_minmer *mi, uint64_t n, int mi_on_device, const int32_t *contig_len,
+                           const int32_t *contig_name_id, const int32_t *contig_group, int32_t n_contigs, float kmer_pct_threshold,
+                           int keep, mm_index_stats *stats)
+{
+  if (!c) return MM_EINVAL;
+  if (n_contigs < 1 || !contig_len) return fail(c, MM_EINVAL, "no contigs");
+  if (n && !mi) return fail(c, MM_EINVAL, "null minmer list");
+  CU(c, cudaSetDevice(c->device));
+  const auto t0 = std::chrono::steady_clock::now();
+  const image_guard guard = start_build(c);
+  mm_built_index B;
+  std::string err;
+  const int rc = mm_build_index_from_records(mi, mi_on_device, n, n_contigs, kmer_pct_threshold, (keep & MM_KEEP_UNFILTERED) != 0,
+                                             c->stream, &B, err);
+  if (rc != MM_OK) return fail(c, rc, "index build: %s", err.c_str());
+  c->launches += 8;
+  return image_from_build(c, B, n_contigs, contig_len, contig_name_id, contig_group, keep, stats, t0);
+}
+
+/* host copies of what mm_index_build left on the device (needs MM_KEEP_LOOKUP); any output may be NULL */
 int mm_index_download(mm_ctx *c, mm_minmer *mi, uint64_t *keys, uint64_t *offsets, mm_ipoint *points, uint8_t *is_freq)
 {
   if (!c || !c->blob_ready) return fail(c, MM_ESTATE, "no index");
-  if ((keys || offsets || points || is_freq) && !c->built_kept) return fail(c, MM_ESTATE, "the lookup arrays were not kept (keep_lookup)");
+  if ((keys || offsets || points || is_freq) && !c->built_kept) return fail(c, MM_ESTATE, "the lookup arrays were not kept (MM_KEEP_LOOKUP)");
   CU(c, cudaSetDevice(c->device));
   const mm_blob_header &h = c->hdr;
   if (mi && h.n_minmers) {
@@ -1364,6 +1388,39 @@ int mm_index_download(mm_ctx *c, mm_minmer *mi, uint64_t *keys, uint64_t *offset
     CU(c, cudaMemcpyAsync(points, d.get(), B.n_points * sizeof(mm_ipoint), cudaMemcpyDeviceToHost, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
   }
+  return MM_OK;
+}
+
+/* the kept records before the frequent-seed drop, packed to mm_minmer on the device a slice at a time (a slice of 2^24
+ * records is 384 MB: the whole list at once would take 24 bytes per record of device memory more), then freed */
+int mm_index_download_unfiltered(mm_ctx *c, mm_minmer *out, uint64_t cap, uint64_t *n)
+{
+  if (!c || !n) return MM_EINVAL;
+  if (!c->unf_kept) return fail(c, MM_ESTATE, "no records before the frequent-seed drop were kept (MM_KEEP_UNFILTERED)");
+  *n = c->unf_n;
+  if (cap < c->unf_n) return fail(c, MM_ECAPACITY, "need room for %llu records", (unsigned long long)c->unf_n);
+  if (c->unf_n && !out) return fail(c, MM_EINVAL, "null output");
+  CU(c, cudaSetDevice(c->device));
+  const uint64_t CH = 1ULL << 24;
+  mm_devbuf<mm_minmer> packed;
+  if (c->unf_n) CU(c, packed.reserve(std::min(CH, c->unf_n)));
+  for (uint64_t at = 0; at < c->unf_n; at += CH) {
+    const uint64_t k = std::min(CH, c->unf_n - at);
+    CU(c, mm_pack_minmers(c->unf, at, k, packed.get(), c->stream));
+    CU(c, cudaMemcpyAsync(out + at, packed.get(), k * sizeof(mm_minmer), cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+    c->launches++;
+  }
+  c->unf.reset(); c->unf_n = 0; c->unf_kept = false;
+  return MM_OK;
+}
+
+int mm_index_release_kept(mm_ctx *c)
+{
+  if (!c) return MM_EINVAL;
+  CU(c, cudaSetDevice(c->device));
+  c->built = mm_built_index{}; c->built_kept = false;
+  c->unf.reset(); c->unf_n = 0; c->unf_kept = false;
   return MM_OK;
 }
 

@@ -954,6 +954,39 @@ __global__ void k_split_minmers(const mm_minmer *aos, uint64_t n, uint64_t *hash
   const mm_minmer m = aos[i];
   hash[i] = m.hash; wpos[i] = m.wpos; wend[i] = m.wpos_end; strand[i] = (int8_t)m.strand;
 }
+/* A loaded minmer list -> the builder's five record columns, each record checked against the one before it for what
+ * mm_index_upload refuses: reason 1 a seqId outside [0, n_contigs), 2 out of (seqId, wpos) order, 4 a negative position.
+ * The first bad record wins: *first_bad = min over them of (index << 8 | reasons). Kept apart from k_split_minmers, which
+ * writes the index image (it has no seqId column) from records mm_index_upload has already checked on the host: one
+ * kernel for both would change the upload path's code. */
+__global__ void k_split_check(const mm_minmer *__restrict__ aos, uint64_t n, int32_t n_contigs, mm_rec_view o,
+                              unsigned long long *first_bad)
+{
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const mm_minmer m = aos[i];
+  o.hash[i] = m.hash; o.wpos[i] = m.wpos; o.wend[i] = m.wpos_end; o.seq[i] = m.seqId; o.strand[i] = (int8_t)m.strand;
+  uint32_t why = 0;
+  if (m.seqId < 0 || m.seqId >= n_contigs) why |= 1u;
+  if (i > 0) {
+    const int32_t ps = aos[i - 1].seqId, pw = aos[i - 1].wpos;
+    if (m.seqId < ps || (m.seqId == ps && m.wpos < pw)) why |= 2u;
+  }
+  if (m.wpos < 0 || m.wpos_end < 0) why |= 4u;
+  if (why) atomicMin(first_bad, ((unsigned long long)i << 8) | why);
+}
+/* the five record columns -> mm_minmer records (_pad = 0), records [first, first + n) */
+__global__ void k_pack_minmers(mm_rec_view in, uint64_t first, uint64_t n, mm_minmer *out)
+{
+  const uint64_t *__restrict__ i_hash = in.hash; const int32_t *__restrict__ i_wpos = in.wpos, *__restrict__ i_wend = in.wend;
+  const int32_t *__restrict__ i_seq = in.seq; const int8_t *__restrict__ i_strand = in.strand;
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint64_t j = first + i;
+  mm_minmer m;
+  m.hash = i_hash[j]; m.wpos = i_wpos[j]; m.wpos_end = i_wend[j]; m.seqId = i_seq[j]; m.strand = i_strand[j]; m._pad = 0;
+  out[i] = m;
+}
 __global__ void k_pack_points(const mm_ipoint *aos, uint64_t n, int32_t n_contigs, uint64_t *packed, uint32_t *err)
 {
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1017,7 +1050,8 @@ __global__ void k_unpack_points(uint64_t n, const uint64_t *__restrict__ pts, co
 } // namespace
 
 int mm_build_index_device(const mm_params &p, const uint8_t *d_seq, const uint64_t *h_contig_off, int32_t n_contigs,
-                          const mm_freq_rule &rule, cudaStream_t st, int sm_count, mm_built_index *out, std::string &err)
+                          const mm_freq_rule &rule, bool keep_unfiltered, cudaStream_t st, int sm_count, mm_built_index *out,
+                          std::string &err)
 {
   *out = mm_built_index{};
   if (!mm_sketch_kmer_supported(p.kmer_size)) { err = "k-mer size not compiled in"; return MM_EINVAL; }
@@ -1047,6 +1081,7 @@ int mm_build_index_device(const mm_params &p, const uint8_t *d_seq, const uint64
       }
       if ((rc = frequency_filter(rule, m, n_mi, perm, rec_key, st, out, err)) != MM_OK) return rc;
     }
+    if (keep_unfiltered) out->mi_unfiltered = std::move(m);
   }
   if (rule.mode == mm_freq_rule::LISTED && rule.n_freq && (rc = append_absent(rule, st, out, err)) != MM_OK) return rc;
   cudaEventRecord(ev.e[3], st);
@@ -1055,6 +1090,72 @@ int mm_build_index_device(const mm_params &p, const uint8_t *d_seq, const uint64
   cudaEventElapsedTime(&out->ms_post, ev.e[1], ev.e[2]);
   cudaEventElapsedTime(&out->ms_lookup, ev.e[2], ev.e[3]);
   return MM_OK;
+}
+
+int mm_build_index_from_records(const mm_minmer *aos, int aos_on_device, uint64_t n, int32_t n_contigs, float kmer_pct_threshold,
+                                bool keep_unfiltered, cudaStream_t st, mm_built_index *out, std::string &err)
+{
+  *out = mm_built_index{};
+  if (n >= (1ULL << 32)) { err = "more than 2^32 minmer records"; return MM_EINVAL; }
+  stage_events ev;
+  CE(ev.create());
+  cudaEventRecord(ev.e[0], st);
+  mm_rec_cols m; /* the records, before the frequent-seed drop */
+  if (n) {
+    mm_devbuf<mm_minmer> staged; /* freed before the lookup, whose temporaries are larger */
+    if (!aos_on_device) {
+      CE(staged.reserve(n));
+      CE(cudaMemcpyAsync(staged.get(), aos, n * sizeof(mm_minmer), cudaMemcpyHostToDevice, st));
+    }
+    const mm_minmer *d_aos = aos_on_device ? aos : staged.get();
+    mm_devbuf<unsigned long long> d_bad;
+    CE(d_bad.reserve(1));
+    CE(cudaMemsetAsync(d_bad.get(), 0xff, 8, st));
+    CE(m.reserve(n));
+    k_split_check<<<blocks(n), 256, 0, st>>>(d_aos, n, n_contigs, m.view(), d_bad.get());
+    CE(cudaGetLastError());
+    unsigned long long bad = 0;
+    CE(cudaMemcpyAsync(&bad, d_bad.get(), 8, cudaMemcpyDeviceToHost, st));
+    CE(cudaStreamSynchronize(st));
+    if (bad != ~0ULL) { /* refused before any kernel indexes anything by seqId */
+      const unsigned long long i = bad >> 8;
+      mm_minmer r;
+      CE(cudaMemcpyAsync(&r, d_aos + i, sizeof r, cudaMemcpyDeviceToHost, st));
+      CE(cudaStreamSynchronize(st));
+      char buf[256];
+      if (bad & 1u)
+        snprintf(buf, sizeof buf, "record %llu: seqId %d is not a contig of this reference (%d contigs)", i, r.seqId, n_contigs);
+      else if (bad & 4u)
+        snprintf(buf, sizeof buf, "record %llu: negative position (wpos %d, wpos_end %d)", i, r.wpos, r.wpos_end);
+      else
+        snprintf(buf, sizeof buf, "record %llu (seqId %d, wpos %d) is out of (seqId, wpos) order", i, r.seqId, r.wpos);
+      err = buf;
+      return MM_EINVAL;
+    }
+  }
+  out->n_minmers_before_filter = n;
+  cudaEventRecord(ev.e[1], st); /* no window scan */
+  cudaEventRecord(ev.e[2], st); /* and no record post-processing */
+  if (n) {
+    int rc;
+    mm_devbuf<uint32_t> perm; mm_devbuf<uint64_t> rec_key;
+    if ((rc = index_lookup(m, n, st, perm, rec_key, out, err)) != MM_OK) return rc;
+    if ((rc = frequency_filter(mm_freq_rule::own_threshold(kmer_pct_threshold), m, n, perm, rec_key, st, out, err)) != MM_OK) return rc;
+  }
+  if (keep_unfiltered) out->mi_unfiltered = std::move(m);
+  cudaEventRecord(ev.e[3], st);
+  CE(cudaStreamSynchronize(st));
+  cudaEventElapsedTime(&out->ms_scan, ev.e[0], ev.e[1]);
+  cudaEventElapsedTime(&out->ms_post, ev.e[1], ev.e[2]);
+  cudaEventElapsedTime(&out->ms_lookup, ev.e[2], ev.e[3]);
+  return MM_OK;
+}
+
+cudaError_t mm_pack_minmers(const mm_rec_cols &in, uint64_t first, uint64_t n, mm_minmer *out, cudaStream_t st)
+{
+  if (n == 0) return cudaSuccess;
+  k_pack_minmers<<<blocks(n), 256, 0, st>>>(in.view(), first, n, out);
+  return cudaGetLastError();
 }
 
 cudaError_t mm_upload_split_minmers(const mm_minmer *aos, uint64_t n, uint64_t *hash, int32_t *wpos, int32_t *wend, int8_t *strand,

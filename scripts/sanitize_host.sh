@@ -9,7 +9,7 @@ mkdir -p "$OUT"
 for san in thread address,undefined; do
   bin=$OUT/t_$(echo $san | tr ',' '_')
   g++ -std=c++17 -O1 -g -fsanitize=$san -fno-sanitize-recover=all -fno-omit-frame-pointer -pthread -w "$ROOT/tests/tools/sanitize_main.cpp" \
-      $H/skch_stats.cpp $H/skch_seqio.cpp $H/skch_index.cpp $H/skch_tail.cpp $H/skch_map.cpp $H/skch_args.cpp $H/skch_cview.cpp \
+      $H/skch_stats.cpp $H/skch_seqio.cpp $H/skch_index.cpp $H/skch_tail.cpp $H/skch_map.cpp $H/skch_args.cpp $H/skch_cview.cpp $H/skch_align.cpp \
       -I"$ROOT/include" -L"$ROOT/mashmap_b200" -lmashmap_nccl -lmashmap_b200 -lz -Wl,-rpath,"$ROOT/mashmap_b200" -o "$bin"
   echo "== -fsanitize=$san"
   TSAN_OPTIONS=halt_on_error=1 ASAN_OPTIONS=detect_leaks=0 "$bin"
