@@ -71,10 +71,41 @@ int mm_align_batch(mm_align_ctx *ctx, const char *qbases, uint64_t n_qbases, con
                    const mm_align_job *jobs, uint64_t n_jobs, mm_align_result *results, uint8_t *ops,
                    uint64_t ops_cap, uint64_t *n_ops);
 
-/* CUDA-event time in milliseconds of each stage of the last mm_align_batch:
+/* CUDA-event time in milliseconds of each stage of the last mm_align_batch or mm_align_batch_tags:
  * [0] H2D  [1] distance and end (HW and NW passes)  [2] start (reverse SHW pass)  [3] Hirschberg levels  [4] leaf NW + traceback
  * [5] D2H  [6] whole call on the host clock  [7] number of Hirschberg levels. */
 int mm_align_last_stage_ms(const mm_align_ctx *ctx, float ms[8]);
+
+/* Flags of mm_align_batch_tags. 0: cg is edlibAlignmentToCigar(EDLIB_CIGAR_STANDARD), runs of M, I, D.
+ * MM_ALIGN_TAG_EQX: cg is edlibAlignmentToCigar(EDLIB_CIGAR_EXTENDED), runs of = (op 0), X (3), I (1), D (2).
+ * MM_ALIGN_TAG_CS: also minimap2's short cs: ":N" per match run, "*tq" per mismatch (target byte, then query byte),
+ * "+bases" / "-bases" per insertion / deletion run; bases are the job's bytes with A-Z lowered to a-z. */
+#define MM_ALIGN_TAG_EQX (1u << 0)
+#define MM_ALIGN_TAG_CS (1u << 1)
+
+/* One job of mm_align_batch_tags: ed and alignment_length as in mm_align_result; the cg body (no "cg:Z:") at
+ * text[cg_offset, cg_offset + cg_len) and, with MM_ALIGN_TAG_CS, the cs body at text[cs_offset, cs_offset + cs_len).
+ * Lengths are 0 for a job with no path (ed < 0 or alignment_length 0). 40 bytes. */
+typedef struct mm_align_tag_result {
+  int32_t ed;
+  int32_t alignment_length;
+  uint64_t cg_offset;
+  uint64_t cg_len;
+  uint64_t cs_offset;
+  uint64_t cs_len;
+} mm_align_tag_result;
+
+/* The alignment of mm_align_batch (same distance, same path) for MM_ALIGN_NW jobs only (any other mode is MM_EINVAL),
+ * returned as tag text written on the device instead of edit ops. flags: 0 or MM_ALIGN_TAG_EQX, optionally with
+ * MM_ALIGN_TAG_CS (other bits are MM_EINVAL). text[text_cap]; on MM_ECAPACITY *n_text holds the text size needed and
+ * nothing else is valid. */
+int mm_align_batch_tags(mm_align_ctx *ctx, const char *qbases, uint64_t n_qbases, const char *tbases, uint64_t n_tbases,
+                        const mm_align_job *jobs, uint64_t n_jobs, uint32_t flags, mm_align_tag_result *results,
+                        char *text, uint64_t text_cap, uint64_t *n_text);
+
+/* CUDA-event time in milliseconds of the formatting kernels of the last mm_align_batch_tags (path compaction, runs,
+ * text); its text D2H counts in stage [5] of mm_align_last_stage_ms. */
+int mm_align_last_tag_ms(const mm_align_ctx *ctx, float *ms);
 
 #ifdef __cplusplus
 }

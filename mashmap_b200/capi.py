@@ -614,10 +614,13 @@ MM_ALIGN_HW, MM_ALIGN_NW = 0, 1  # align_job_dtype["mode"]: edlib's EDLIB_MODE_H
 MM_ALIGN_BAND_MIN_LEN = 32 * 1024  # NW sub-problems with max(q_len, t_len) >= this run banded, one CTA per sweep
 align_result_dtype = np.dtype([("ed", "<i4"), ("start", "<i4"), ("end", "<i4"), ("alignment_length", "<i4"),
                                ("ops_offset", "<u8")])
-assert align_job_dtype.itemsize == 32 and align_result_dtype.itemsize == 24
+align_tag_result_dtype = np.dtype([("ed", "<i4"), ("alignment_length", "<i4"), ("cg_offset", "<u8"), ("cg_len", "<u8"),
+                                   ("cs_offset", "<u8"), ("cs_len", "<u8")])
+MM_ALIGN_TAG_EQX, MM_ALIGN_TAG_CS = 1, 2  # flags of mm_align_batch_tags: extended CIGAR (= / X), minimap2's short cs
+assert align_job_dtype.itemsize == 32 and align_result_dtype.itemsize == 24 and align_tag_result_dtype.itemsize == 40
 
 ALIGN_EXPORTED_SYMBOLS = ["mm_align_ctx_create", "mm_align_ctx_destroy", "mm_align_last_error", "mm_align_batch",
-                          "mm_align_last_stage_ms"]
+                          "mm_align_last_stage_ms", "mm_align_batch_tags", "mm_align_last_tag_ms"]
 
 
 def _align_lib():
@@ -630,6 +633,8 @@ def _align_lib():
         L.mm_align_last_error.restype = C.c_char_p
         L.mm_align_batch.argtypes = [vp, vp, u64, vp, u64, vp, u64, vp, vp, u64, C.POINTER(u64)]
         L.mm_align_last_stage_ms.argtypes = [vp, C.POINTER(C.c_float * 8)]
+        L.mm_align_batch_tags.argtypes = [vp, vp, u64, vp, u64, vp, u64, C.c_uint32, vp, vp, u64, C.POINTER(u64)]
+        L.mm_align_last_tag_ms.argtypes = [vp, C.POINTER(C.c_float)]
         L._align_bound = True
     return L
 
@@ -663,10 +668,38 @@ class AlignContext:
             raise err
         return res, ops[: n.value]
 
+    def align_tags(self, qbases, tbases, jobs, flags=0, text_cap=None):
+        """mm_align_batch_tags: jobs (MM_ALIGN_NW only) as for align(). Returns (results, text) with results an
+        align_tag_result_dtype array and text the bytes its cg / cs offsets point into. On MM_ECAPACITY the raised error
+        carries n_text, the size needed."""
+        L = _align_lib()
+        q = np.ascontiguousarray(qbases, dtype=np.uint8)
+        t = np.ascontiguousarray(tbases, dtype=np.uint8)
+        jobs = np.ascontiguousarray(jobs, dtype=align_job_dtype)
+        res = np.zeros(len(jobs), dtype=align_tag_result_dtype)
+        if text_cap is None:  # a run of L ops takes at most 2L bytes of cg and 3L of cs; a path is at most Q + T ops
+            ops = int(jobs["q_len"].astype(np.int64).sum() + jobs["t_len"].astype(np.int64).sum())
+            text_cap = ops * (5 if flags & MM_ALIGN_TAG_CS else 2)
+        text = np.zeros(max(int(text_cap), 1), dtype=np.uint8)
+        n = C.c_uint64()
+        rc = L.mm_align_batch_tags(self._ctx, _ptr(q), len(q), _ptr(t), len(t), _ptr(jobs), len(jobs), int(flags),
+                                   _ptr(res), _ptr(text), int(text_cap), C.byref(n))
+        if rc != MM_OK:
+            err = MashmapError(rc, L.mm_align_last_error(self._ctx).decode())
+            err.n_text = n.value
+            raise err
+        return res, text[: n.value].tobytes()
+
     def stage_ms(self):
         a = (C.c_float * 8)()
         _align_lib().mm_align_last_stage_ms(self._ctx, C.byref(a))
         return list(a)
+
+    def tag_ms(self):
+        """the formatting kernels' time of the last align_tags, in ms"""
+        a = C.c_float()
+        _align_lib().mm_align_last_tag_ms(self._ctx, C.byref(a))
+        return a.value
 
     def close(self):
         if self._ctx:

@@ -22,18 +22,7 @@ const char kBase[4] = {'A', 'C', 'T', 'G'};
 inline char base(uint8_t x) { return (x & 8) ? 'N' : kBase[x & 3]; }
 inline char complement(uint8_t x) { return (x & 8) ? 'N' : kBase[(x & 3) ^ 2]; }  // A <-> T (0, 2), C <-> G (1, 3)
 
-/* edlibAlignmentToCigar(EDLIB_CIGAR_STANDARD): runs of match / mismatch as M, insertion I, deletion D */
-void putCigar(std::string &out, const uint8_t *ops, int n)
-{
-  static const char ch[4] = {'M', 'I', 'D', 'M'};
-  for (int i = 0; i < n;) {
-    int j = i + 1;
-    while (j < n && ch[ops[j]] == ch[ops[i]]) j++;
-    out += std::to_string(j - i);
-    out += ch[ops[i]];
-    i = j;
-  }
-}
+inline char lower(char b) { return (char)(b | 0x20); }  // A C G T N -> a c g t n
 
 }  // namespace
 
@@ -48,54 +37,70 @@ MappingAligner::~MappingAligner() { mm_align_ctx_destroy(ctx); }
 void MappingAligner::align(const Item *items, size_t n, std::vector<std::string> &tags)
 {
   const auto t0 = std::chrono::steady_clock::now();
+  const uint32_t flags = (param.align_eqx ? MM_ALIGN_TAG_EQX : 0) | (param.align_cs ? MM_ALIGN_TAG_CS : 0);
   tags.assign(n, std::string());
   std::vector<char> qb, tb;
   std::vector<mm_align_job> jobs;
   std::vector<size_t> owner;  // item of each job
-  std::vector<mm_align_result> res;
-  std::vector<uint8_t> ops;
+  std::vector<mm_align_tag_result> res;
   auto flush = [&]() {
     if (jobs.empty()) return;
     res.resize(jobs.size());
-    ops.resize(qb.size() + tb.size());  // NW paths are at most Q + T ops
-    uint64_t n_ops = 0;
-    if (mm_align_batch(ctx, qb.data(), qb.size(), tb.data(), tb.size(), jobs.data(), jobs.size(), res.data(), ops.data(),
-                       ops.size(), &n_ops) != MM_OK)
-      die(std::string("mm_align_batch: ") + mm_align_last_error(ctx));
+    // a run of L ops takes at most 2L bytes of cg and 3L of cs, and NW paths are at most Q + T ops
+    const uint64_t need = (qb.size() + tb.size()) * (param.align_cs ? 5 : 2);
+    if (need > textCap) { text.reset(new char[need]); textCap = need; }
+    uint64_t n_text = 0;
+    if (mm_align_batch_tags(ctx, qb.data(), qb.size(), tb.data(), tb.size(), jobs.data(), jobs.size(), flags, res.data(),
+                            text.get(), textCap, &n_text) != MM_OK)
+      die(std::string("mm_align_batch_tags: ") + mm_align_last_error(ctx));
     for (size_t j = 0; j < jobs.size(); j++) {
-      const mm_align_result &r = res[j];
+      const mm_align_tag_result &r = res[j];
       // with k = -1 edlib always has a distance; it has no path only where its Hirschberg split meets a one-column
       // target, which takes a query of more than 3 Mbp (DESIGN.md section 10)
       if (r.ed < 0 || r.alignment_length == 0) { unaligned++; continue; }
       std::string &t = tags[owner[j]];
       t = "\tNM:i:" + std::to_string(r.ed) + "\tcg:Z:";
-      putCigar(t, ops.data() + r.ops_offset, r.alignment_length);
+      t.append(text.get() + r.cg_offset, r.cg_len);
+      if (param.align_cs) t.append("\tcs:Z:").append(text.get() + r.cs_offset, r.cs_len);
       aligned++;
     }
     bases += qb.size() + tb.size();
     qb.clear(); tb.clear(); jobs.clear(); owner.clear();
   };
+  // the query region, reverse-complemented for a '-' mapping, and the target region
+  auto query = [&](const MappingResult &m, const uint8_t *q, auto put) {
+    const int64_t qs = m.queryStartPos, qe = m.queryEndPos;
+    if (m.strand == strnd::FWD)
+      for (int64_t x = qs; x < qe; x++) put(base(nibble(q, (uint64_t)x)));
+    else
+      for (int64_t x = qe - 1; x >= qs; x--) put(complement(nibble(q, (uint64_t)x)));
+  };
+  auto target = [&](const MappingResult &m, auto put) {
+    const uint8_t *t = ref.refNibbles(m.refSeqId);
+    for (int64_t x = m.refStartPos; x < (int64_t)m.refEndPos; x++) put(base(nibble(t, (uint64_t)x)));
+  };
   for (size_t i = 0; i < n; i++) {
     const MappingResult &m = *items[i].m;
-    const int64_t qs = m.queryStartPos, ql = (int64_t)m.queryEndPos - qs;
-    const int64_t ts = m.refStartPos, tl = (int64_t)m.refEndPos - ts;
+    const int64_t ql = (int64_t)m.queryEndPos - m.queryStartPos, tl = (int64_t)m.refEndPos - m.refStartPos;
     if (ql > param.align_max_len || tl > param.align_max_len) { tooLong++; continue; }
     if (ql <= 0 || tl <= 0) {  // NW of an empty region: every base of the other one is inserted / deleted
       if (ql <= 0 && tl <= 0) { unaligned++; continue; }
-      tags[i] = "\tNM:i:" + std::to_string(ql > 0 ? ql : tl) + "\tcg:Z:" + std::to_string(ql > 0 ? ql : tl) + (ql > 0 ? "I" : "D");
+      std::string &t = tags[i];
+      t = "\tNM:i:" + std::to_string(ql > 0 ? ql : tl) + "\tcg:Z:" + std::to_string(ql > 0 ? ql : tl) + (ql > 0 ? "I" : "D");
+      if (param.align_cs) {
+        t += ql > 0 ? "\tcs:Z:+" : "\tcs:Z:-";
+        auto put = [&](char b) { t += lower(b); };
+        if (ql > 0) query(m, items[i].query, put);
+        else target(m, put);
+      }
       aligned++;
       continue;
     }
     if (!jobs.empty() && qb.size() + tb.size() + (uint64_t)(ql + tl) > BATCH_BASES) flush();
     jobs.push_back(mm_align_job{qb.size(), tb.size(), (int32_t)ql, (int32_t)tl, -1, MM_ALIGN_NW});
     owner.push_back(i);
-    const uint8_t *q = items[i].query;
-    if (m.strand == strnd::FWD)
-      for (int64_t x = qs; x < qs + ql; x++) qb.push_back(base(nibble(q, (uint64_t)x)));
-    else
-      for (int64_t x = qs + ql - 1; x >= qs; x--) qb.push_back(complement(nibble(q, (uint64_t)x)));
-    const uint8_t *t = ref.refNibbles(m.refSeqId);
-    for (int64_t x = ts; x < ts + tl; x++) tb.push_back(base(nibble(t, (uint64_t)x)));
+    query(m, items[i].query, [&](char b) { qb.push_back(b); });
+    target(m, [&](char b) { tb.push_back(b); });
   }
   flush();
   seconds += std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();

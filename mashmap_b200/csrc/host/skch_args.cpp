@@ -33,7 +33,8 @@ const OptDef kOptions[] = {
     {"reportPercentage", nullptr, false},
     // B200-specific
     {"device", nullptr, true}, {"devices", nullptr, true}, {"hostIndex", nullptr, false}, {"batchBases", nullptr, true}, {"subBatchBases", nullptr, true},
-    {"align", nullptr, false}, {"alignMaxLen", nullptr, true}, {"indexShards", nullptr, true},
+    {"align", nullptr, false}, {"alignMaxLen", nullptr, true}, {"eqx", nullptr, false}, {"cs", nullptr, false},
+    {"indexShards", nullptr, true},
 };
 
 [[noreturn]] void usage_error(const std::string &msg)
@@ -115,6 +116,8 @@ void parseandSave(int argc, char **argv, Parameters &parameters)
   if (found("help")) {
     std::cerr << "mashmap-b200 -r ref.fa -q seq.fq [OPTIONS]   (options as in MashMap v3.1.3, plus --device N | --devices 0-7, --batchBases N,\n"
                  "    --align [--alignMaxLen N, default 100000]: append NM:i and cg:Z (edlib NW over each mapping's region, on the GPU),\n"
+                 "    --eqx (with --align): cg:Z with =/X for matches and mismatches instead of M, --cs (with --align): also append\n"
+                 "    minimap2's short cs:Z difference string (relative to the target's forward strand, bases in lower case),\n"
                  "    --indexShards N [default 1]: cut the reference index by contig into N device images (shard i on the i-th device of\n"
                  "    --devices, round robin), for references whose index does not fit one GPU; the output is the same)" << std::endl;
     exit(0);
@@ -129,6 +132,10 @@ void parseandSave(int argc, char **argv, Parameters &parameters)
       usage_error("ERROR, --alignMaxLen needs a positive whole number of bases, not '" + v + "'");
     parameters.align_max_len = std::stoll(v);
   }
+  for (const char *o : {"eqx", "cs"})
+    if (found(o) && !parameters.align) usage_error(std::string("ERROR, --") + o + " is given without --align");
+  parameters.align_eqx = found("eqx");
+  parameters.align_cs = found("cs");
   if (!found("ref") && !found("refList")) usage_error("ERROR, skch::parseandSave, Provide reference file(s)");
 
   if (found("ref")) parameters.refSequences.push_back(opt["ref"]);

@@ -117,6 +117,8 @@ struct Parameters {
   // --alignMaxLen: longer query or target regions are printed without the tags. One warp aligns one mapping without a band:
   // 100 kb x 100 kb takes 1.9 s, 1 Mbp x 1 Mbp 341 s (H100 80GB HBM3, 400 W; scripts/map_align_perf.py)
   int64_t align_max_len = 100000;
+  bool align_eqx = false;         // --eqx: cg:Z as an extended CIGAR (= / X / I / D)
+  bool align_cs = false;          // --cs: also cs:Z, minimap2's short difference string
 };
 
 namespace fixed {  // map_parameters.hpp:86-102

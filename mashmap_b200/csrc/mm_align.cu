@@ -32,14 +32,21 @@
  * band:
  *   k_band_nw       (a) rule 1' for one pass of a k schedule the host drives
  *   k_band_col      (c) one half-column of a Hirschberg node (two CTAs per node), then k_band_split for the split row
+ *
+ * mm_align_batch_tags formats the paths on the device instead of returning them (DESIGN.md section 10, "Tag text on
+ * the device"), flat over the ops of a wave of jobs: k_tag_gather (compact the leaves), k_tag_mark + cub select (run
+ * starts), k_tag_runs + cub scans (run text lengths, offsets and base positions), k_tag_jobs (job text offsets),
+ * k_tag_write (one thread per output byte).
  */
 #include <cstdlib>
+#include <cub/cub.cuh>
 #include <cuda_runtime.h>
 
 #include <algorithm>
 #include <chrono>
 #include <climits>
 #include <cstring>
+#include <functional>
 #include <string>
 #include <vector>
 
@@ -552,7 +559,168 @@ __global__ void k_band_split(const Prob *probs, int n, int nsym, uint8_t *scratc
   if (lane == 0) out[p.res] = r;
 }
 
+/* ---- tag text (mm_align_batch_tags), flat over the ops of a wave of jobs --------------------------------------------
+ * The wave's paths lie end to end in one op array (path[x]: the op in bits 0-1, bit 7 on a job's first op). A run is a
+ * maximal stretch of one letter inside one job; its text is written by threads balanced over output bytes. */
+enum { TAG_CG = 0, TAG_CG_EQX = 1, TAG_CS = 2 };
+constexpr uint8_t TAG_FIRST = 0x80;
+
+struct TagLeaf {
+  uint64_t src;   // a traced leaf: its ops at ops + src
+  uint32_t dst;   // its first op in the wave's paths
+  int16_t fill;   // -1: traced; 1 / 2: a leaf with an empty side, all insertions / all deletions
+  int16_t first;  // the first leaf of its job
+};
+
+struct TagJob {
+  uint64_t q, t;   // the job's q_offset / t_offset
+  uint32_t op0;    // its first op in the wave's paths
+  uint32_t q0, t0; // query / target bases the wave's earlier paths consume
+};
+
+/* the letter class of an op: the standard CIGAR folds mismatches into matches */
+__device__ __forceinline__ int tag_key(uint8_t p, int kind)
+{
+  const int op = p & 3;
+  return kind == TAG_CG && op == 3 ? 0 : op;
+}
+
+__device__ __forceinline__ int tag_digits(uint64_t v)
+{
+  int d = 1;
+  while (v >= 10) { v /= 10; d++; }
+  return d;
+}
+
+/* digit k (most significant first) of the nd decimal digits of v */
+__device__ __forceinline__ char tag_digit(uint64_t v, int nd, int k)
+{
+  for (int i = nd - 1 - k; i > 0; i--) v /= 10;
+  return (char)('0' + v % 10);
+}
+
+__device__ __forceinline__ char tag_lower(uint8_t b) { return (char)(b >= 'A' && b <= 'Z' ? b + 32 : b); }
+
+/* last index i in [0, n) with a[i] <= x (a ascending, a[0] <= x) */
+template <class T>
+__device__ __forceinline__ uint32_t tag_find(const T *a, uint32_t n, uint64_t x)
+{
+  uint32_t lo = 0, hi = n - 1;
+  while (lo < hi) {
+    const uint32_t mid = lo + ((hi - lo + 1) >> 1);
+    if ((uint64_t)a[mid] <= x) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+
+/* (1) the wave's leaves compacted into one path per job; a leaf with an empty side is filled here */
+__global__ void k_tag_gather(const TagLeaf *leaves, uint32_t n_leaves, const uint8_t *ops, uint32_t n, uint8_t *path)
+{
+  const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
+  if (x >= n) return;
+  uint32_t lo = 0, hi = n_leaves - 1;
+  while (lo < hi) {
+    const uint32_t mid = lo + ((hi - lo + 1) >> 1);
+    if (leaves[mid].dst <= x) lo = mid;
+    else hi = mid - 1;
+  }
+  const TagLeaf l = leaves[lo];
+  const uint8_t op = l.fill >= 0 ? (uint8_t)l.fill : ops[l.src + (x - l.dst)];
+  path[x] = op | (l.first && x == l.dst ? TAG_FIRST : 0);
+}
+
+/* (2) run starts: a job's first op or a change of letter */
+__global__ void k_tag_mark(const uint8_t *path, uint32_t n, int kind, uint8_t *mark)
+{
+  const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
+  if (x >= n) return;
+  const uint8_t p = path[x];
+  mark[x] = x == 0 || (p & TAG_FIRST) || tag_key(p, kind) != tag_key(path[x - 1], kind);
+}
+
+/* (3, 4) per run r < R: its text length and, for cs, the query / target bases it consumes and its job; r = R closes the
+ * scans with zeros */
+__global__ void k_tag_runs(const uint8_t *path, uint32_t n, const uint32_t *first, uint32_t R, int kind,
+                           const TagJob *jobs, uint32_t n_jobs, uint64_t *tlen, uint32_t *qc, uint32_t *tc,
+                           uint32_t *rjob)
+{
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r > R) return;
+  if (r == R) {
+    tlen[R] = 0;
+    if (kind == TAG_CS) { qc[R] = 0; tc[R] = 0; }
+    return;
+  }
+  const uint32_t f = first[r], len = (r + 1 < R ? first[r + 1] : n) - f;
+  const int op = path[f] & 3;
+  if (kind != TAG_CS) {
+    tlen[r] = tag_digits(len) + 1;
+    return;
+  }
+  tlen[r] = op == 0 ? 1 + tag_digits(len) : op == 3 ? 3ull * len : 1ull + len;
+  qc[r] = op == 2 ? 0 : len;
+  tc[r] = op == 1 ? 0 : len;
+  uint32_t lo = 0, hi = n_jobs - 1;
+  while (lo < hi) {
+    const uint32_t mid = lo + ((hi - lo + 1) >> 1);
+    if (jobs[mid].op0 <= f) lo = mid;
+    else hi = mid - 1;
+  }
+  rjob[r] = lo;
+}
+
+/* each job's text start: the offset of the run at its first op; j = n_jobs gives the wave's total */
+__global__ void k_tag_jobs(const uint32_t *first, uint32_t R, const TagJob *jobs, uint32_t n_jobs, const uint64_t *toff,
+                           uint64_t *jtext)
+{
+  const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j > n_jobs) return;
+  jtext[j] = toff[j == n_jobs ? R : tag_find(first, R, jobs[j].op0)];
+}
+
+/* (5) one byte of text per thread, its run found by binary search over the run offsets */
+__global__ void k_tag_write(const uint8_t *path, uint32_t n, const uint32_t *first, uint32_t R, const uint64_t *toff,
+                            uint64_t total, int kind, const uint32_t *qpos, const uint32_t *tpos, const uint32_t *rjob,
+                            const TagJob *jobs, const uint8_t *dq, const uint8_t *dt, char *text)
+{
+  const uint64_t b = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+  if (b >= total) return;
+  const uint32_t r = tag_find(toff, R, b);
+  const uint64_t k = b - toff[r];
+  const uint32_t f = first[r], len = (r + 1 < R ? first[r + 1] : n) - f;
+  const int op = path[f] & 3;
+  char ch;
+  if (kind != TAG_CS) {
+    const int nd = tag_digits(len);
+    ch = k < (uint64_t)nd ? tag_digit(len, nd, (int)k) : (kind == TAG_CG ? "MIDM" : "=IDX")[op];
+  } else if (op == 0) {
+    ch = k == 0 ? ':' : tag_digit(len, tag_digits(len), (int)k - 1);
+  } else {
+    const TagJob &jb = jobs[rjob[r]];
+    const uint64_t q = jb.q + (qpos[r] - jb.q0), t = jb.t + (tpos[r] - jb.t0);
+    if (op == 3) {
+      const uint64_t m = k / 3;
+      const int s = (int)(k - 3 * m);
+      ch = s == 0 ? '*' : tag_lower(s == 1 ? dt[t + m] : dq[q + m]);
+    } else {
+      ch = k == 0 ? (op == 1 ? '+' : '-') : tag_lower(op == 1 ? dq[q + k - 1] : dt[t + k - 1]);
+    }
+  }
+  text[b] = ch;
+}
+
 thread_local std::string g_create_error;
+
+struct TagBufs {  // device arrays of the formatting pass, grown as needed
+  mm_devbuf<TagLeaf> leaves;
+  mm_devbuf<TagJob> jobs;
+  mm_devbuf<uint8_t> path, mark, tmp;
+  mm_devbuf<uint32_t> first, qc, tc, qpos, tpos, rjob;
+  mm_devbuf<uint64_t> tlen, toff, jtext;
+  mm_devbuf<int64_t> n_runs;
+  mm_devbuf<char> text;
+};
 
 }  // namespace
 
@@ -562,10 +730,11 @@ struct mm_align_ctx {
   cudaStream_t st = nullptr;
   cudaEvent_t e0 = nullptr, e1 = nullptr;
   std::string err;
-  float ms[8] = {0};
+  float ms[9] = {0}; /* mm_align_last_stage_ms's 8 slots, then [8] the formatting kernels of mm_align_batch_tags */
   mm_devbuf<uint8_t> q, t, code, scratch, ops;
   mm_devbuf<Prob> probs;
   mm_devbuf<unsigned char> out_a, out_b, out_c, out_n; /* int or int4 results, by stage */
+  TagBufs tag;
 };
 
 namespace {
@@ -665,6 +834,388 @@ struct Node {
   uint64_t q, t;
 };
 
+/* Validates a batch and gives every distinct byte of it a code (equality is byte identity). */
+int check_batch(mm_align_ctx *c, const char *qbases, uint64_t n_q, const char *tbases, uint64_t n_t,
+                const mm_align_job *jobs, uint64_t n_jobs, uint8_t code[256], int &nsym)
+{
+  for (uint64_t j = 0; j < n_jobs; j++) {
+    const mm_align_job &b = jobs[j];
+    if (b.q_len < 1 || b.t_len < 1 || b.q_offset + (uint64_t)b.q_len > n_q || b.t_offset + (uint64_t)b.t_len > n_t) {
+      c->err = "job " + std::to_string(j) + ": empty or out-of-range region";
+      return MM_EINVAL;
+    }
+    if (b.mode != MM_ALIGN_HW && b.mode != MM_ALIGN_NW) {
+      c->err = "job " + std::to_string(j) + ": mode " + std::to_string(b.mode) + " is neither MM_ALIGN_HW nor MM_ALIGN_NW";
+      return MM_EINVAL;
+    }
+  }
+  nsym = 0;
+  if (n_jobs == 0) return MM_OK;
+  bool seen[256] = {false};
+  for (uint64_t i = 0; i < n_q; i++) seen[(uint8_t)qbases[i]] = true;
+  for (uint64_t i = 0; i < n_t; i++) seen[(uint8_t)tbases[i]] = true;
+  for (int x = 0; x < 256; x++) code[x] = seen[x] ? (uint8_t)nsym++ : 0;
+  if (nsym > 16) {
+    c->err = "more than 16 distinct byte values in one batch";
+    return MM_EINVAL;
+  }
+  return MM_OK;
+}
+
+/* A batch aligned up to the leaves' traceback (stages 0-4). nodes are the leaves, a job's consecutive and in path
+ * order; a leaf with both sides non-empty has its ops in c->ops at off[i] and their count in c->out_n[i]; a leaf with an
+ * empty side is all insertions or all deletions and is written by the caller. */
+struct Paths {
+  std::vector<int> ed, end, start;
+  std::vector<Node> nodes;
+  std::vector<uint64_t> off;
+  std::vector<char> failed;
+  int levels = 0;
+};
+
+void align_paths(mm_align_ctx *c, const char *qbases, uint64_t n_q, const char *tbases, uint64_t n_t,
+                 const mm_align_job *jobs, uint64_t n_jobs, const uint8_t code[256], int nsym, Paths &P)
+{
+  ck(c, cudaSetDevice(c->device), "cudaSetDevice");
+  {
+    StageTimer tm(c, 0);
+    ck(c, c->q.reserve(n_q), "query allocation");
+    ck(c, c->t.reserve(n_t), "target allocation");
+    ck(c, c->code.reserve(256), "table allocation");
+    ck(c, cudaMemcpyAsync(c->q.get(), qbases, n_q, cudaMemcpyHostToDevice, c->st), "H2D");
+    ck(c, cudaMemcpyAsync(c->t.get(), tbases, n_t, cudaMemcpyHostToDevice, c->st), "H2D");
+    ck(c, cudaMemcpyAsync(c->code.get(), code, 256, cudaMemcpyHostToDevice, c->st), "H2D");
+  }
+  const uint8_t *dq = c->q.get(), *dt = c->t.get(), *dc = c->code.get();
+  auto sweep_bytes = [nsym](const Prob &p) { return scratch_bytes(p.ql, nsym, 1, 0); };
+
+  // (a) distance and end; HW and NW jobs in launches of their own, long NW jobs banded
+  std::vector<int> &ed = P.ed, &end = P.end, &start = P.start;
+  ed.assign(n_jobs, 0); end.assign(n_jobs, 0); start.assign(n_jobs, 0);
+  std::vector<std::pair<int, int>> band_ed;  // (job, distance) of the long NW jobs
+  {
+    StageTimer tm(c, 1);
+    std::vector<Prob> hw, nw, band;
+    for (uint64_t j = 0; j < n_jobs; j++) {
+      const mm_align_job &b = jobs[j];
+      Prob p{b.q_offset, b.t_offset, b.q_len, b.t_len, b.k, (int)j, 0, 0};
+      if (b.mode == MM_ALIGN_NW && is_long(b.q_len, b.t_len)) {
+        // k schedule: the first bound leaves 32 diagonals of slack on each side of the length difference
+        const long long D = std::abs((long long)b.q_len - b.t_len);
+        const long long kmax = b.k < 0 ? std::max(b.q_len, b.t_len) : b.k;
+        if (D > kmax) band_ed.push_back({(int)j, -1});  // ed >= |Q - T|
+        else { p.k = (int)std::min(kmax, std::max(64LL, D + 64)); band.push_back(p); }
+        continue;
+      }
+      (b.mode == MM_ALIGN_NW ? nw : hw).push_back(p);
+    }
+    ck(c, c->out_a.reserve(n_jobs * 4), "output allocation");
+    ck(c, c->out_b.reserve(n_jobs * 4), "output allocation");
+    if (!hw.empty())
+      run_waves(c, hw, sweep_bytes, [&](const Prob *dp, int n, int grid, int blk) {
+        k_align_hw<<<grid, blk, 0, c->st>>>(dp, n, dq, dt, dc, nsym, c->scratch.get(), (int *)c->out_a.get(),
+                                            (int *)c->out_b.get());
+      });
+    if (!nw.empty())
+      run_waves(c, nw, sweep_bytes, [&](const Prob *dp, int n, int grid, int blk) {
+        k_align_nw<<<grid, blk, 0, c->st>>>(dp, n, dq, dt, dc, nsym, c->scratch.get(), (int *)c->out_a.get(),
+                                            (int *)c->out_b.get());
+      });
+    // Banded passes until each long job is decided. A pass's score is exact when it is <= the pass's bound and is the
+    // cost of a real path (so >= the distance) otherwise: the next bound is that score or 4x the bound, whichever is
+    // smaller, capped at the job's k (k < 0: at max(Q, T), where the band holds every row). A pass at the job's k
+    // that stays above it decides -1, as edlib does.
+    std::vector<int> v(n_jobs);
+    while (!band.empty()) {
+      ck(c, c->out_c.reserve(n_jobs * 4), "output allocation");
+      run_band(c, band, sweep_bytes, [&](const Prob *dp, int n, int threads) {
+        k_band_nw<<<n, threads, 0, c->st>>>(dp, dq, dt, dc, nsym, c->scratch.get(), (int *)c->out_c.get());
+      });
+      ck(c, cudaMemcpy(v.data(), c->out_c.get(), n_jobs * 4, cudaMemcpyDeviceToHost), "D2H");
+      std::vector<Prob> next;
+      for (Prob p : band) {
+        const mm_align_job &b = jobs[p.res];
+        const long long kmax = b.k < 0 ? std::max(b.q_len, b.t_len) : b.k, s = v[p.res];
+        if (s <= p.k) band_ed.push_back({p.res, (int)s});
+        else if (p.k >= kmax) band_ed.push_back({p.res, -1});
+        else { p.k = (int)std::min({kmax, s, 4LL * p.k}); next.push_back(p); }
+      }
+      band.swap(next);
+    }
+    ck(c, cudaMemcpyAsync(ed.data(), c->out_a.get(), n_jobs * 4, cudaMemcpyDeviceToHost, c->st), "D2H");
+    ck(c, cudaMemcpyAsync(end.data(), c->out_b.get(), n_jobs * 4, cudaMemcpyDeviceToHost, c->st), "D2H");
+  }
+  for (const auto &x : band_ed) {
+    ed[x.first] = x.second;
+    end[x.first] = x.second >= 0 ? jobs[x.first].t_len - 1 : -1;
+  }
+  // (b) start of the HW jobs; end = -1 (the whole query inserted before the target) has start 0, as every NW job has
+  {
+    StageTimer tm(c, 2);
+    std::vector<Prob> probs;
+    for (uint64_t j = 0; j < n_jobs; j++)
+      if (jobs[j].mode == MM_ALIGN_HW && ed[j] >= 0 && end[j] >= 0)
+        probs.push_back(Prob{jobs[j].q_offset, jobs[j].t_offset, jobs[j].q_len, end[j] + 1, 0, (int)j, 0, 0});
+    if (!probs.empty()) {
+      run_waves(c, probs, sweep_bytes, [&](const Prob *dp, int n, int grid, int blk) {
+        k_align_shw<<<grid, blk, 0, c->st>>>(dp, n, dq, dt, dc, nsym, c->scratch.get(), (int *)c->out_a.get());
+      });
+      std::vector<int> s(n_jobs);
+      ck(c, cudaMemcpyAsync(s.data(), c->out_a.get(), n_jobs * 4, cudaMemcpyDeviceToHost, c->st), "D2H");
+      ck(c, cudaStreamSynchronize(c->st), "D2H");
+      for (const Prob &p : probs) start[p.res] = s[p.res];
+    }
+  }
+  // (c) Hirschberg levels; the node list stays in alignment order
+  std::vector<Node> &nodes = P.nodes;
+  std::vector<char> &failed = P.failed;
+  failed.assign(n_jobs, 0);
+  for (uint64_t j = 0; j < n_jobs; j++)
+    if (ed[j] >= 0)
+      nodes.push_back(Node{(int)j, jobs[j].q_len, end[j] - start[j] + 1, ed[j], jobs[j].q_offset,
+                           jobs[j].t_offset + (uint64_t)start[j]});
+  int &levels = P.levels;
+  {
+    StageTimer tm(c, 3);
+    while (true) {
+      std::vector<Prob> probs;
+      for (size_t i = 0; i < nodes.size(); i++)
+        if (!is_leaf(nodes[i].ql, nodes[i].tl))
+          probs.push_back(Prob{nodes[i].q, nodes[i].t, nodes[i].ql, nodes[i].tl, nodes[i].score, (int)probs.size(), 0,
+                               i});
+      if (probs.empty()) break;
+      levels++;
+      ck(c, c->out_a.reserve(probs.size() * sizeof(int4)), "output allocation");
+      std::vector<Prob> shortp, longp;  // copies: probs keeps the node order for the merge below
+      for (const Prob &p : probs) (is_long(p.ql, p.tl) ? longp : shortp).push_back(p);
+      if (!shortp.empty())
+        run_waves(c, shortp, [nsym](const Prob &p) { return scratch_bytes(p.ql, nsym, 1, (uint64_t)p.ql * 8 + 16); },
+                  [&](const Prob *dp, int n, int grid, int blk) {
+                    k_align_hirsch<<<grid, blk, 0, c->st>>>(dp, n, dq, dt, dc, nsym, c->scratch.get(),
+                                                            (int4 *)c->out_a.get());
+                  });
+      if (!longp.empty())  // both halves of a node as two CTAs, then the split
+        run_band(c, longp, [nsym](const Prob &p) { return band_node_bytes(p.ql, nsym); },
+                 [&](const Prob *dp, int n, int threads) {
+                   k_band_col<<<2 * n, threads, 0, c->st>>>(dp, dq, dt, dc, nsym, c->scratch.get());
+                   k_band_split<<<(n + 3) / 4, 128, 0, c->st>>>(dp, n, nsym, c->scratch.get(),
+                                                                (int4 *)c->out_a.get());
+                 });
+      std::vector<int4> sp(probs.size());
+      ck(c, cudaMemcpy(sp.data(), c->out_a.get(), sp.size() * sizeof(int4), cudaMemcpyDeviceToHost), "D2H");
+      std::vector<Node> next;
+      next.reserve(nodes.size() + probs.size());
+      size_t pi = 0;
+      for (size_t i = 0; i < nodes.size(); i++) {
+        const Node &nd = nodes[i];
+        if (pi < probs.size() && probs[pi].out == i) {
+          const int4 r = sp[pi++];
+          if (!r.w) { failed[nd.job] = 1; continue; }
+          const int ulh = r.x + 1, lw = nd.tl / 2;
+          next.push_back(Node{nd.job, ulh, lw, r.y, nd.q, nd.t});
+          next.push_back(Node{nd.job, nd.ql - ulh, nd.tl - lw, r.z, nd.q + (uint64_t)ulh, nd.t + (uint64_t)lw});
+        } else {
+          next.push_back(nd);
+        }
+      }
+      nodes.swap(next);
+    }
+  }
+  // (d) leaves in waves under the budget; ops of leaf i at [off[i], off[i] + ql + tl)
+  std::vector<uint64_t> &off = P.off;
+  off.assign(nodes.size() + 1, 0);
+  for (size_t i = 0; i < nodes.size(); i++) off[i + 1] = off[i] + (uint64_t)nodes[i].ql + nodes[i].tl;
+  {
+    StageTimer tm(c, 4);
+    std::vector<Prob> probs;
+    for (size_t i = 0; i < nodes.size(); i++) {
+      const Node &nd = nodes[i];
+      if (failed[nd.job]) continue;
+      if (nd.ql == 0 || nd.tl == 0) continue;  // all deletions / all insertions (edlib.hxx:1136-1143), filled later
+      probs.push_back(Prob{nd.q, nd.t, nd.ql, nd.tl, nd.score, (int)i, 0, off[i]});
+    }
+    if (!probs.empty()) {
+      ck(c, c->ops.reserve(off.back()), "op buffer allocation");
+      ck(c, c->out_n.reserve(nodes.size() * 4), "output allocation");
+      run_waves(c, probs, [nsym](const Prob &p) { return scratch_bytes(p.ql, nsym, (uint64_t)p.tl, 0); },
+                [&](const Prob *dp, int n, int grid, int blk) {
+                  k_align_leaf<<<grid, blk, 0, c->st>>>(dp, n, dq, dt, dc, nsym, c->scratch.get(),
+                                                        c->ops.get(), (int *)c->out_n.get());
+                });
+    }
+  }
+}
+
+inline bool traced(const Node &nd) { return nd.ql && nd.tl; }
+
+void cub_run(mm_align_ctx *c, const std::function<cudaError_t(void *, size_t &)> &call)
+{
+  size_t bytes = 0;
+  ck(c, call(nullptr, bytes), "cub");
+  ck(c, c->tag.tmp.reserve(bytes + 16), "cub temporary allocation");
+  ck(c, call(c->tag.tmp.get(), bytes), "cub");
+}
+
+inline unsigned grid256(uint64_t n) { return (unsigned)((n + 255) / 256); }
+
+/* One formatting pass over a wave's paths (c->tag.path, n ops, nj jobs): jtext[w] = the text offset of wave job w
+ * (jtext[nj] = the pass's total). The text is written, to host[0, total), only when it fits in room bytes. */
+void format_pass(mm_align_ctx *c, uint32_t n, uint32_t nj, int kind, char *host, uint64_t room,
+                 std::vector<uint64_t> &jtext)
+{
+  TagBufs &g = c->tag;
+  int64_t R = 0;
+  {
+    StageTimer tm(c, 8);
+    k_tag_mark<<<grid256(n), 256, 0, c->st>>>(g.path.get(), n, kind, g.mark.get());
+    ck(c, cudaGetLastError(), "kernel launch");
+    const cub::CountingInputIterator<uint32_t> idx(0);
+    cub_run(c, [&](void *t, size_t &bytes) {
+      return cub::DeviceSelect::Flagged(t, bytes, idx, g.mark.get(), g.first.get(), g.n_runs.get(), (int64_t)n, c->st);
+    });
+    ck(c, cudaMemcpyAsync(&R, g.n_runs.get(), 8, cudaMemcpyDeviceToHost, c->st), "D2H");
+    ck(c, cudaStreamSynchronize(c->st), "run starts");
+    const uint32_t r = (uint32_t)R;
+    k_tag_runs<<<grid256(r + 1ull), 256, 0, c->st>>>(g.path.get(), n, g.first.get(), r, kind, g.jobs.get(), nj,
+                                                    g.tlen.get(), g.qc.get(), g.tc.get(), g.rjob.get());
+    ck(c, cudaGetLastError(), "kernel launch");
+    cub_run(c, [&](void *t, size_t &bytes) {
+      return cub::DeviceScan::ExclusiveSum(t, bytes, g.tlen.get(), g.toff.get(), (int64_t)r + 1, c->st);
+    });
+    if (kind == TAG_CS) {
+      cub_run(c, [&](void *t, size_t &bytes) {
+        return cub::DeviceScan::ExclusiveSum(t, bytes, g.qc.get(), g.qpos.get(), (int64_t)r + 1, c->st);
+      });
+      cub_run(c, [&](void *t, size_t &bytes) {
+        return cub::DeviceScan::ExclusiveSum(t, bytes, g.tc.get(), g.tpos.get(), (int64_t)r + 1, c->st);
+      });
+    }
+    k_tag_jobs<<<grid256(nj + 1ull), 256, 0, c->st>>>(g.first.get(), r, g.jobs.get(), nj, g.toff.get(), g.jtext.get());
+    ck(c, cudaGetLastError(), "kernel launch");
+    jtext.resize(nj + 1);
+    ck(c, cudaMemcpyAsync(jtext.data(), g.jtext.get(), (nj + 1) * 8, cudaMemcpyDeviceToHost, c->st), "D2H");
+    ck(c, cudaStreamSynchronize(c->st), "run text offsets");
+    if (jtext[nj] > room) return;
+    const uint64_t total = jtext[nj];
+    ck(c, g.text.reserve(total), "text allocation");
+    k_tag_write<<<grid256(total), 256, 0, c->st>>>(g.path.get(), n, g.first.get(), r, g.toff.get(), total, kind,
+                                                  g.qpos.get(), g.tpos.get(), g.rjob.get(), g.jobs.get(), c->q.get(),
+                                                  c->t.get(), g.text.get());
+    ck(c, cudaGetLastError(), "kernel launch");
+  }
+  StageTimer tm(c, 5);
+  ck(c, cudaMemcpyAsync(host, g.text.get(), jtext[nj], cudaMemcpyDeviceToHost, c->st), "D2H");
+}
+
+/* mm_align_batch_tags after align_paths: the traced leaves' lengths come back, then the paths are formatted in waves of
+ * whole jobs of at most `cap` ops (a longer job is a wave of its own), which bounds the pass's device arrays. */
+uint64_t format_tags(mm_align_ctx *c, const mm_align_job *jobs, uint64_t n_jobs, uint32_t flags, const Paths &P,
+                     mm_align_tag_result *results, char *text, uint64_t text_cap)
+{
+  const std::vector<Node> &nodes = P.nodes;
+  std::vector<int> dn(nodes.size(), 0);
+  bool any = false;
+  for (const Node &nd : nodes) any |= !P.failed[nd.job] && traced(nd);
+  if (any) {
+    StageTimer tm(c, 5);
+    ck(c, cudaMemcpyAsync(dn.data(), c->out_n.get(), nodes.size() * 4, cudaMemcpyDeviceToHost, c->st), "D2H");
+  }
+  std::vector<uint64_t> len(n_jobs, 0);
+  for (size_t i = 0; i < nodes.size(); i++)
+    if (!P.failed[nodes[i].job]) len[nodes[i].job] += traced(nodes[i]) ? dn[i] : nodes[i].ql + nodes[i].tl;
+  for (uint64_t j = 0; j < n_jobs; j++)
+    results[j] = mm_align_tag_result{P.ed[j], P.failed[j] ? 0 : (int32_t)len[j], 0, 0, 0, 0};
+
+  // about 48 bytes of device arrays per op: a wave takes about a quarter of the scratch budget
+  const uint64_t cap = std::min<uint64_t>(std::max<uint64_t>(c->budget / (4 * 48), 1u << 20), 1u << 30);
+  struct Wave {
+    std::vector<TagJob> jobs;
+    std::vector<TagLeaf> leaves;
+    std::vector<uint64_t> ids;
+    uint64_t n = 0;
+  };
+  std::vector<Wave> waves;
+  uint64_t max_n = 0, max_leaves = 0, max_jobs = 0;
+  size_t ni = 0;
+  for (uint64_t j = 0; j < n_jobs; j++) {
+    if (P.failed[j] || len[j] == 0) continue;
+    if (waves.empty() || waves.back().n + len[j] > cap) waves.emplace_back();
+    Wave &w = waves.back();
+    uint64_t q0 = 0, t0 = 0;
+    if (!w.ids.empty()) {
+      const mm_align_job &prev = jobs[w.ids.back()];
+      q0 = w.jobs.back().q0 + prev.q_len;
+      t0 = w.jobs.back().t0 + prev.t_len;
+    }
+    w.jobs.push_back(TagJob{jobs[j].q_offset, jobs[j].t_offset, (uint32_t)w.n, (uint32_t)q0, (uint32_t)t0});
+    w.ids.push_back(j);
+    while (nodes[ni].job < (int)j) ni++;
+    for (bool first = true; ni < nodes.size() && nodes[ni].job == (int)j; ni++, first = false) {
+      const Node &nd = nodes[ni];
+      w.leaves.push_back(TagLeaf{P.off[ni], (uint32_t)w.n, (int16_t)(traced(nd) ? -1 : nd.ql == 0 ? 2 : 1), first});
+      w.n += traced(nd) ? dn[ni] : nd.ql + nd.tl;
+    }
+    max_n = std::max(max_n, w.n);
+    max_leaves = std::max<uint64_t>(max_leaves, w.leaves.size());
+    max_jobs = std::max<uint64_t>(max_jobs, w.jobs.size());
+  }
+  if (waves.empty()) return 0;
+
+  // Everything is sized for the largest wave before the first launch: an array that grows frees its old one, and
+  // cudaFree waits for the whole device, including the mapping kernels that run beside the aligner.
+  const int kinds[2] = {flags & MM_ALIGN_TAG_EQX ? TAG_CG_EQX : TAG_CG, TAG_CS};
+  const int passes = flags & MM_ALIGN_TAG_CS ? 2 : 1;
+  TagBufs &g = c->tag;
+  ck(c, g.leaves.reserve(max_leaves), "leaf table allocation");
+  ck(c, g.jobs.reserve(max_jobs), "job table allocation");
+  ck(c, g.jtext.reserve(max_jobs + 1), "job text allocation");
+  ck(c, g.path.reserve(max_n), "path allocation");
+  ck(c, g.mark.reserve(max_n), "run allocation");
+  ck(c, g.first.reserve(max_n), "run allocation");
+  ck(c, g.tlen.reserve(max_n + 1), "run allocation");
+  ck(c, g.toff.reserve(max_n + 1), "run allocation");
+  ck(c, g.n_runs.reserve(1), "run allocation");
+  ck(c, g.text.reserve(max_n * (passes == 2 ? 3 : 2)), "text allocation");  // 2 bytes of cg, 3 of cs per op at most
+  if (passes == 2)
+    for (mm_devbuf<uint32_t> *b : {&g.qc, &g.tc, &g.qpos, &g.tpos, &g.rjob})
+      ck(c, b->reserve(max_n + 1), "run allocation");
+  {
+    size_t b0 = 0, b1 = 0, b2 = 0;
+    const cub::CountingInputIterator<uint32_t> idx(0);
+    ck(c, cub::DeviceSelect::Flagged(nullptr, b0, idx, g.mark.get(), g.first.get(), g.n_runs.get(), (int64_t)max_n,
+                                     c->st), "cub");
+    ck(c, cub::DeviceScan::ExclusiveSum(nullptr, b1, g.tlen.get(), g.toff.get(), (int64_t)max_n + 1, c->st), "cub");
+    ck(c, cub::DeviceScan::ExclusiveSum(nullptr, b2, g.qc.get(), g.qpos.get(), (int64_t)max_n + 1, c->st), "cub");
+    ck(c, g.tmp.reserve(std::max({b0, b1, b2}) + 16), "cub temporary allocation");
+  }
+  uint64_t pos = 0;
+  for (const Wave &w : waves) {
+    const uint32_t nj = (uint32_t)w.jobs.size();
+    ck(c, cudaMemcpyAsync(g.leaves.get(), w.leaves.data(), w.leaves.size() * sizeof(TagLeaf), cudaMemcpyHostToDevice,
+                          c->st), "H2D");
+    ck(c, cudaMemcpyAsync(g.jobs.get(), w.jobs.data(), nj * sizeof(TagJob), cudaMemcpyHostToDevice, c->st), "H2D");
+    {
+      StageTimer tm(c, 8);
+      k_tag_gather<<<grid256(w.n), 256, 0, c->st>>>(g.leaves.get(), (uint32_t)w.leaves.size(), c->ops.get(),
+                                                    (uint32_t)w.n, g.path.get());
+      ck(c, cudaGetLastError(), "kernel launch");
+    }
+    for (int k = 0; k < passes; k++) {
+      std::vector<uint64_t> jt;
+      // past the caller's buffer only the size is still needed
+      format_pass(c, (uint32_t)w.n, nj, kinds[k], text + std::min(pos, text_cap), pos <= text_cap ? text_cap - pos : 0,
+                  jt);
+      for (uint32_t x = 0; x < nj; x++) {
+        mm_align_tag_result &r = results[w.ids[x]];
+        (k == 0 ? r.cg_offset : r.cs_offset) = pos + jt[x];
+        (k == 0 ? r.cg_len : r.cs_len) = jt[x + 1] - jt[x];
+      }
+      pos += jt[nj];
+    }
+  }
+  return pos;
+}
+
 }  // namespace
 
 extern "C" {
@@ -717,7 +1268,7 @@ const char *mm_align_last_error(const mm_align_ctx *ctx) { return ctx ? ctx->err
 int mm_align_last_stage_ms(const mm_align_ctx *ctx, float ms[8])
 {
   if (!ctx || !ms) return MM_EINVAL;
-  std::memcpy(ms, ctx->ms, sizeof(ctx->ms));
+  std::memcpy(ms, ctx->ms, 8 * sizeof(float));
   return MM_OK;
 }
 
@@ -729,200 +1280,24 @@ int mm_align_batch(mm_align_ctx *c, const char *qbases, uint64_t n_q, const char
   const auto h0 = std::chrono::steady_clock::now();
   std::fill(c->ms, c->ms + 8, 0.f);
   *n_ops = 0;
-  for (uint64_t j = 0; j < n_jobs; j++) {
-    const mm_align_job &b = jobs[j];
-    if (b.q_len < 1 || b.t_len < 1 || b.q_offset + (uint64_t)b.q_len > n_q || b.t_offset + (uint64_t)b.t_len > n_t) {
-      c->err = "job " + std::to_string(j) + ": empty or out-of-range region";
-      return MM_EINVAL;
-    }
-    if (b.mode != MM_ALIGN_HW && b.mode != MM_ALIGN_NW) {
-      c->err = "job " + std::to_string(j) + ": mode " + std::to_string(b.mode) + " is neither MM_ALIGN_HW nor MM_ALIGN_NW";
-      return MM_EINVAL;
-    }
-  }
-  if (n_jobs == 0) return MM_OK;
-  // symbols: every distinct byte of the batch gets a code (equality is byte identity)
   uint8_t code[256];
-  bool seen[256] = {false};
-  for (uint64_t i = 0; i < n_q; i++) seen[(uint8_t)qbases[i]] = true;
-  for (uint64_t i = 0; i < n_t; i++) seen[(uint8_t)tbases[i]] = true;
   int nsym = 0;
-  for (int x = 0; x < 256; x++) code[x] = seen[x] ? (uint8_t)nsym++ : 0;
-  if (nsym > 16) {
-    c->err = "more than 16 distinct byte values in one batch";
-    return MM_EINVAL;
-  }
+  if (const int rc = check_batch(c, qbases, n_q, tbases, n_t, jobs, n_jobs, code, nsym)) return rc;
+  if (n_jobs == 0) return MM_OK;
   try {
-    ck(c, cudaSetDevice(c->device), "cudaSetDevice");
-    {
-      StageTimer tm(c, 0);
-      ck(c, c->q.reserve(n_q), "query allocation");
-      ck(c, c->t.reserve(n_t), "target allocation");
-      ck(c, c->code.reserve(256), "table allocation");
-      ck(c, cudaMemcpyAsync(c->q.get(), qbases, n_q, cudaMemcpyHostToDevice, c->st), "H2D");
-      ck(c, cudaMemcpyAsync(c->t.get(), tbases, n_t, cudaMemcpyHostToDevice, c->st), "H2D");
-      ck(c, cudaMemcpyAsync(c->code.get(), code, 256, cudaMemcpyHostToDevice, c->st), "H2D");
-    }
-    const uint8_t *dq = c->q.get(), *dt = c->t.get(), *dc = c->code.get();
-    auto sweep_bytes = [nsym](const Prob &p) { return scratch_bytes(p.ql, nsym, 1, 0); };
-
-    // (a) distance and end; HW and NW jobs in launches of their own, long NW jobs banded
-    std::vector<int> ed(n_jobs), end(n_jobs), start(n_jobs, 0);
-    std::vector<std::pair<int, int>> band_ed;  // (job, distance) of the long NW jobs
-    {
-      StageTimer tm(c, 1);
-      std::vector<Prob> hw, nw, band;
-      for (uint64_t j = 0; j < n_jobs; j++) {
-        const mm_align_job &b = jobs[j];
-        Prob p{b.q_offset, b.t_offset, b.q_len, b.t_len, b.k, (int)j, 0, 0};
-        if (b.mode == MM_ALIGN_NW && is_long(b.q_len, b.t_len)) {
-          // k schedule: the first bound leaves 32 diagonals of slack on each side of the length difference
-          const long long D = std::abs((long long)b.q_len - b.t_len);
-          const long long kmax = b.k < 0 ? std::max(b.q_len, b.t_len) : b.k;
-          if (D > kmax) band_ed.push_back({(int)j, -1});  // ed >= |Q - T|
-          else { p.k = (int)std::min(kmax, std::max(64LL, D + 64)); band.push_back(p); }
-          continue;
-        }
-        (b.mode == MM_ALIGN_NW ? nw : hw).push_back(p);
-      }
-      ck(c, c->out_a.reserve(n_jobs * 4), "output allocation");
-      ck(c, c->out_b.reserve(n_jobs * 4), "output allocation");
-      if (!hw.empty())
-        run_waves(c, hw, sweep_bytes, [&](const Prob *dp, int n, int grid, int blk) {
-          k_align_hw<<<grid, blk, 0, c->st>>>(dp, n, dq, dt, dc, nsym, c->scratch.get(), (int *)c->out_a.get(),
-                                              (int *)c->out_b.get());
-        });
-      if (!nw.empty())
-        run_waves(c, nw, sweep_bytes, [&](const Prob *dp, int n, int grid, int blk) {
-          k_align_nw<<<grid, blk, 0, c->st>>>(dp, n, dq, dt, dc, nsym, c->scratch.get(), (int *)c->out_a.get(),
-                                              (int *)c->out_b.get());
-        });
-      // Banded passes until each long job is decided. A pass's score is exact when it is <= the pass's bound and is the
-      // cost of a real path (so >= the distance) otherwise: the next bound is that score or 4x the bound, whichever is
-      // smaller, capped at the job's k (k < 0: at max(Q, T), where the band holds every row). A pass at the job's k
-      // that stays above it decides -1, as edlib does.
-      std::vector<int> v(n_jobs);
-      while (!band.empty()) {
-        ck(c, c->out_c.reserve(n_jobs * 4), "output allocation");
-        run_band(c, band, sweep_bytes, [&](const Prob *dp, int n, int threads) {
-          k_band_nw<<<n, threads, 0, c->st>>>(dp, dq, dt, dc, nsym, c->scratch.get(), (int *)c->out_c.get());
-        });
-        ck(c, cudaMemcpy(v.data(), c->out_c.get(), n_jobs * 4, cudaMemcpyDeviceToHost), "D2H");
-        std::vector<Prob> next;
-        for (Prob p : band) {
-          const mm_align_job &b = jobs[p.res];
-          const long long kmax = b.k < 0 ? std::max(b.q_len, b.t_len) : b.k, s = v[p.res];
-          if (s <= p.k) band_ed.push_back({p.res, (int)s});
-          else if (p.k >= kmax) band_ed.push_back({p.res, -1});
-          else { p.k = (int)std::min({kmax, s, 4LL * p.k}); next.push_back(p); }
-        }
-        band.swap(next);
-      }
-      ck(c, cudaMemcpyAsync(ed.data(), c->out_a.get(), n_jobs * 4, cudaMemcpyDeviceToHost, c->st), "D2H");
-      ck(c, cudaMemcpyAsync(end.data(), c->out_b.get(), n_jobs * 4, cudaMemcpyDeviceToHost, c->st), "D2H");
-    }
-    for (const auto &x : band_ed) {
-      ed[x.first] = x.second;
-      end[x.first] = x.second >= 0 ? jobs[x.first].t_len - 1 : -1;
-    }
-    // (b) start of the HW jobs; end = -1 (the whole query inserted before the target) has start 0, as every NW job has
-    {
-      StageTimer tm(c, 2);
-      std::vector<Prob> probs;
-      for (uint64_t j = 0; j < n_jobs; j++)
-        if (jobs[j].mode == MM_ALIGN_HW && ed[j] >= 0 && end[j] >= 0)
-          probs.push_back(Prob{jobs[j].q_offset, jobs[j].t_offset, jobs[j].q_len, end[j] + 1, 0, (int)j, 0, 0});
-      if (!probs.empty()) {
-        run_waves(c, probs, sweep_bytes, [&](const Prob *dp, int n, int grid, int blk) {
-          k_align_shw<<<grid, blk, 0, c->st>>>(dp, n, dq, dt, dc, nsym, c->scratch.get(), (int *)c->out_a.get());
-        });
-        std::vector<int> s(n_jobs);
-        ck(c, cudaMemcpyAsync(s.data(), c->out_a.get(), n_jobs * 4, cudaMemcpyDeviceToHost, c->st), "D2H");
-        ck(c, cudaStreamSynchronize(c->st), "D2H");
-        for (const Prob &p : probs) start[p.res] = s[p.res];
-      }
-    }
-    // (c) Hirschberg levels; the node list stays in alignment order
-    std::vector<Node> nodes;
-    std::vector<char> failed(n_jobs, 0);
-    for (uint64_t j = 0; j < n_jobs; j++)
-      if (ed[j] >= 0)
-        nodes.push_back(Node{(int)j, jobs[j].q_len, end[j] - start[j] + 1, ed[j], jobs[j].q_offset,
-                             jobs[j].t_offset + (uint64_t)start[j]});
-    int levels = 0;
-    {
-      StageTimer tm(c, 3);
-      while (true) {
-        std::vector<Prob> probs;
-        for (size_t i = 0; i < nodes.size(); i++)
-          if (!is_leaf(nodes[i].ql, nodes[i].tl))
-            probs.push_back(Prob{nodes[i].q, nodes[i].t, nodes[i].ql, nodes[i].tl, nodes[i].score, (int)probs.size(), 0,
-                                 i});
-        if (probs.empty()) break;
-        levels++;
-        ck(c, c->out_a.reserve(probs.size() * sizeof(int4)), "output allocation");
-        std::vector<Prob> shortp, longp;  // copies: probs keeps the node order for the merge below
-        for (const Prob &p : probs) (is_long(p.ql, p.tl) ? longp : shortp).push_back(p);
-        if (!shortp.empty())
-          run_waves(c, shortp, [nsym](const Prob &p) { return scratch_bytes(p.ql, nsym, 1, (uint64_t)p.ql * 8 + 16); },
-                    [&](const Prob *dp, int n, int grid, int blk) {
-                      k_align_hirsch<<<grid, blk, 0, c->st>>>(dp, n, dq, dt, dc, nsym, c->scratch.get(),
-                                                              (int4 *)c->out_a.get());
-                    });
-        if (!longp.empty())  // both halves of a node as two CTAs, then the split
-          run_band(c, longp, [nsym](const Prob &p) { return band_node_bytes(p.ql, nsym); },
-                   [&](const Prob *dp, int n, int threads) {
-                     k_band_col<<<2 * n, threads, 0, c->st>>>(dp, dq, dt, dc, nsym, c->scratch.get());
-                     k_band_split<<<(n + 3) / 4, 128, 0, c->st>>>(dp, n, nsym, c->scratch.get(),
-                                                                  (int4 *)c->out_a.get());
-                   });
-        std::vector<int4> sp(probs.size());
-        ck(c, cudaMemcpy(sp.data(), c->out_a.get(), sp.size() * sizeof(int4), cudaMemcpyDeviceToHost), "D2H");
-        std::vector<Node> next;
-        next.reserve(nodes.size() + probs.size());
-        size_t pi = 0;
-        for (size_t i = 0; i < nodes.size(); i++) {
-          const Node &nd = nodes[i];
-          if (pi < probs.size() && probs[pi].out == i) {
-            const int4 r = sp[pi++];
-            if (!r.w) { failed[nd.job] = 1; continue; }
-            const int ulh = r.x + 1, lw = nd.tl / 2;
-            next.push_back(Node{nd.job, ulh, lw, r.y, nd.q, nd.t});
-            next.push_back(Node{nd.job, nd.ql - ulh, nd.tl - lw, r.z, nd.q + (uint64_t)ulh, nd.t + (uint64_t)lw});
-          } else {
-            next.push_back(nd);
-          }
-        }
-        nodes.swap(next);
-      }
-    }
-    // (d) leaves in waves under the budget; ops of leaf i at [off[i], off[i] + ql + tl)
-    std::vector<uint64_t> off(nodes.size() + 1, 0);
-    for (size_t i = 0; i < nodes.size(); i++) off[i + 1] = off[i] + (uint64_t)nodes[i].ql + nodes[i].tl;
+    Paths P;
+    align_paths(c, qbases, n_q, tbases, n_t, jobs, n_jobs, code, nsym, P);
+    const std::vector<Node> &nodes = P.nodes;
+    const std::vector<uint64_t> &off = P.off;
+    const std::vector<char> &failed = P.failed;
+    const std::vector<int> &ed = P.ed, &start = P.start, &end = P.end;
     std::vector<uint8_t> leaf_ops(off.back());
     std::vector<int> leaf_n(nodes.size(), 0);
-    {
-      StageTimer tm(c, 4);
-      std::vector<Prob> probs;
-      for (size_t i = 0; i < nodes.size(); i++) {
-        const Node &nd = nodes[i];
-        if (failed[nd.job]) continue;
-        if (nd.ql == 0 || nd.tl == 0) {  // all deletions / all insertions (edlib.hxx:1136-1143)
-          std::fill(leaf_ops.begin() + off[i], leaf_ops.begin() + off[i] + nd.ql + nd.tl, nd.ql == 0 ? 2 : 1);
-          leaf_n[i] = nd.ql + nd.tl;
-          continue;
-        }
-        probs.push_back(Prob{nd.q, nd.t, nd.ql, nd.tl, nd.score, (int)i, 0, off[i]});
-      }
-      if (!probs.empty()) {
-        ck(c, c->ops.reserve(off.back()), "op buffer allocation");
-        ck(c, c->out_n.reserve(nodes.size() * 4), "output allocation");
-        run_waves(c, probs, [nsym](const Prob &p) { return scratch_bytes(p.ql, nsym, (uint64_t)p.tl, 0); },
-                  [&](const Prob *dp, int n, int grid, int blk) {
-                    k_align_leaf<<<grid, blk, 0, c->st>>>(dp, n, dq, dt, dc, nsym, c->scratch.get(),
-                                                          c->ops.get(), (int *)c->out_n.get());
-                  });
-      }
+    for (size_t i = 0; i < nodes.size(); i++) {
+      const Node &nd = nodes[i];
+      if (failed[nd.job] || traced(nd)) continue;
+      std::fill(leaf_ops.begin() + off[i], leaf_ops.begin() + off[i] + nd.ql + nd.tl, nd.ql == 0 ? 2 : 1);
+      leaf_n[i] = nd.ql + nd.tl;
     }
     {
       StageTimer tm(c, 5);
@@ -967,11 +1342,55 @@ int mm_align_batch(mm_align_ctx *c, const char *qbases, uint64_t n_q, const char
       r.ops_offset += leaf_n[i];
     }
     for (uint64_t j = 0; j < n_jobs; j++) results[j].ops_offset -= failed[j] ? 0 : len[j];
-    c->ms[7] = (float)levels;
+    c->ms[7] = (float)P.levels;
   } catch (const Failure &f) {
     return f.code;
   }
   c->ms[6] = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - h0).count();
+  return MM_OK;
+}
+
+int mm_align_batch_tags(mm_align_ctx *c, const char *qbases, uint64_t n_q, const char *tbases, uint64_t n_t,
+                        const mm_align_job *jobs, uint64_t n_jobs, uint32_t flags, mm_align_tag_result *results,
+                        char *text, uint64_t text_cap, uint64_t *n_text)
+{
+  if (!c || (n_jobs && (!jobs || !results || !n_text)) || (text_cap && !text)) return MM_EINVAL;
+  const auto h0 = std::chrono::steady_clock::now();
+  std::fill(c->ms, c->ms + 9, 0.f);
+  if (n_text) *n_text = 0;
+  if (flags & ~(uint32_t)(MM_ALIGN_TAG_EQX | MM_ALIGN_TAG_CS)) {
+    c->err = "flags " + std::to_string(flags) + " hold bits other than MM_ALIGN_TAG_EQX and MM_ALIGN_TAG_CS";
+    return MM_EINVAL;
+  }
+  uint8_t code[256];
+  int nsym = 0;
+  if (const int rc = check_batch(c, qbases, n_q, tbases, n_t, jobs, n_jobs, code, nsym)) return rc;
+  for (uint64_t j = 0; j < n_jobs; j++)
+    if (jobs[j].mode != MM_ALIGN_NW) {
+      c->err = "job " + std::to_string(j) + ": mm_align_batch_tags takes MM_ALIGN_NW jobs only";
+      return MM_EINVAL;
+    }
+  if (n_jobs == 0) return MM_OK;
+  try {
+    Paths P;
+    align_paths(c, qbases, n_q, tbases, n_t, jobs, n_jobs, code, nsym, P);
+    *n_text = format_tags(c, jobs, n_jobs, flags, P, results, text, text_cap);
+    c->ms[7] = (float)P.levels;
+    if (*n_text > text_cap) {
+      c->err = "text buffer too small";
+      return MM_ECAPACITY;
+    }
+  } catch (const Failure &f) {
+    return f.code;
+  }
+  c->ms[6] = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - h0).count();
+  return MM_OK;
+}
+
+int mm_align_last_tag_ms(const mm_align_ctx *ctx, float *ms)
+{
+  if (!ctx || !ms) return MM_EINVAL;
+  *ms = ctx->ms[8];
   return MM_OK;
 }
 
